@@ -1,18 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 rasterizer (BASELINE.json: Mpix/s fwd+bwd @ 1M splats, 1600x1200).
+"""bench.py -- headline benchmark of the H100 rasterizer (BASELINE.json: Mpix/s fwd+bwd @ 1M splats, 1600x1200).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step is one pass of the hot path over one synthetic camera: `_C.rasterize_gaussians` followed by
 `_C.rasterize_gaussians_backward` with fixed upstream gradients (SURVEY.md 8d).  Prints ONE JSON line (rank 0).
 
-Protocol (SURVEY.md 8d: median of >= 20 timed iterations after >= 5 warm-ups):
-  * a *window* is EXACTLY `--steps` iterations bracketed by barrier + torch.cuda.synchronize() on both sides, with a CUDA
-    event between consecutive iterations (on the launching stream); per iteration the time is the MAX over ranks;
-  * windows are repeated until at least `--min-time` seconds (default 0.5) and at least 20 iterations have been timed;
-  * `ms_per_step` = MEDIAN of all per-iteration times, `value` = W*H / that; min / median / max and the per-window means
-    are in `timing` so a perturbed window is visible instead of being averaged in;
+Protocol (SURVEY.md 8d: median of >= 20 timed iterations after >= 5 warm-ups, so use --steps >= 20):
+  * each measured quantity is timed over EXACTLY `--steps` iterations bracketed by barrier + torch.cuda.synchronize() on both
+    sides, with a CUDA event between consecutive iterations (on the launching stream); per iteration the time is the MAX over ranks;
+  * `ms_per_step` = MEDIAN of the per-iteration times, `value` = W*H / that; min / median / max are in `timing`;
   * SM clocks / throttle reasons are sampled by a separate PROCESS (NVML, no GIL contention with the timed loop) that
     runs during every timed phase of the run.
   value        inputs resident in HBM
@@ -20,16 +18,18 @@ Protocol (SURVEY.md 8d: median of >= 20 timed iterations after >= 5 warm-ups):
                step's host inputs -- camera matrices and the 8-bit ground-truth image -- copied from pinned host
                memory inside the timed region and the loss read back to the host every step; same protocol
   roofline     dominant kernel (backward render): algorithmic bytes (SURVEY.md 8d) / its average launch duration,
-               measured live with CUDA events the library records on the launching stream; `traffic` and the
-               instruction count behind `roofline_issue` are REPLAYED from the committed ncu capture (labelled so)
+               measured live with CUDA events the library records on the launching stream
   cpu_baseline the CPU oracle port (oracle/oracle.c, 1 thread) on a bounded sample of the same workload, plus the
                pure-torch config[0] plumbing timing -- reported, not a target
-`--impl reference` times the reference's own CUDA rasterizer (oracle/_ref/ref_dgr_C.so, built from /root/reference
+`--impl reference` times the reference's own CUDA rasterizer (oracle/_ref/ref_dgr_C.so, built from a reference checkout
 by oracle/build_ref.py) on the same config through the same harness: the reference has NO CPU implementation of
 this path (BASELINE.md section 2), so its arm runs where it can -- on the GPU (see DESIGN.md "Measurement").  That arm
 never imports the product's extension modules.
 N > 1: tile rows of the one image are sharded over the ranks (strong scaling); the screen-space gradient rows are
 exchanged once per backward.
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step returned to its caller as DIR/<name>.npy
+(float32; images at a fixed seeded sample of pixels, gradients at a fixed seeded sample of Gaussians, 64 MB at most), so that
+two builds can be compared output for output on the same inputs.
 """
 from __future__ import annotations
 
@@ -52,7 +52,7 @@ import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
 METRIC = "Mpix/s fwd+bwd @1M splats 1600x1200"
-SM_COUNT = 148
+DUMP_PIXELS, DUMP_ROWS = 1 << 18, 1 << 16    # 15 image planes x 1 MB + 71 gradient floats x 256 KB: about 34 MB
 
 
 # ---- clocks ----------------------------------------------------------------------------------------------------
@@ -78,8 +78,7 @@ with open(path, "w", buffering=1) as f:
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed regions by a separate process (B200_PROFILING.md 'clocks'
-    line): NVML every 10 ms in a helper python process; `nvidia-smi -lms` as the fallback.  Nothing of it runs in this
+    """SM clock / throttle reasons sampled DURING the timed regions by a separate process: NVML every 10 ms in a helper python process; `nvidia-smi -lms` as the fallback.  Nothing of it runs in this
     process, so the timed loop does not share the GIL with it."""
     REASON_BITS = (("sw_power_cap", 0x4), ("hw_slowdown", 0x8), ("sw_thermal_slowdown", 0x20), ("hw_thermal_slowdown", 0x40))
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
@@ -221,6 +220,49 @@ def cpu_baseline():
     return res
 
 
+def device_info(dev, nvml_index):
+    """Name, SM count and power limit of the card the numbers were measured on (read-only queries)."""
+    info = {"name": torch.cuda.get_device_name(dev), "sm_count": torch.cuda.get_device_properties(dev).multi_processor_count, "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={nvml_index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"], capture_output=True,
+                             text=True, timeout=30).stdout.strip()
+        info["power_limit_w"] = float(out.splitlines()[0])
+    except Exception:
+        pass
+    return info
+
+
+def dump_outputs(out_dir, last, H, W, P):
+    """What one timed step returned to its caller, as float32 .npy files: the forward maps at DUMP_PIXELS seeded pixel positions,
+    the radii and the eight gradient tensors at DUMP_ROWS seeded Gaussians (the same positions in every run with the same
+    arguments), num_rendered, and the positions themselves.  Multi-GPU: rank 0's replicated gradients only."""
+    import numpy as np
+    from rade_gs_b200 import rawapi
+    os.makedirs(out_dir, exist_ok=True)
+    fwd, bwd = last
+    if not isinstance(bwd, dict):
+        bwd = dict(zip(rawapi.BWD_KEYS, bwd))
+    pix = np.sort(np.random.default_rng(0).choice(H * W, size=min(DUMP_PIXELS, H * W), replace=False))
+    rows = np.sort(np.random.default_rng(1).choice(P, size=min(DUMP_ROWS, P), replace=False))
+    arrays = {"num_rendered": np.array([int(fwd["num_rendered"])], np.float64), "pixel_index": pix.astype(np.float64),
+              "gaussian_index": rows.astype(np.float64)}
+    pix_t, rows_t = torch.from_numpy(pix), torch.from_numpy(rows)
+    for k in ("color", "coord", "mcoord", "alpha", "normal", "depth", "mdepth"):
+        if k in fwd:
+            m = fwd[k]
+            arrays[k] = m.reshape(m.shape[0], -1)[:, pix_t.to(m.device)].float().cpu().numpy()
+    if "radii" in fwd:
+        arrays["radii"] = fwd["radii"][rows_t.to(fwd["radii"].device)].float().cpu().numpy()
+    for k in rawapi.BWD_KEYS:
+        g = bwd[k]
+        arrays["grad_" + k] = g[rows_t.to(g.device)].float().cpu().numpy() if g.numel() else np.zeros((0,), np.float32)
+    total = sum(v.nbytes for v in arrays.values())
+    assert total <= 64 << 20, total
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
+    return {"dir": out_dir, "files": len(arrays), "bytes": total}
+
+
 # SURVEY.md 8d per-variant constants: (A_v gather bytes per instance, O_v fwd bytes per pixel, I_v bwd bytes per pixel, G_v grad floats per Gaussian)
 VARIANT_BYTES = {(False, False): (36, 24, 28, 10), (False, True): (60, 52, 68, 16), (True, False): (84, 76, 92, 22), (True, True): (96, 88, 104, 25)}
 
@@ -246,8 +288,9 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="C2")
-    ap.add_argument("--min-time", type=float, default=0.5, help="seconds of timed work per measured quantity (windows of --steps are repeated)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs (sampled) as DIR/<name>.npy; with --gpus N > 1 only rank 0's "
+                    "gradients (the maps stay per-rank slabs)")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3)
     a.steps = max(a.steps, 1)
@@ -309,31 +352,24 @@ def main():
         torch.cuda.synchronize()
 
     def measure(fn):
-        """Windows of exactly --steps iterations (barrier + synchronize on both sides, CUDA events between iterations on the
-        launching stream, max over ranks per iteration) until --min-time seconds and >= 20 iterations are on record."""
-        iters, windows, last, total = [], [], None, 0.0
+        """Exactly --steps iterations (barrier + synchronize on both sides, CUDA events between iterations on the launching
+        stream, max over ranks per iteration)."""
+        last = None
         fn()                      # one more untimed step: the first call after a phase change pays one-off allocator / event set-up
         torch.cuda.synchronize()
-        while True:
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(a.steps + 1)]
-            barrier()
-            ev[0].record()
-            for i in range(a.steps):
-                last = fn()
-                ev[i + 1].record()
-            barrier()
-            t = torch.tensor([ev[i].elapsed_time(ev[i + 1]) for i in range(a.steps)] + [ev[0].elapsed_time(ev[a.steps])], device=dev, dtype=torch.float64)
-            if multi:
-                dist.all_reduce(t, op=dist.ReduceOp.MAX)
-            t = t.tolist()
-            iters += t[:-1]
-            windows.append(t[-1] / a.steps)
-            total += t[-1] * 1e-3
-            if (total >= a.min_time and len(iters) >= 20) or len(windows) >= 200:
-                break
-        med = statistics.median(iters)
-        return {"ms": med, "min_ms": min(iters), "max_ms": max(iters), "iterations": len(iters), "windows": len(windows),
-                "window_mean_ms": {"min": min(windows), "median": statistics.median(windows), "max": max(windows)}, "timed_s": total}, last
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(a.steps + 1)]
+        barrier()
+        ev[0].record()
+        for i in range(a.steps):
+            last = fn()
+            ev[i + 1].record()
+        barrier()
+        t = torch.tensor([ev[i].elapsed_time(ev[i + 1]) for i in range(a.steps)] + [ev[0].elapsed_time(ev[a.steps])], device=dev, dtype=torch.float64)
+        if multi:
+            dist.all_reduce(t, op=dist.ReduceOp.MAX)
+        t = t.tolist()
+        iters = t[:-1]
+        return {"ms": statistics.median(iters), "min_ms": min(iters), "max_ms": max(iters), "iterations": len(iters), "timed_s": t[-1] * 1e-3}, last
 
     import contextlib
     with (ClockSampler(local) if rank == 0 else contextlib.nullcontext()) as clk:
@@ -342,6 +378,7 @@ def main():
             last = step_resident()
         launches0 = C.launch_count() if ours else 0
         t_res, last = measure(step_resident)
+        last_resident = last
         launches = (C.launch_count() - launches0) if ours else None
         ms_per_step = t_res["ms"]
         value = W * H / (ms_per_step * 1e-3) / 1e6
@@ -402,10 +439,10 @@ def main():
     clocks = clk.summary() if clk is not None else {}
 
     # ---- per-stage device times (separate pass, events recorded by the library on the launching stream) ----
-    roofline = roofline_issue = stages = step_hbm = None
+    roofline = stages = step_hbm = None
     if ours and hasattr(C, "stage_timing"):
         C.stage_timing(True)
-        for _ in range(max(a.steps, 20)):
+        for _ in range(a.steps):
             step_resident()
         torch.cuda.synchronize()
         stages = C.stage_times()          # {name: (total_ms, launches)}
@@ -415,8 +452,8 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_source = "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_source = "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet: 3350 GB/s HBM3 (not measured)"
         if not multi:
             Pv = int((rawapi.forward(C, sc, coord, depth)["radii"] > 0).sum().item())
             alg = algorithmic_bytes(P, Pv, R, W * H, tiles, 16, coord, depth)
@@ -425,28 +462,9 @@ def main():
             tot, n = stages.get("render_backward", (0.0, 0))
             if n:
                 dur = tot / n * 1e-3
-                prof, prof_name = None, f"profiles/r02_ncu_render_backward_{a.config}.json"
-                try:
-                    prof = json.load(open(os.path.join(ROOT, prof_name)))
-                except Exception:
-                    pass
-                traffic = None
-                if prof:
-                    traffic = float(prof["dram__bytes_read.sum"]["value"]) * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}.get(prof["dram__bytes_read.sum"].get("unit", "Mbyte"), 1e6) + \
-                        float(prof["dram__bytes_write.sum"]["value"]) * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}.get(prof["dram__bytes_write.sum"].get("unit", "Mbyte"), 1e6)
                 roofline = {"kernel": "render_backward_kernel", "bound": "hbm", "achieved": alg["render_backward"] / dur / 1e9, "peak": peak, "unit": "GB/s",
-                            "frac": alg["render_backward"] / dur / 1e9 / peak, "traffic": traffic,
-                            "traffic_source": (f"REPLAYED from {prof_name} (one `ncu --set full` capture of this kernel on this config), not measured in this run"
-                                               if traffic is not None else None),
-                            "algorithmic_bytes": alg["render_backward"], "avg_launch_ms": tot / n, "peak_source": peak_source,
-                            "note": "this kernel is warp-instruction-issue bound, not HBM bound (records are L2-resident); see roofline_issue and DESIGN.md section 4"}
-                if prof and "smsp__inst_executed.sum" in prof:
-                    inst = float(prof["smsp__inst_executed.sum"]["value"])
-                    clk_hz = (clocks.get("sm_mhz") or 1965.0) * 1e6
-                    floor = inst / (SM_COUNT * 4 * clk_hz)
-                    roofline_issue = {"kernel": "render_backward_kernel", "bound": "warp-instruction issue (4 schedulers/SM, 1 inst/clk each)",
-                                      "warp_instructions": inst, "warp_instructions_source": f"REPLAYED from {prof_name}",
-                                      "sm_clock_mhz": clk_hz / 1e6, "floor_ms": floor * 1e3, "avg_launch_ms": tot / n, "frac": floor / dur}
+                            "frac": alg["render_backward"] / dur / 1e9 / peak, "algorithmic_bytes": alg["render_backward"], "avg_launch_ms": tot / n,
+                            "peak_source": peak_source, "note": "algorithmic bytes over kernel time; the blend kernels are instruction-issue bound (DESIGN.md section 4)"}
             step_alg = sum(alg.values())
             step_hbm = {"algorithmic_bytes": step_alg, "achieved": step_alg / (ms_per_step * 1e-3) / 1e9, "unit": "GB/s", "peak": peak, "frac": step_alg / (ms_per_step * 1e-3) / 1e9 / peak,
                         "per_stage": {}}
@@ -466,27 +484,27 @@ def main():
                                    f"require_depth={depth} require_coord={coord}, fwd+bwd at the _C boundary, num_rendered={R if not multi else 'per-slab'}",
                        "parallelism": (f"tile-row slabs x{world}, gradient-row exchange: {exchange.mode}" + (f" over {exchange.window}" if exchange.window else "") + (f" (peer self-check failed: {exchange.fallback_reason})" if exchange.fallback_reason else "")
                                        if multi else "single GPU"),
-                       "l2": "per-step working set (192 MB SH + 248 MB SH grads + 64 MB records + sort buffers) exceeds the 126 MB L2; no explicit flush",
-                       "protocol": f"median of {t_res['iterations']} per-iteration CUDA-event times ({t_res['windows']} windows of {a.steps} steps, barrier+synchronize around each window, max over ranks per iteration)"},
+                       "l2": "per-step working set (192 MB SH + 248 MB SH grads + 64 MB records + sort buffers) exceeds the 50 MB L2; no explicit flush",
+                       "protocol": f"median of {t_res['iterations']} per-iteration CUDA-event times (one window of {a.steps} steps, barrier+synchronize around it, max over ranks per iteration)"},
             "timing": t_res,
             "e2e": {"value": e2e_value, "unit": "Mpix/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4, "ms_per_step": t_e2e["ms"], "timing": t_e2e,
                     "api": "GaussianRasterizer autograd module (what render() calls) + L1 vs 8-bit GT image + depth/normal/alpha regularisers; camera + GT image H2D from pinned memory every step (GT on a side stream), loss.item() D2H"},
-            "gpu_launches": launches, "clocks": clocks,
+            "gpu_launches": launches, "clocks": clocks, "device": device_info(dev, clk.index if clk is not None else local),
         }
         if stages:
             line["stage_ms"] = {k: v[0] / max(v[1], 1) for k, v in stages.items()}
         if roofline:
             line["roofline"] = roofline
-        if roofline_issue:
-            line["roofline_issue"] = roofline_issue
         if step_hbm:
             line["step_hbm"] = step_hbm
         if a.impl == "reference":
             line["cpu_baseline"] = {"value": value, "unit": "Mpix/s", "cores": 0, "kind": "reference",
-                                    "sample": "reference CUDA rasterizer (oracle/_ref, sm_100a build of /root/reference) on 1xB200; the reference has no CPU rasterizer"}
+                                    "sample": f"reference CUDA rasterizer (oracle/_ref, sm_90a build of the reference) on 1x{torch.cuda.get_device_name(dev)}; the reference has no CPU rasterizer"}
             line["e2e"] = {"value": e2e_value, "unit": "Mpix/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4, "ms_per_step": t_e2e["ms"], "timing": t_e2e}
         elif not a.no_cpu_baseline and not multi:
             line["cpu_baseline"] = cpu_baseline()
+        if a.dump_outputs:
+            line["dump_outputs"] = dump_outputs(a.dump_outputs, last_resident, H, W, P)
         print(json.dumps(line), flush=True)
     if multi:
         exchange.close()

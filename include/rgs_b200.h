@@ -1,5 +1,5 @@
 /*
- * rgs_b200.h -- C ABI of the B200-native differentiable Gaussian-splat rasterizer.
+ * rgs_b200.h -- C ABI of the H100-native (sm_90a) differentiable Gaussian-splat rasterizer.
  *
  * This is the drop-in boundary of the hot path.  The reference binds the same path through a pybind11
  * torch extension (`diff_gaussian_rasterization._C`, reference: submodules/diff-gaussian-rasterization/

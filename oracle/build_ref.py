@@ -2,18 +2,19 @@
 
 TEST INFRASTRUCTURE ONLY -- nothing in the product path imports this.
 
-The sources are compiled from where they lie under /root/reference (never copied into the repo):
+The sources are compiled from where they lie in a RaDe-GS checkout (never copied into the repo): $RADE_GS_REFERENCE when it is
+set, else the checkout this repository is developed beside, `reference/` next to the repository's root directory:
     submodules/diff-gaussian-rasterization/{cuda_rasterizer/{forward,backward,rasterizer_impl}.cu,
                                             rasterize_points.cu, ext.cpp}
 with two non-source workarounds (SURVEY.md section 0):
   * `-I oracle/glm_shim`  -- third_party/glm is an empty directory in the checkout; the shim is our own
     header restating the glm operators the reference uses;
   * `-include cstdint`    -- cuda_rasterizer/rasterizer_impl.h uses std::uintptr_t without including it.
-Flags otherwise follow the reference's setup.py (no fast-math, default -fmad) plus the sm_100a gencode.
+Flags otherwise follow the reference's setup.py (no fast-math, default -fmad) plus the sm_90a gencode.
 
 The module is exported under the name `ref_dgr_C` (the reference's own name is
 `diff_gaussian_rasterization._C`, which the product occupies) and exposes the reference's four pybind
-symbols unchanged.  Outputs go only to oracle/_ref/ (git-ignored, but shipped to the GPU box).
+symbols unchanged.  Outputs go only to oracle/_ref/ (git-ignored).
 
 Usage:  python oracle/build_ref.py [--force]
 """
@@ -26,7 +27,8 @@ import sysconfig
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_ROOT = "/root/reference/submodules/diff-gaussian-rasterization"
+REF_CHECKOUT = os.environ.get("RADE_GS_REFERENCE") or os.path.join(os.path.dirname(os.path.dirname(HERE)), "reference")
+REF_ROOT = os.path.join(REF_CHECKOUT, "submodules", "diff-gaussian-rasterization")
 OUT_DIR = os.path.join(HERE, "_ref")
 OBJ_DIR = os.path.join(HERE, "_build", "ref")
 MODULE = "ref_dgr_C"
@@ -48,7 +50,7 @@ def target() -> str:
 
 
 def build(force: bool = False, verbose: bool = True) -> str | None:
-    """Returns the path of the built module, or None when /root/reference is absent and nothing is prebuilt."""
+    """Returns the path of the built module, or None when the reference checkout is absent and nothing is prebuilt."""
     out = target()
     if not available():
         return out if os.path.exists(out) else None
@@ -70,7 +72,7 @@ def build(force: bool = False, verbose: bool = True) -> str | None:
     def compile_one(src: str) -> str:
         obj = os.path.join(OBJ_DIR, os.path.basename(src) + ".o")
         if src.endswith(".cu"):
-            cmd = [nvcc, "-c", src, "-o", obj, "-gencode", "arch=compute_100a,code=sm_100a",
+            cmd = [nvcc, "-c", src, "-o", obj, "-gencode", "arch=compute_90a,code=sm_90a",
                    "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-w"] + common
         else:
             cmd = ["g++", "-c", src, "-o", obj, "-fPIC", "-w"] + common
@@ -93,14 +95,15 @@ def build(force: bool = False, verbose: bool = True) -> str | None:
 
 
 def load():
-    """Import the prebuilt reference module (GPU box or here).  Raises if it was never built."""
+    """Import the prebuilt reference module.  Raises if it was never built."""
     import importlib.util
 
     import torch  # noqa: F401  (libtorch must be loaded before the extension)
 
     path = target()
     if not os.path.exists(path):
-        raise FileNotFoundError(path + " missing: run `python oracle/build_ref.py` where /root/reference exists")
+        raise FileNotFoundError(path + " missing: run `python oracle/build_ref.py` with a RaDe-GS checkout at " + REF_CHECKOUT +
+                                " (or named by $RADE_GS_REFERENCE)")
     spec = importlib.util.spec_from_file_location(MODULE, path)
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)

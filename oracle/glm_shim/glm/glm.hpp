@@ -1,7 +1,7 @@
 // Minimal stand-in for the subset of g-truc/glm that the reference rasterizer uses.
 //
 // TEST INFRASTRUCTURE ONLY.  The reference checkout pins glm as an un-vendored submodule
-// (g-truc/glm @ 6f14f4792a0cde5d0cf2c910506724d61cb95834, /root/reference/.SUBMODULES.json) and the
+// (g-truc/glm @ 6f14f4792a0cde5d0cf2c910506724d61cb95834, the reference's .SUBMODULES.json) and the
 // directory third_party/glm is empty, so the reference CUDA sources cannot be compiled without
 // something that answers `#include <glm/glm.hpp>`.  This header is written from scratch for that one
 // purpose (oracle/build_ref.py).  It is never included by the product kernels.

@@ -5,7 +5,7 @@
  * this; the product (rade-gs_b200/) never does and has no CPU path.
  *
  * It restates, serially and without atomics, what the reference computes (paths relative to
- * /root/reference/submodules/diff-gaussian-rasterization/cuda_rasterizer/):
+ * submodules/diff-gaussian-rasterization/cuda_rasterizer/ of the reference):
  *   orc_preprocess           forward.cu:270-304 (cov3D), :77-264 (cov2D, planes, normal), :23-74 (SH), :307-423
  *   orc_eig_sym3             auxiliary.h:182-401 (Householder + QL with absolute 1e-7 tests)
  *   orc_binning              rasterizer_impl.cu:70-111 (keys), :373-381 (stable sort), :151-173 (ranges)
@@ -17,7 +17,7 @@
  *   orc_integrate            forward.cu:857-900 (points), rasterizer_impl.cu:114-145 (point -> tile), forward.cu:938-1372
  *
  * Parity pin: tests/test_oracle_golden.py checks every function against tests/golden/<case>.npz, which were
- * produced by the unmodified reference CUDA build on a B200 (tools/gen_golden.py).
+ * produced by the unmodified reference CUDA build (tools/gen_golden.py).
  *
  * Arithmetic is float with the same double-promoted sub-expressions as the reference; gcc is run with
  * -ffp-contract=off, so results differ from the CUDA builds (which contract to FMA) in the last bits only.

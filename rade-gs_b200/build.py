@@ -1,4 +1,4 @@
-"""In-tree build of the B200 rasterizer (sm_100a only).
+"""In-tree build of the H100 rasterizer (sm_90a only).
 
 Produces, next to the Python packages so they travel with the source tree:
   rade-gs_b200/rade_gs_b200/librgs_b200.so              -- the C-ABI library (include/rgs_b200.h), no torch dependency
@@ -28,7 +28,7 @@ HEADERS = ["rgs_common.cuh", "rgs_geom.cuh", "rgs_render_common.cuh", os.path.jo
 # division / sqrt (2-3 instructions instead of ~10 with a slow-path call); the eigen-solver inside it uses explicit IEEE
 # intrinsics.  Forward preprocess keeps IEEE division: its expression chain decides the tile keys bit-exactly.
 EXTRA_FLAGS = {"rgs_preprocess_bwd.cu": ["-prec-div=false", "-prec-sqrt=false"]}
-NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr", "-Xcudafe", "--diag_suppress=177"]
 
 
@@ -61,7 +61,7 @@ def build_core(force=False, verbose=False) -> str:
     objs = [o for o, _ in res]
     if force or any(ch for _, ch in res) or not os.path.exists(LIB):
         tmp = LIB + ".tmp"   # link to a temporary name and rename: a snapshot of the tree never sees a half-written library
-        _run([NVCC, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "shared"], verbose)
+        _run([NVCC, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "shared"], verbose)
         os.replace(tmp, LIB)
         print("[build] wrote", LIB, flush=True)
     return LIB

@@ -1,4 +1,4 @@
-// rgs_common.cuh -- shared definitions of the B200 rasterizer kernels (sm_100a only).
+// rgs_common.cuh -- shared definitions of the rasterizer kernels (sm_90a only).
 //
 // Layouts here are private to the library (the reference treats its three byte buffers as opaque too,
 // cuda_rasterizer/rasterizer_impl.h:22-94); include/rgs_b200.h is the public surface.
@@ -20,7 +20,7 @@ constexpr int TILE_PIX = TILE_X * TILE_Y;
 //         8 r 9 g 10 b 11 t_center | 12 nx 13 ny 14 nz 15 cam_plane[5] |
 //         16 vx 17 vy 18 vz 19 cam_plane[0] | 20..23 cam_plane[1..4]
 // Pairs that are multiplied by a common factor in the blend sit in even/odd slots (mx,my), (ray.x,ray.y), (r,g),
-// (b,t), (nx,ny): they land in aligned register pairs and go through Blackwell's packed fp32x2 FMUL2/FFMA2.
+// (b,t), (nx,ny): they are loaded as float4 and blended pairwise (ffma2 / fmul2 in rgs_render_common.cuh).
 constexpr int REC_FLOATS_BASE = 16;   // variants none / depth
 constexpr int REC_FLOATS_COORD = 24;  // variants coord / coord+depth
 
@@ -195,6 +195,16 @@ inline void ensure_dynamic_smem(Kernel kernel, size_t bytes, size_t (&configured
 		cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
 		configured[dev] = bytes;
 	}
+}
+
+// SM count of the CURRENT device (sizes grid-stride launches), queried once per device.
+inline int sm_count() {
+	static int cached[64] = {};
+	int dev = 0;
+	cudaGetDevice(&dev);
+	dev &= 63;
+	if (cached[dev] == 0) cudaDeviceGetAttribute(&cached[dev], cudaDevAttrMultiProcessorCount, dev);
+	return cached[dev];
 }
 
 // kernels' host launchers (one translation unit each)

@@ -10,7 +10,7 @@
 //      Gaussian at every one of its points.
 // Step 2 makes every pixel thread scan all points and all Gaussians of its tile again per batch of points.
 //
-// B200 design: the contribution sets go to HBM as bit masks (one bit per list entry and pixel, written coalesced by the
+// Design: the contribution sets go to HBM as bit masks (one bit per list entry and pixel, written coalesced by the
 // pixel threads), and step 2 becomes POINT-parallel: points are sorted by pixel (CUB radix sort on the pixel index),
 // one thread per point walks only the set bits of its pixel's mask.  Neighbouring lanes hold points of the same or
 // adjacent pixels, so mask words and splat records are broadcast loads.  No per-thread id arrays (no local-memory

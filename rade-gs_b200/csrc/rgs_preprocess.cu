@@ -1,4 +1,4 @@
-// rgs_preprocess.cu -- per-Gaussian forward preprocess for sm_100a.
+// rgs_preprocess.cu -- per-Gaussian forward preprocess for sm_90a.
 //
 // Replaces preprocessCUDA<3,false> + computeCov3D + computeCov2D<false> + computeColorFromSH
 // (reference: cuda_rasterizer/forward.cu:23-74, 77-264, 270-304, 307-423) and checkFrustum

@@ -1,4 +1,4 @@
-// rgs_preprocess_bwd.cu -- per-Gaussian backward preprocess for sm_100a.
+// rgs_preprocess_bwd.cu -- per-Gaussian backward preprocess for sm_90a.
 //
 // Replaces, fused into one kernel, computeCov2DCUDA + preprocessCUDA<3> backward with
 // computeColorFromSH / computeCov3D backward (reference: cuda_rasterizer/backward.cu:145-488, 560-628,
@@ -692,7 +692,7 @@ void launch_preprocess_backward(const FwdParams& p, GeomView g, const int* radii
 	else
 		nonzero_rows_kernel<GRAD_FLOATS_COORD / 4><<<(p.P + 255) / 256, 256, 0, s>>>(p.P, radii, reinterpret_cast<const float4*>(grad_accum), list, count);
 	// the list length stays on the device (no host sync): grids sized for "every row listed", CTAs beyond the list leave at once
-	const int sms = 148;
+	const int sms = sm_count();
 	const int rows_grid = min((p.P + 127) / 128, sms * 16);
 	preprocess_backward_rows_kernel<<<rows_grid, 128, 0, s>>>(p, g, radii, grad_accum, out, fix_mip, list, count);
 	count_launch(2 + 8 + (has_sh ? 1 : 0));

@@ -1,4 +1,4 @@
-// rgs_render_bwd.cu -- per-tile backward of the alpha blend for sm_100a.
+// rgs_render_bwd.cu -- per-tile backward of the alpha blend for sm_90a.
 //
 // Replaces renderCUDA<3,COORD,DEPTH,NORMAL> backward (reference: cuda_rasterizer/backward.cu:631-1016,
 // dispatch :1101-1163).  The per-pixel recurrence (back-to-front re-traversal, T recovered by division,
@@ -31,11 +31,11 @@ __device__ __forceinline__ void warp_reduce_scatter(float (&v)[N], int lane) {
 		const bool upper = (lane & mask) != 0;
 #pragma unroll
 		for (int k = 0; k < h; k += 2) {
-			// two values per step: the adds go through the packed fp32x2 pipe (one FADD2 instead of two FADD)
+			// two values per step, added lane by lane (fadd2)
 			const float s0 = upper ? v[k] : v[k + h], s1 = upper ? v[k + 1] : v[k + h + 1];
 			const float2 keep = make_float2(upper ? v[k + h] : v[k], upper ? v[k + h + 1] : v[k + 1]);
 			const float2 recv = make_float2(__shfl_xor_sync(0xffffffffu, s0, mask), __shfl_xor_sync(0xffffffffu, s1, mask));
-			const float2 sum = __fadd2_rn(keep, recv);
+			const float2 sum = fadd2(keep, recv);
 			v[k] = sum.x;
 			v[k + 1] = sum.y;
 		}
@@ -241,7 +241,7 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 				const int contributor = pos0 - jj;  // 0-based position in the tile list (backward.cu:837)
 				const uint32_t sa = s_addr + (uint32_t)jj * 16u;
 				const float4 q0 = lds128(sa), q1 = lds128(sa + BATCH * 16u);  // (mx my A B) (C o ray.x ray.y)
-				const float2 d = __fadd2_rn(make_float2(q0.x, q0.y), npix);   // centre - pixel
+				const float2 d = fadd2(make_float2(q0.x, q0.y), npix);   // centre - pixel
 				const float dx = d.x, dy = d.y;
 				const float power = -0.5f * (q0.z * dx * dx + q1.x * dy * dy) - q0.w * dx * dy;
 				const float G = expf(power);
@@ -261,7 +261,7 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 				// -- one running scalar instead of 8 running blends + 8 "last" values (same algebra, different rounding).
 				//
 				// Channels that share a factor are kept in aligned register pairs -- (r,g) (b,t) (nx,ny) on the record side,
-				// (g_r,g_g) (g_b,g_t) (g_nx,g_ny) on the pixel side -- and go through the packed fp32x2 FMUL2 / FFMA2.
+				// (g_r,g_g) (g_b,g_t) (g_nx,g_ny) on the pixel side -- and go through the two-lane helpers fmul2 / ffma2.
 				const float alpha = ok ? alpha_raw : 0.f;
 				float4 q2 = lds128(sa + 2 * BATCH * 16u);  // r g b t_center
 				float gv[GF];
@@ -270,10 +270,10 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 				const float w = alpha * T;  // dchannel_dcolor
 				const float2 w2 = make_float2(w, w);
 				if constexpr (DEPTH) q2.w = q2.w + (q1.z * dx + q1.w * dy);  // t = t_center + ray . d
-				float2 S2 = __ffma2_rn(make_float2(q2.x, q2.y), g_rg, make_float2(dL_dalpha, 0.f));
-				S2 = __ffma2_rn(make_float2(q2.z, q2.w), g_bt, S2);
-				const float2 c_rg = __fmul2_rn(w2, g_rg);
-				float2 c_bt = __fmul2_rn(w2, g_bt);  // (dL_dcolor.b, dL_dt before the median term)
+				float2 S2 = ffma2(make_float2(q2.x, q2.y), g_rg, make_float2(dL_dalpha, 0.f));
+				S2 = ffma2(make_float2(q2.z, q2.w), g_bt, S2);
+				const float2 c_rg = fmul2(w2, g_rg);
+				float2 c_bt = fmul2(w2, g_bt);  // (dL_dcolor.b, dL_dt before the median term)
 				gv[G_COL + 0] = c_rg.x;
 				gv[G_COL + 1] = c_rg.y;
 				gv[G_COL + 2] = c_bt.x;
@@ -303,13 +303,13 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 					if (is_median) dL_dt += dL_dpixel_mt;
 				}
 				gv[G_T] = dL_dt;
-				const float2 g_ray = __fmul2_rn(make_float2(dL_dt, dL_dt), d);
+				const float2 g_ray = fmul2(make_float2(dL_dt, dL_dt), d);
 				gv[G_RAYX] = g_ray.x;
 				gv[G_RAYY] = g_ray.y;
 				float S;
 				if constexpr (GEO) {
-					S2 = __ffma2_rn(make_float2(q3.x, q3.y), g_nxy, S2);
-					const float2 c_n = __fmul2_rn(w2, g_nxy);
+					S2 = ffma2(make_float2(q3.x, q3.y), g_nxy, S2);
+					const float2 c_n = fmul2(w2, g_nxy);
 					S = fmaf(q3.z, g_nz, S2.x + S2.y);
 					gv[G_NRM + 0] = c_n.x;
 					gv[G_NRM + 1] = c_n.y;
@@ -323,21 +323,21 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 				const float Gm = ok ? G : 0.f;  // the reference skips this pair entirely: every term below carries a factor G
 
 				const float dL_dG = q1.y * dL_dopa;
-				const float2 gd = __fmul2_rn(make_float2(Gm, Gm), d);  // (G dx, G dy)
+				const float2 gd = fmul2(make_float2(Gm, Gm), d);  // (G dx, G dy)
 				const float dG_ddelx = -gd.x * q0.z - gd.y * q0.w;
 				const float dG_ddely = -gd.y * q1.x - gd.x * q0.w;
-				float2 dL_ddel = __fmul2_rn(make_float2(dL_dG, dL_dG), make_float2(dG_ddelx, dG_ddely));
-				const float2 ab = __fmul2_rn(dL_ddel, make_float2(ddelx_dx, ddely_dy));
+				float2 dL_ddel = fmul2(make_float2(dL_dG, dL_dG), make_float2(dG_ddelx, dG_ddely));
+				const float2 ab = fmul2(dL_ddel, make_float2(ddelx_dx, ddely_dy));
 				gv[G_MABS] = abs(ab.x) + abs(ab.y);
 				if constexpr (COORD) {
 					dL_ddel.x += dL_dcoords[0] * q4.w + dL_dcoords[1] * q5.y + dL_dcoords[2] * q5.w;
 					dL_ddel.y += dL_dcoords[0] * q5.x + dL_dcoords[1] * q5.z + dL_dcoords[2] * q3.w;
 				}
-				if constexpr (DEPTH) dL_ddel = __ffma2_rn(make_float2(dL_dt, dL_dt), make_float2(q1.z, q1.w), dL_ddel);
+				if constexpr (DEPTH) dL_ddel = ffma2(make_float2(dL_dt, dL_dt), make_float2(q1.z, q1.w), dL_ddel);
 				gv[G_MX] = dL_ddel.x;  // * 0.5 W in backward-preprocess
 				gv[G_MY] = dL_ddel.y;  // * 0.5 H
 				const float hG = -0.5f * dL_dG;
-				const float2 cxy = __fmul2_rn(__fmul2_rn(make_float2(gd.x, gd.x), d), make_float2(hG, hG));
+				const float2 cxy = fmul2(fmul2(make_float2(gd.x, gd.x), d), make_float2(hG, hG));
 				gv[G_CONX] = cxy.x;
 				gv[G_CONY] = cxy.y;
 				gv[G_CONW] = gd.y * dy * hG;

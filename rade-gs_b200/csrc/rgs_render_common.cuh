@@ -14,6 +14,13 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src)
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
 
+// Two-lane float ops on the (x, y) pairs the records keep side by side.  Hopper has no packed fp32x2 pipe, so each lane is
+// one scalar op; the _rn intrinsics keep every product and sum separately rounded (no contraction into FMAs), which is
+// the rounding the blend and its gradient were validated with.
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+
 // Conservative test: can splat (centre c, conic A,B,C, opacity o) reach alpha >= 1/255 anywhere in the
 // pixel box [x0,x1]x[y0,y1]?  alpha = o*exp(-q), q = 0.5(A dx^2 + C dy^2) + B dx dy, so the splat matters
 // only where q <= ln(255 o).  q is convex when the conic is positive definite; its minimum over a box is

@@ -1,4 +1,4 @@
-// rgs_render_fwd.cu -- per-tile forward alpha blend for sm_100a.
+// rgs_render_fwd.cu -- per-tile forward alpha blend for sm_90a.
 //
 // Replaces renderCUDA<3,COORD,DEPTH,NORMAL> forward (reference: cuda_rasterizer/forward.cu:428-693,
 // dispatch :696-742).  Same tile size (16x16, part of the key contract), same per-pixel arithmetic
@@ -119,12 +119,12 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 4 : 5)) render_forward_kern
 				if (ok) {
 					const float aT = alpha * T;
 					const float2 aT2 = make_float2(aT, aT);
-					// (r,g), (b,t), (nx,ny), (nz,1) sit in aligned register pairs: four packed FFMA2 blend 8 channels
-					C01 = __ffma2_rn(make_float2(q2.x, q2.y), aT2, C01);
+					// (r,g), (b,t), (nx,ny), (nz,1) are blended as pairs: four two-lane FMAs cover 8 channels
+					C01 = ffma2(make_float2(q2.x, q2.y), aT2, C01);
 					const bool before_median = T > 0.5;
 					float t = 0.f;
 					if constexpr (DEPTH) t = q2.w + (q1.z * dx + q1.w * dy);
-					C2D = __ffma2_rn(make_float2(q2.z, t), aT2, C2D);  // (blue, ray-space depth)
+					C2D = ffma2(make_float2(q2.z, t), aT2, C2D);  // (blue, ray-space depth)
 					if constexpr (GEO) {
 						const float4 q3 = s[3 * BATCH + jj];
 						if constexpr (COORD) {
@@ -141,8 +141,8 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 4 : 5)) render_forward_kern
 						if constexpr (DEPTH) {
 							if (before_median) mDepth = t;
 						}
-						N01 = __ffma2_rn(make_float2(q3.x, q3.y), aT2, N01);
-						N2W = __ffma2_rn(make_float2(q3.z, 1.f), aT2, N2W);  // (normal z, weight)
+						N01 = ffma2(make_float2(q3.x, q3.y), aT2, N01);
+						N2W = ffma2(make_float2(q3.z, 1.f), aT2, N2W);  // (normal z, weight)
 						if (before_median) max_contributor = contributor;
 					} else {
 						N2W.y += aT;

@@ -1,4 +1,4 @@
-"""Drop-in ``diff_gaussian_rasterization`` package backed by the B200-native rasterizer.
+"""Drop-in ``diff_gaussian_rasterization`` package backed by the H100-native (sm_90a) rasterizer.
 
 Public surface kept identical to the reference wrapper
 (reference: submodules/diff-gaussian-rasterization/diff_gaussian_rasterization/__init__.py):
@@ -28,8 +28,8 @@ try:
     from . import _C
 except ImportError as _exc:  # fail loudly: a silent fallback would void every parity claim
     raise ImportError(
-        "diff_gaussian_rasterization._C (B200 build) is missing or failed to load: run "
-        "`python rade-gs_b200/build.py` (needs nvcc, sm_100a).  Original error: %s" % (_exc,)
+        "diff_gaussian_rasterization._C (sm_90a build) is missing or failed to load: run "
+        "`python rade-gs_b200/build.py` (needs nvcc, sm_90a).  Original error: %s" % (_exc,)
     ) from _exc
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians"]

@@ -76,8 +76,7 @@ def exchange_sum_(acc: torch.Tensor, group=None, mode: str | None = None) -> tor
     ``sparse`` (opt-in): a rank's rows are zero for every Gaussian that does not reach its slab (with 8 slabs a splat touches
     1.25 of them on average), so each rank ships only its non-zero rows -- index + row, one all-gather -- and every rank
     rebuilds the sum by adding the ranks' rows in rank order (fixed order: same bits everywhere, like an all-reduce).
-    Measured on 8 B200 at C2 it LOSES to NCCL's all-reduce (1.67 vs 1.43 ms per step, profiles/r01_bench_ours_n8*.json): the
-    two size exchanges with their host synchronisations and eight index_add_ passes cost more than the 0.5 ms all-reduce
+    Its two size exchanges with their host synchronisations and eight index_add_ passes can cost more than the all-reduce
     they replace.  Kept because the control flow is the starting point for a fused device-side exchange (no host syncs).
     """
     if not (dist.is_available() and dist.is_initialized()):

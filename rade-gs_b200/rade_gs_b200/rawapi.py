@@ -1,4 +1,4 @@
-"""Thin helpers that call a `_C`-style module (the B200 build or the reference build) on a synthetic Scene.
+"""Thin helpers that call a `_C`-style module (this build or the reference build) on a synthetic Scene.
 
 Both modules export the reference's `rasterize_gaussians` / `rasterize_gaussians_backward`
 (reference: rasterize_points.h:18-76), so the same two functions drive either one -- this is what the parity
@@ -60,7 +60,7 @@ class _Cursor:
 
 
 def ours_views(fwd: dict, sc) -> dict:
-    """Decode the B200 build's buffers (layout: rgs_api.cu carve_geom / carve_bin / carve_img)."""
+    """Decode this build's buffers (layout: rgs_api.cu carve_geom / carve_bin / carve_img)."""
     P = sc.means3D.shape[0]
     R = int(fwd["num_rendered"])
     coord, depth = fwd["_call"]["require_coord"], fwd["_call"]["require_depth"]

@@ -7,6 +7,7 @@ convention (``scene/cameras.py:54-57``, ``utils/graphics_utils.py:67-87``).
 """
 from __future__ import annotations
 
+import contextlib
 import math
 from dataclasses import dataclass
 
@@ -19,6 +20,18 @@ CONFIGS = {
     "C3": (3_000_000, 1920, 1080, 1600.0, -5.0, True, False),
     "C4": (10_000_000, 4096, 4096, 3600.0, -5.6, False, True),
 }
+
+
+@contextlib.contextmanager
+def _one_thread():
+    """Synthesis on one CPU thread: torch's threaded, vectorised exp / normal sampling can change last bits with the thread
+    count, and the stored fixtures pin these inputs by their bits (tools/golden_inputs.py)."""
+    n = torch.get_num_threads()
+    torch.set_num_threads(1)
+    try:
+        yield
+    finally:
+        torch.set_num_threads(n)
 
 
 @dataclass
@@ -76,6 +89,11 @@ def look_at_view(eye, target, up=(0.0, -1.0, 0.0)) -> torch.Tensor:
 def make_scene(P: int, W: int, H: int, focal: float, mu: float, seed: int = 1234, sh_rest_std: float = 0.1,
                view: torch.Tensor | None = None, bg=(0.0, 0.0, 0.0), zmin: float = 2.0, zmax: float = 10.0) -> Scene:
     """SURVEY.md appendix C recipe.  Draw order: z, x, y, scales, rotations, opacity, SH-dc, SH-rest."""
+    with _one_thread():
+        return _make_scene(P, W, H, focal, mu, seed, sh_rest_std, view, bg, zmin, zmax)
+
+
+def _make_scene(P, W, H, focal, mu, seed, sh_rest_std, view, bg, zmin, zmax) -> Scene:
     g = torch.Generator().manual_seed(seed)
     tanx, tany = W / (2 * focal), H / (2 * focal)
 
@@ -119,7 +137,8 @@ def make_upstream_grads(H: int, W: int, seed: int = 4321, device="cpu") -> dict:
     def N(c, s=1.0):
         return (torch.randn(c, H, W, generator=g) * s).to(device)
 
-    return {
-        "color": N(3), "coord": N(3, 0.1), "mcoord": N(3, 0.1), "depth": N(1, 0.1), "mdepth": N(1, 0.1),
-        "alpha": N(1, 0.1), "normal": N(3, 0.1),
-    }
+    with _one_thread():
+        return {
+            "color": N(3), "coord": N(3, 0.1), "mcoord": N(3, 0.1), "depth": N(1, 0.1), "mdepth": N(1, 0.1),
+            "alpha": N(1, 0.1), "normal": N(3, 0.1),
+        }

@@ -1,4 +1,4 @@
-"""Shared test plumbing.  `-m "not gpu"` runs here on CPU; `-m gpu` runs on the B200 box."""
+"""Shared test plumbing.  `-m "not gpu"` runs without a GPU; `-m gpu` needs an H100."""
 import os
 import sys
 
@@ -6,18 +6,18 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for p in (os.path.join(ROOT, "rade-gs_b200"), os.path.join(ROOT, "oracle"), ROOT):
+for p in (os.path.join(ROOT, "rade-gs_b200"), os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tools"), ROOT):
     if p not in sys.path:
         sys.path.insert(0, p)
 
 GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 _ALL_GOLDEN = sorted(f[:-4] for f in os.listdir(GOLDEN_DIR) if f.endswith(".npz")) if os.path.isdir(GOLDEN_DIR) else []
-GOLDEN_CASES = [c for c in _ALL_GOLDEN if not c.startswith(("integrate_", "fused_"))]       # rasterize fwd/bwd (tools/gen_golden.py)
+GOLDEN_CASES = [c for c in _ALL_GOLDEN if not c.startswith(("integrate_", "fused_", "refbuild_"))]  # rasterize fwd/bwd (tools/gen_golden.py)
 INTEGRATE_CASES = [c for c in _ALL_GOLDEN if c.startswith("integrate_")]        # integrate (tools/gen_golden_integrate.py)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -30,14 +30,22 @@ def pytest_collection_modifyitems(config, items):
         has_gpu = False
     if has_gpu:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (run with -m gpu on the B200 box)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (run with -m gpu on an H100)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)
 
 
 def load_golden(name):
-    return dict(np.load(os.path.join(GOLDEN_DIR, name + ".npz")))
+    """A fixture as a dict of arrays.  Fixtures made from seeded scenes store a digest of their inputs instead of the inputs:
+    those are regenerated (tools/golden_inputs.py) and must match it bit for bit."""
+    d = dict(np.load(os.path.join(GOLDEN_DIR, name + ".npz")))
+    if "inputs_digest" in d:
+        import golden_inputs
+        inputs = golden_inputs.inputs_of(name)
+        assert golden_inputs.digest(inputs) == str(d.pop("inputs_digest")), f"{name}: the regenerated inputs differ from the fixture's"
+        d.update(inputs)
+    return d
 
 
 def golden_oracle_inputs(d):

@@ -1,5 +1,5 @@
 """The widened rows (SURVEY.md 8f-1, 8f-2, 8f-4) against fixtures produced by the REFERENCE'S OWN Python functions
-(tools/gen_golden_fused.py imports utils/loss_utils.py, utils/graphics_utils.py and scene/gaussian_model.py from /root/reference
+(tools/gen_golden_fused.py imports utils/loss_utils.py, utils/graphics_utils.py and scene/gaussian_model.py from the reference checkout
 and writes tests/golden/fused_*.npz).  GPU tests compare the fused kernels with those outputs; the CPU tests pin the PLY writer /
 reader to the bytes the reference's save_ply produced.
 

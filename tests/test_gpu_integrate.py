@@ -1,5 +1,5 @@
 """`GaussianRasterizer.integrate` (SURVEY.md 8f row 3) on the GPU against (1) the fixtures produced by the unmodified reference
-build, (2) the CPU oracle on fresh scenes, (3) the reference build itself on the box when present.
+build, (2) the CPU oracle on fresh scenes, (3) digests and samples of the reference build's results on a 50k-splat scene.
 
 Tolerances as in tests/test_oracle_integrate.py: integers, radii, projected coordinates and the points-per-pixel channel
 exact; float results 1e-4 (+1e-4 relative) with at most 1e-3 of the elements across an alpha threshold."""
@@ -117,14 +117,22 @@ def test_integrate_many_points_in_one_pixel_and_empty_inputs():
 
 
 def test_integrate_next_to_the_reference_build():
-    """Mesh-extraction-like load (50k splats, 9 points per splat) next to the reference's own kernel on the same GPU."""
-    import build_ref
-    if not os.path.exists(build_ref.target()):
-        pytest.skip("reference build oracle/_ref/ref_dgr_C.so not present on this box")
-    ref = build_ref.load()
+    """Mesh-extraction-like load (50k splats, 9 points per splat) against what the reference's own kernel computed on the same
+    inputs (tools/gen_golden_refbuild.py: digests of the exact results, samples of the float ones)."""
     sys.path.insert(0, os.path.join(ROOT, "tools"))
-    from gen_golden_integrate import call_reference
+    from gen_golden_refbuild import digest, scene_digest
+    d = load_golden("refbuild_integrate_50k")
     sc, pts = _fresh_scene(50_000, 400, 304, 330.0, -3.0, 9, 450_000)
+    assert scene_digest(sc) + digest(pts) == str(d["in_digest"]), "the synthetic inputs differ from the ones the fixture was made from"
     ours = _run_ours(sc, pts)
-    r = call_reference(ref, sc.to(DEV), pts.to(DEV), 3)
-    _check(ours, {k: v.cpu().numpy() for k, v in zip(NAMES, r[1:7])}, "ref-50k")
+    assert digest(ours["radii"]) == str(d["sha_radii"])
+    assert digest(ours["point_coordinate"]) == str(d["sha_point_coordinate"])
+    assert digest(ours["color"][8]) == str(d["sha_points_per_pixel"])
+    assert digest(ours["point_sdf"] == -1000.0) == str(d["sha_untouched"])
+    assert not ours["color"][5].any()
+    color = ours["color"].reshape(9, -1)[:, d["pix"]]
+    for ch in (0, 1, 2, 3, 4, 6, 7):
+        close_with_outliers(color[ch], d["color"][ch], f"ref-50k/color[{ch}]")
+    for k in ("alpha_integrated", "color_integrated", "point_sdf"):
+        close_with_outliers(ours[k][d["pts"]], d[k], f"ref-50k/{k}")
+    assert (ours["alpha_integrated"][ours["point_sdf"] == -1000.0] == 1.0).all()

@@ -84,10 +84,9 @@ def _worker(rank, world, port, outdir, exchange_mode, variant, compact=False):
             res[f"{step}/bits_differ_from_rank0"] = int((flat.view(torch.int32) != ref.view(torch.int32)).sum())
         np.save(os.path.join(outdir, f"res{rank}.npy"), res, allow_pickle=True)
         ev = {k: v for k, v in res.items() if k.endswith("/evidence")}
-        if ev:   # keep the full evidence where the driver of the GPU box can collect it
+        if ev:   # keep the full evidence next to the per-rank results
             try:
-                os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-                with open(os.path.join(ROOT, "gpurun_out", "multi_mismatch_evidence.txt"), "a") as f:
+                with open(os.path.join(outdir, "multi_mismatch_evidence.txt"), "a") as f:
                     f.write(f"world {world} rank {rank} exchange {exchange_mode} variant {variant} compact {compact}: {ev}\n")
             except OSError:
                 pass

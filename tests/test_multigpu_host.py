@@ -258,7 +258,7 @@ def _bcast_worker(rank, world, port, tmpdir):
 
 
 def test_broadcast_scene_makes_the_replicated_state_bit_identical(tmp_path):
-    """Slabs only compose to the single-GPU image when every rank rasterizes the same bits (profiles/r02_crossrank_inputs_probe.txt)."""
+    """Slabs only compose to the single-GPU image when every rank rasterizes the same bits."""
     port = 36500 + (os.getpid() % 2000)
     mp.spawn(_bcast_worker, args=(2, port, str(tmp_path)), nprocs=2, join=True)
     a, b = (torch.load(tmp_path / f"bcast{r}.pt") for r in range(2))

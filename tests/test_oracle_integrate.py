@@ -1,5 +1,5 @@
 """Pins the oracle's restatement of `integrate_gaussians_to_points` (oracle.c: orc_inte_geometry, orc_integrate) to the
-fixtures the UNMODIFIED reference CUDA build produced on a B200 (tools/gen_golden_integrate.py).
+fixtures the UNMODIFIED reference CUDA build produced (tools/gen_golden_integrate.py).
 
 Tolerances: integer results (radii, num_rendered, points per pixel) and the projected point coordinates are exact; float
 maps and per-point results within 1e-4 absolute (observed: <= 5e-6), allowing 1e-3 of the elements to sit on the other

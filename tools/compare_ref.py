@@ -1,6 +1,6 @@
-"""GPU-side parity report: B200 build vs the reference build (oracle/_ref/ref_dgr_C.so) on the same inputs.
+"""GPU-side parity report: this build vs the reference build (oracle/_ref/ref_dgr_C.so) on the same inputs.
 
-Run on the GPU box:  python tools/compare_ref.py [--cfg small|C1|C2|C3] [--ks 0.0] [--coord 0/1] [--depth 0/1] [--time]
+Needs a GPU:  python tools/compare_ref.py [--cfg small|C1|C2|C3] [--ks 0.0] [--coord 0/1] [--depth 0/1] [--time]
 Prints exact-match counts for the integer contract (radii, num_rendered, sorted ids, tile ranges, n_contrib) and
 error statistics for images / gradients.  Test infrastructure, not product.
 """

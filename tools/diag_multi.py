@@ -1,4 +1,4 @@
-"""N-rank diagnosis of the sharded forward (run with torchrun on an N-GPU box):
+"""N-rank diagnosis of the sharded forward (run with torchrun on an N-GPU node):
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29544 tools/diag_multi.py
 

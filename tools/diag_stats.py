@@ -1,4 +1,4 @@
-"""Workload statistics that decide optimisation choices (run on the GPU box):  python tools/diag_stats.py [C2]
+"""Workload statistics that decide optimisation choices (needs a GPU):  python tools/diag_stats.py [C2]
   * visible Gaussians whose accumulator row is all-zero after backward-render (no pixel received them): backward-preprocess and
     the SH backward could skip them;
   * hits per (warp, splat) and live-lane statistics are in the ncu captures (smsp__thread_inst_executed_per_inst_executed)."""

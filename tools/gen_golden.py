@@ -1,8 +1,8 @@
 """Generate the golden fixtures under tests/golden/ from the UNMODIFIED reference build (oracle/_ref/ref_dgr_C.so).
 
-Must run where a GPU is (the reference has no CPU path):   gpurun -- python tools/gen_golden.py
-The outputs land in gpurun_out/golden/*.npz; copy them to tests/golden/ and commit them together with this script.
-Each fixture holds the inputs, the settings, every forward output, the reference's internal per-Gaussian /
+Must run where a GPU is (the reference has no CPU path):   python tools/gen_golden.py [CASE ...]
+The outputs land in golden_out/; copy them to tests/golden/ and commit them together with this script.
+Each fixture holds a digest of the inputs (regenerated from the case's seed by tools/golden_inputs.py), the settings, every forward output, the reference's internal per-Gaussian /
 binning state (decoded from its buffers, SURVEY.md appendix B) and the eight gradient tensors.  The reference's
 backward uses float atomics, so gradients are stored as the mean of two runs and the observed run-to-run
 difference is stored next to them (`grad_noise_*`).
@@ -20,6 +20,8 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from rade_gs_b200 import rawapi, scenes  # noqa: E402
+
+import golden_inputs  # noqa: E402
 
 # name: (P, W, H, focal, mu, seed, coord, depth, kernel_size, sh_degree, look_at, precomp)
 CASES = {
@@ -66,7 +68,7 @@ def main():
     import build_ref
     ref = build_ref.load()
     dev = torch.device("cuda:0")
-    out_dir = os.path.join(ROOT, "gpurun_out", "golden")
+    out_dir = "golden_out"
     os.makedirs(out_dir, exist_ok=True)
     for name, c in CASES.items():
         if only and name not in only:
@@ -82,13 +84,10 @@ def main():
         v = rawapi.ref_views(f, sc)
         rec = {"meta_" + k: np.array(val) for k, val in c.items() if not isinstance(val, str)}
         rec["meta_view"] = np.array(c["view"])
-        for k in ("means3D", "scales", "rotations", "opacities", "shs", "viewmatrix", "projmatrix", "campos", "bg"):
-            rec["in_" + k] = getattr(sc_cpu, k).numpy()
+        inputs = golden_inputs.rasterize_inputs(name)
+        assert all(np.array_equal(inputs["gin_" + k], val.cpu().numpy()) for k, val in grads.items())
+        rec["inputs_digest"] = np.array(golden_inputs.digest(inputs))
         rec["in_tanfov"] = np.array([sc_cpu.tanfovx, sc_cpu.tanfovy], dtype=np.float64)
-        for k, val in extra.items():
-            rec["in_" + k] = val.numpy()
-        for k, val in grads.items():
-            rec["gin_" + k] = val.cpu().numpy()
         rec["num_rendered"] = np.array(f["num_rendered"])
         for k in ("color", "coord", "mcoord", "alpha", "normal", "depth", "mdepth", "radii"):
             rec["out_" + k] = f[k].cpu().numpy()

@@ -1,4 +1,4 @@
-"""Generate tests/golden/fused_*.npz from the REFERENCE'S OWN Python functions (run here, on CPU, where /root/reference exists).
+"""Generate tests/golden/fused_*.npz from the REFERENCE'S OWN Python functions (on CPU; the reference checkout beside the repository, or $RADE_GS_REFERENCE).
 
 Pins the widened rows (SURVEY.md 8f-1, 8f-2, 8f-4) to the reference itself instead of to restatements:
   fused_losses.npz     utils/loss_utils.py:17-18 `l1_loss`, :35-63 `ssim`, and train.py:163's combination; values + autograd gradients
@@ -26,7 +26,7 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("RADE_GS_REFERENCE") or os.path.join(os.path.dirname(ROOT), "reference")
 sys.path[:0] = [os.path.join(ROOT, "tests", "ref_stubs"), REF]
 torch.Tensor.cuda = lambda self, *a, **k: self            # noqa: E731  CPU run of code that says .cuda()
 torch.nn.Module.cuda = lambda self, *a, **k: self         # noqa: E731

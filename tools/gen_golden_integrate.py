@@ -1,7 +1,8 @@
 """Golden fixtures for `integrate_gaussians_to_points` (SURVEY.md 8f row 3) from the UNMODIFIED reference build.
 
-Must run where a GPU is:   gpurun -- python tools/gen_golden_integrate.py
-Outputs land in gpurun_out/golden/integrate_*.npz; copy them to tests/golden/ and commit them with this script.
+Must run where a GPU is:   python tools/gen_golden_integrate.py [OUT_DIR]
+Outputs land in OUT_DIR (default golden_out/) as integrate_*.npz; copy them to tests/golden/ and commit them with this script.
+The inputs are stored as a digest; tools/golden_inputs.py rebuilds them from the case's seed.
 
 The reference path has undefined behaviour outside a safe envelope, which the cases stay inside:
   * its `condition` tensor is allocated with PN (points) entries but indexed by Gaussian (rasterize_points.cu:318,
@@ -77,7 +78,7 @@ def main():
     import build_ref
     ref = build_ref.load()
     dev = torch.device("cuda:0")
-    out_dir = os.path.join(ROOT, "gpurun_out", "golden")
+    out_dir = sys.argv[1] if len(sys.argv) > 1 else "golden_out"
     os.makedirs(out_dir, exist_ok=True)
     for name, c in CASES.items():
         sc_cpu, pts_cpu = build_case(c)
@@ -91,10 +92,9 @@ def main():
             assert torch.equal(a, b), f"{name}: reference output {k} differs between two runs"
         rec = {"meta_" + k: np.array(v) for k, v in c.items() if not isinstance(v, str)}
         rec["meta_view"] = np.array(c["view"])
-        for k in ("means3D", "scales", "rotations", "opacities", "shs", "viewmatrix", "projmatrix", "campos", "bg"):
-            rec["in_" + k] = getattr(sc_cpu, k).numpy()
+        import golden_inputs
+        rec["inputs_digest"] = np.array(golden_inputs.digest(golden_inputs.integrate_inputs(name)))
         rec["in_tanfov"] = np.array([sc_cpu.tanfovx, sc_cpu.tanfovy], dtype=np.float64)
-        rec["in_points3D"] = pts_cpu.numpy()
         rec["num_rendered"] = np.array(r1[0])
         for k, a in zip(names, r1[1:7]):
             rec["out_" + k] = a.cpu().numpy()

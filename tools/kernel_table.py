@@ -1,5 +1,5 @@
 """Condense `ncu --metrics ... --csv` (tools/gpu_kernel_table.sh) into one row per kernel: the LAST captured launch of each
-(steady state), with its share of the step.  usage: python tools/kernel_table.py gpurun_out/kernel_table_C2.csv out.csv"""
+(steady state), with its share of the step.  usage: python tools/kernel_table.py kernel_table_C2.csv out.csv"""
 import collections
 import csv
 import re

@@ -1,5 +1,5 @@
 """Summarise an ncu report's SASS page: instructions executed grouped by opcode and the hottest SASS regions.
-usage: python tools/ncu_hot.py gpurun_out/prof_bwd.ncu-rep [top]"""
+usage: python tools/ncu_hot.py prof_bwd.ncu-rep [top]"""
 import collections
 import csv
 import subprocess

@@ -2,7 +2,7 @@
 counters"): reads the `ncu --csv` launch lists tools/gpu_r2_ncu.sh wrote for one rank's share of the step at each N and prints,
 per N, kernel time, DRAM bytes (dram__bytes_read.sum + dram__bytes_write.sum) and GB/s, and the step totals.
 
-    python tools/per_n_hbm.py gpurun_out/ncu_slab_C2_n{1,2,4,8}.csv > profiles/r02_ncu_hbm_per_n_C2.txt"""
+    python tools/per_n_hbm.py ncu_slab_C2_n{1,2,4,8}.csv > hbm_per_n_C2.txt"""
 import collections
 import csv
 import re

@@ -1,4 +1,4 @@
-"""Run the B200 path a few times on one config (for ncu captures and quick timing).  python tools/run_once.py [cfg] [iters]"""
+"""Run the path a few times on one config (for ncu captures and quick timing).  python tools/run_once.py [cfg] [iters]"""
 import os
 import sys
 

@@ -1,10 +1,11 @@
-"""SASS evidence: opcode histogram per kernel of librgs_b200.so (cuobjdump -sass), written to profiles/.
+"""SASS evidence: opcode histogram per kernel of librgs_b200.so (cuobjdump -sass).
 
-    python tools/sass_histogram.py > profiles/r02_sass_opcodes.txt
+    python tools/sass_histogram.py > sass_opcodes.txt
 
-Columns: the opcodes the design claims (LDGSTS = cp.async staging, FFMA2/FMUL2/FADD2 = packed fp32x2 blend arithmetic,
-RED/ATOM = gradient scatter, SHFL = warp reduce-scatter, MUFU = exp / rcp, BAR = CTA barriers) and the ones it must NOT contain
-on this path (UTMALDG / UTCMMA / LDTM = TMA / tcgen05: the north star rules tensor cores out, cp.async is the staging path)."""
+Columns: the opcodes the design claims (LDGSTS = cp.async staging, RED/ATOM = gradient scatter, SHFL = warp reduce-scatter,
+MUFU = exp / rcp, BAR = CTA barriers) and ones it must NOT contain: FFMA2/FMUL2/FADD2 (packed fp32x2) and UTCMMA / LDTM
+(tcgen05), which sm_90a does not have; UTMALDG (TMA), which Hopper has but this path does not use (records are staged with
+cp.async); HMMA (the north star rules tensor cores out)."""
 import collections
 import os
 import re
@@ -32,7 +33,7 @@ def main():
             op = m.group(1)
             cur["total"] += 1
             cur[op] += 1
-    print("SASS opcode histogram of librgs_b200.so (sm_100a), one row per kernel; static instruction counts")
+    print("SASS opcode histogram of librgs_b200.so (sm_90a), one row per kernel; static instruction counts")
     print(f"{'kernel':78s}" + "".join(f"{c:>8s}" for c in COLS))
     for name, c in kernels.items():
         if not name.startswith("rgs::"):
