@@ -274,6 +274,19 @@ int32_t rgs_normal_consistency(int32_t H, int32_t W, int32_t from_depth, float i
                                float w_expected, float w_median, double* loss_sum, float* d_normal, float* d_expected,
                                float* d_median, void* cuda_stream);
 
+/* ---- initial Gaussian scales: simple_knn's distCUDA2 (reference scene/gaussian_model.py:20, :315-316) ----
+ * points [P,3] (device, fp32) -> mean_dist2 [P] (device): the mean of the squared Euclidean distances from point i to its 3 nearest
+ * OTHER points, where "other" is decided by index (an exact duplicate of i is a neighbour at distance 0).  Exact in fp32: every pair
+ * distance is (dx*dx + dy*dy) + dz*dz with dx = p.x - q.x etc., each operation separately rounded (no FMA contraction), and the
+ * result is ((d0 + d1) + d2) / 3.0f with IEEE division over the three smallest values d0 <= d1 <= d2.  The result is therefore a pure
+ * function of the multiset of neighbour distances: independent of input order, traversal order and thread count.
+ * Fewer than 4 points: the mean over the P - 1 others (ascending sum / (P - 1)); a lone point gets 1.0.
+ * A point with a NaN or infinite coordinate is nobody's neighbour and gets NaN; the other rows are computed as if it were absent
+ * (including the small-cloud rule when fewer than 4 finite points remain).
+ * Scratch memory comes through `scratch` (about 60 bytes per point).  One stream synchronisation inside.  P == 0 returns 0 without
+ * any CUDA call; P < 0 or a NULL pointer with P > 0 returns RGS_E_INVALID. */
+int32_t rgs_knn_mean_dist2(int32_t P, const float* points, float* mean_dist2, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+
 /* Introspection for parity tests: views into the private buffers written by rgs_forward
  * (the reference keeps the same data at BinningState::point_list / ImageState::ranges,
  * rasterizer_impl.cu:237-250,224-235).  Pointers are device addresses inside the given buffers. */

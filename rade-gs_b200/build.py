@@ -22,7 +22,7 @@ LIB = os.path.join(HERE, "rade_gs_b200", "librgs_b200.so")
 GLUE = os.path.join(HERE, "diff_gaussian_rasterization", "_C.so")
 NVCC = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
 
-CORE_SOURCES = ["rgs_api.cu", "rgs_preprocess.cu", "rgs_binning.cu", "rgs_render_fwd.cu", "rgs_render_bwd.cu", "rgs_preprocess_bwd.cu", "rgs_activation.cu", "rgs_image_loss.cu", "rgs_integrate.cu", "rgs_exchange.cu"]
+CORE_SOURCES = ["rgs_api.cu", "rgs_preprocess.cu", "rgs_binning.cu", "rgs_render_fwd.cu", "rgs_render_bwd.cu", "rgs_preprocess_bwd.cu", "rgs_activation.cu", "rgs_image_loss.cu", "rgs_integrate.cu", "rgs_exchange.cu", "rgs_knn.cu"]
 HEADERS = ["rgs_common.cuh", "rgs_geom.cuh", "rgs_render_common.cuh", os.path.join(ROOT, "include", "rgs_b200.h")]
 # per-file extra flags: backward-preprocess is pure gradient arithmetic with a 1e-3 tolerance -> approximate float
 # division / sqrt (2-3 instructions instead of ~10 with a slow-path call); the eigen-solver inside it uses explicit IEEE

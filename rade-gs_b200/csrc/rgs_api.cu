@@ -535,6 +535,16 @@ int32_t rgs_compute_3d_filter(int32_t P, const float* xyz, int32_t n_cams, const
 	return after_launch();
 }
 
+int32_t rgs_knn_mean_dist2(int32_t P, const float* points, float* mean_dist2, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (P < 0) return fail(RGS_E_INVALID, "negative point count");
+	if (P == 0) return RGS_OK;
+	if (!points || !mean_dist2 || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = scratch(scratch_user, knn_scratch_bytes(P));
+	if (!buf) return fail(RGS_E_ALLOC, "knn scratch callback returned NULL");
+	const cudaError_t e = launch_knn_mean_dist2(P, points, mean_dist2, buf, (cudaStream_t)cuda_stream);
+	return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, std::string("knn: ") + cudaGetErrorString(e));
+}
+
 int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt, float* dmaps,
                                  double* sums, void* cuda_stream) {
 	if (planes < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");

@@ -287,6 +287,11 @@ size_t integrate_sort_temp_bytes(int PN);
 size_t integrate_mask_words(int64_t R, int tiles);
 void launch_integrate(const FwdParams& p, GeomView g, BinView b, ImgView img, const int* radii, IntegrateView v, IntegrateOut out, cudaStream_t s);
 
+// mean squared distance to the 3 nearest other points (rgs_knn.cu; simple_knn's distCUDA2).  One stream synchronisation
+// inside (the finite-point count sizes the tree); returns the first CUDA error.
+size_t knn_scratch_bytes(int P);
+cudaError_t launch_knn_mean_dist2(int P, const float* points, float* out, char* scratch, cudaStream_t s);
+
 // fused image-side losses (rgs_image_loss.cu; SURVEY.md 8f row 2)
 void launch_ssim_l1_forward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, float* dmaps, double* sums,
                             cudaStream_t s);

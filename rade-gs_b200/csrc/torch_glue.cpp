@@ -728,6 +728,22 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> NormalCon
 	return std::make_tuple(loss, dn, de.view(map_expected.sizes()), dm.view(map_median.sizes()));
 }
 
+// simple_knn's distCUDA2 (reference scene/gaussian_model.py:315-316): points [P,3] float32 on a CUDA device -> [P] float32,
+// the mean squared distance to the 3 nearest other points (rgs_knn_mean_dist2).  Non-contiguous input is accepted.
+torch::Tensor KnnMeanDist2(const torch::Tensor& points) {
+	TORCH_CHECK(points.dim() == 2 && points.size(1) == 3, "distCUDA2: points must have dimensions (num_points, 3), got ", points.sizes());
+	TORCH_CHECK(points.scalar_type() == torch::kFloat32, "distCUDA2: points must be float32, got ", points.scalar_type());
+	TORCH_CHECK(points.is_cuda(), "distCUDA2: points must be a CUDA tensor: no CPU path");
+	TORCH_CHECK(points.size(0) <= INT32_MAX, "distCUDA2: at most 2^31 - 1 points");
+	const c10::cuda::CUDAGuard guard(points.device());
+	const int P = (int)points.size(0);
+	torch::Tensor x = points.contiguous();
+	torch::Tensor out = new_empty({P}, x.options());
+	torch::Tensor scratch = torch::empty({0}, x.options().dtype(torch::kByte));
+	if (P) check(rgs_knn_mean_dist2(P, x.data_ptr<float>(), out.data_ptr<float>(), resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -759,6 +775,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("activate_forward", &ActivateForward);
 	m.def("activate_backward", &ActivateBackward);
 	m.def("densification_stats", &DensificationStats);
+	m.def("knn_mean_dist2", &KnnMeanDist2, py::arg("points"));
 	m.def("grad_stride", [](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });
