@@ -77,14 +77,22 @@ def ours_views(fwd: dict, sc) -> dict:
     b = _Cursor(fwd["binning"])
     point_list = b.take(R, torch.int32, 4)
     keys = b.take(R, torch.int64, 8)
+    # forward-render's ballots: word (chunk_base[tile] + k) * 8 + warp holds, for list positions [32k, 32k + 32) of the tile, the
+    # entries that warp's 8x4 pixel block did not cull (warp w covers tile columns 8 (w & 1) .. +7, rows 4 (w >> 1) .. +3)
+    hitmask = b.take((R // 32 + tiles + 1) * 8, torch.int32, 4)
     i = _Cursor(fwd["img"])
     ranges = i.take(tiles * 2, torch.int32, 4).view(tiles, 2)
     i.take(tiles, torch.int32, 4)   # tile_count (counted back down to zero by the scatter)
     totals = i.take(2, torch.int32, 4)
-    i.take(tiles, torch.int32, 4)   # chunk_base
+    chunk_base = i.take(tiles, torch.int32, 4)  # first 32-entry chunk of each tile's list, in hit-mask words / 8
     n_contrib = i.take(2 * N, torch.int32, 4).view(2, sc.height, sc.width)
+    accum_depth = i.take(N if depth else 0, torch.float32, 4).view(-1, sc.width)
+    normal_length = i.take(N if (coord or depth) else 0, torch.float32, 4).view(-1, sc.width)
+    accum_coord = i.take(3 * N if coord else 0, torch.float32, 4).view(-1, sc.height, sc.width)
     return dict(totals=totals, records=rec, depths=depths, tiles_touched=tiles_touched, offsets=offsets, clamped=clamped, point_list=point_list,
-                keys=keys, ranges=ranges, n_contrib=n_contrib,
+                keys=keys, hitmask=hitmask, ranges=ranges, chunk_base=chunk_base, n_contrib=n_contrib,
+                accum_depth=(accum_depth if depth else None), normal_length=(normal_length if (coord or depth) else None),
+                accum_coord=(accum_coord if coord else None),
                 means2D=rec[:, 0:2], conic_opacity=torch.stack([rec[:, 2], rec[:, 3], rec[:, 4], rec[:, 5]], 1), ts=rec[:, 11],
                 ray_planes=rec[:, 6:8], rgb=rec[:, 8:11], normals=rec[:, 12:15],
                 camera_planes=(torch.cat([rec[:, 19:24], rec[:, 15:16]], 1) if coord else None),
