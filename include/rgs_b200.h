@@ -39,7 +39,8 @@ typedef enum rgs_status {
 	RGS_E_INVALID = -1,      /* bad argument (shape/flag combination the reference rejects)            */
 	RGS_E_CUDA = -2,         /* CUDA runtime error (message in rgs_last_error)                         */
 	RGS_E_UNSUPPORTED = -3,  /* e.g. prefiltered=true (mis-wired in the reference, SURVEY app. A-15)    */
-	RGS_E_ALLOC = -4         /* a resize callback returned NULL                                        */
+	RGS_E_ALLOC = -4,        /* a resize callback returned NULL                                        */
+	RGS_E_CAPACITY = -5      /* rgs_tsdf_touch: the frame-local hash is full; grow it and call again     */
 } rgs_status;
 
 /* Resize callback: make the buffer at least `bytes` long and return its device address.
@@ -286,6 +287,123 @@ int32_t rgs_normal_consistency(int32_t H, int32_t W, int32_t from_depth, float i
  * Scratch memory comes through `scratch` (about 60 bytes per point).  One stream synchronisation inside.  P == 0 returns 0 without
  * any CUDA call; P < 0 or a NULL pointer with P > 0 returns RGS_E_INVALID. */
 int32_t rgs_knn_mean_dist2(int32_t P, const float* points, float* mean_dist2, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+
+/* ---- TSDF fusion and marching cubes on a sparse voxel-block grid (reference mesh_extract.py:66-105, there Open3D's
+ * VoxelBlockGrid on the CPU) ----
+ * Every value the functions below store is fixed bit for bit by this contract; every arithmetic step is one IEEE fp32
+ * operation rounded on its own (no FMA contraction), in the order written.  Open3D's own rules (pixel rounding, image-border
+ * test, touch shape, triangle table) are not known here: where this contract chooses, it says so; bit parity with Open3D is
+ * not a goal.
+ *
+ * Grid.  Voxels form blocks of 16^3 (RGS_TSDF_BLOCK_RES; no other resolution).  Grid point g = 16 * block + local (integer
+ * vectors, 0 <= local < 16) sits at the world point (float)g_k * voxel_size per component k.  Inside a block the voxels are
+ * stored x fastest: v = x + 16 y + 256 z, so a pool seen as [capacity, 16, 16, 16, C] is indexed [block, z, y, x, c].
+ * A block key packs the block coordinate with 21 bits per axis: key = (bx + 2^20) << 42 | (by + 2^20) << 21 | (bz + 2^20),
+ * -2^20 <= b < 2^20, so ascending keys are ascending (bx, by, bz).  The hash is open addressing with linear probing over
+ * `hash_slots` (a power of two); a free slot holds key RGS_TSDF_EMPTY_KEY and value -1.  Blocks are never freed.
+ *
+ * Camera (rgs_tsdf_camera).  The caller converts its parameters to fp32 once: fx, fy, cx, cy and the world->camera
+ * extrinsic [R | t] (R row-major).  trunc = trunc_voxel_multiplier * voxel_size (one fp32 product).  A call whose camera
+ * centre c = -R^T t (evaluated in double) has some c_k +- (depth_max + trunc) outside the key range (blocks
+ * [-2^20 + 1, 2^20 - 2]) returns RGS_E_INVALID; a pixel whose touched blocks would still leave the range (very wide fields
+ * of view) touches nothing, so keys never wrap and every grid point is an exact fp32 integer times voxel_size.
+ *
+ * Touch (rgs_tsdf_touch; Open3D compute_unique_block_coordinates).  Pixel (i, j) (column, row) is valid when
+ * 0 < d <= depth_max, d = depth[j, i] / depth_scale.  Its ray through the pixel centre: xn = ((i + 0.5) - cx) / fx,
+ * yn = ((j + 0.5) - cy) / fy; for z in {d - trunc, d + trunc} the camera point is (xn * z, yn * z, z), q = p_c - t and
+ * p_w,k = (R_0k q.x + R_1k q.y) + R_2k q.z; its block coordinate is floor(p_w,k / (16 * voxel_size)).  Every block of the
+ * axis-aligned box spanned by the two block coordinates is touched (a box, not a DDA walk; with the default multiplier 8 at
+ * most 2 x 2 x 2).  The result is the set of touched blocks in ascending key order.
+ *
+ * Integrate (rgs_tsdf_integrate; Open3D integrate).  The given blocks are inserted first (a new block's voxels are the
+ * zeros the caller filled the pools with).  Then each voxel of those blocks, at p = g * voxel_size, is updated by exactly
+ * one thread, so the grid does not depend on scheduling, block order or duplicate coordinates:
+ *   x_c = ((R_00 p.x + R_01 p.y) + R_02 p.z) + t_0 (likewise y_c, z_c);  u = (fx * x_c) / z_c + cx,  v = (fy * y_c) / z_c + cy;
+ *   pixel (floor u, floor v), accepted iff it lies in [0, W) x [0, H) (chosen: the pixel whose square contains (u, v));
+ *   skipped when z_c <= 0, the pixel is not accepted, d <= 0, d > depth_max or sdf = d - z_c < -trunc;
+ *   otherwise obs = min(sdf, trunc) / trunc, tsdf <- (w * tsdf + obs) / (w + 1), each colour channel
+ *   col <- (w * col + c) / (w + 1) with c the float colour as given, then w <- w + 1.
+ *
+ * Extract (rgs_tsdf_extract; Open3D extract_triangle_mesh).  A voxel is valid when it is allocated and w >= weight_threshold;
+ * it is inside when tsdf < 0 (0 is outside).  The cell at g (corners g + {0,1}^3, corner c = cx + 2 cy + 4 cz, case bit c set
+ * when corner c is inside) emits triangles iff its 8 corners are valid.  Edge e of a cell runs along axis a = e / 4 from the
+ * corner offset by (e & 1, e >> 1 & 1) on the other two axes in ascending axis order; its vertex belongs to grid point
+ * g + offset, and the vertex of (g, a) sits at g * voxel_size with component a advanced: g_a * vs + t * vs,
+ * t = f0 / (f0 - f1), colour c0 + t * (c1 - c0) (0: g, 1: g + e_a).  A vertex exists iff an emitted triangle uses it.
+ * Triangle table, derived by rule (rgs_tsdf.cu, constexpr): on each cube face the sign-change edges are joined by segments
+ * (on a face whose diagonal corners share a sign, each inside corner is cut off by its own segment); every segment is
+ * directed so that direction x (outward face normal) points to the inside corner of its first edge; the directed segments
+ * form closed loops; each loop is walked from its lowest-numbered edge e0 -> e1 -> ... and fanned as (e0, e_k, e_k+1).  The
+ * right-hand normal of every triangle then points toward increasing tsdf, and two cells agree on their shared face, so the
+ * mesh over fully valid cells is watertight.  Order: active blocks by key; vertices by (block, voxel, axis); triangles by
+ * (block, voxel, table order).  The mesh is therefore the same bits for every run and every grid capacity.
+ *
+ * Normals (rgs_tsdf_vertex_normals; Open3D compute_vertex_normals).  n_f = (v1 - v0) x (v2 - v0), each component
+ * a.y * b.z - a.z * b.y etc. rounded per operation; each vertex sums n_f over its triangles in ascending triangle index from
+ * (0, 0, 0), then n / sqrtf((n.x n.x + n.y n.y) + n.z n.z) (IEEE sqrt and division); a zero length gives (0, 0, 0).
+ *
+ * Memory.  The library allocates nothing persistent: the caller owns every array of rgs_tsdf_grid and grows it on the host.
+ * counters[0] = allocated blocks, counters[1] = blocks of the last touch, counters[2] = RGS_TSDF_* flags (sticky).  Growth:
+ * allocate pools of twice the capacity (old contents copied to the front, the rest zero), a new hash (all free), call
+ * rgs_tsdf_rehash, keep the counters.  rgs_tsdf_touch's read of the counters (the one host read per view) returns the
+ * allocated count: a caller that keeps allocated + blocks passed to integrate <= capacity never overflows.  A block that
+ * finds no slot is skipped and sets RGS_TSDF_OVERFLOW, which every later call that reads the counters reports. */
+#define RGS_TSDF_BLOCK_RES 16
+#define RGS_TSDF_EMPTY_KEY 0xffffffffffffffffull
+#define RGS_TSDF_OVERFLOW 1          /* counters[2]: a block found no pool slot (grid state incomplete) */
+#define RGS_TSDF_BAD_COORD 2         /* counters[2]: integrate got a block coordinate outside the key range */
+typedef struct rgs_tsdf_grid {
+	float voxel_size;
+	int64_t capacity;           /* blocks the pools hold                                                              */
+	int64_t hash_slots;         /* power of two, >= 2 * capacity                                                      */
+	uint64_t* hash_keys;        /* [hash_slots]                                                                       */
+	int32_t* hash_values;       /* [hash_slots] pool index of the block                                               */
+	float* tsdf;                /* [capacity * 4096]                                                                  */
+	float* weight;              /* [capacity * 4096]                                                                  */
+	float* color;               /* [capacity * 4096 * 3]                                                              */
+	int32_t* stamps;            /* [capacity] last integrate call that claimed the block (start at 0)                 */
+	int64_t frame_slots;        /* power of two: touch's frame-local hash                                             */
+	uint64_t* frame_keys;       /* [frame_slots]                                                                      */
+	uint64_t* frame_list;       /* [frame_slots / 2]                                                                  */
+	int32_t* counters;          /* [4] see above                                                                      */
+} rgs_tsdf_grid;
+
+typedef struct rgs_tsdf_camera {
+	int32_t width, height;
+	float fx, fy, cx, cy;
+	float R[9];                 /* world -> camera rotation, row-major */
+	float t[3];
+	float depth_scale, depth_max, trunc_voxel_multiplier;
+} rgs_tsdf_camera;
+
+/* depth [H, W] fp32.  Writes the touched blocks in ascending key order to block_coords (int32 [frame_slots / 2, 3]) and
+ * returns their count, or RGS_E_CAPACITY / another negative status.  allocated (host, may be NULL) receives counters[0].
+ * Scratch through `scratch`.  One stream synchronisation inside. */
+int64_t rgs_tsdf_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, const float* depth, int32_t* block_coords, int64_t* allocated,
+                       rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+/* block_coords int32 [n, 3] (device), depth [H, W], color [H, W, 3] fp32.  call_id > 0, different for every call on the
+ * grid.  Scratch through `scratch`.  No host synchronisation. */
+int32_t rgs_tsdf_integrate(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, int64_t n, const int32_t* block_coords, const float* depth,
+                           const float* color, int32_t call_id, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+/* Inserts every allocated block of the old hash into grid's (empty) hash with its pool index. */
+int32_t rgs_tsdf_rehash(const rgs_tsdf_grid* grid, const uint64_t* old_keys, const int32_t* old_values, int64_t old_slots, void* cuda_stream);
+/* Active blocks in ascending key order: keys and pool indices (capacity entries each).  Returns the count.  One stream
+ * synchronisation inside. */
+int64_t rgs_tsdf_active_blocks(const rgs_tsdf_grid* grid, uint64_t* keys, int32_t* pool_index, rgs_resize_fn scratch, void* scratch_user,
+                               void* cuda_stream);
+/* Marching cubes.  The outputs come through `resize` with these user pointers: vertices fp32 [V, 3], colors fp32 [V, 3],
+ * triangles int32 [F, 3]; V and F are written to num_vertices / num_triangles (host).  Two stream synchronisations inside. */
+typedef struct rgs_tsdf_mesh_out {
+	void* vertices_user;
+	void* colors_user;
+	void* triangles_user;
+	int64_t num_vertices, num_triangles;
+} rgs_tsdf_mesh_out;
+int32_t rgs_tsdf_extract(const rgs_tsdf_grid* grid, float weight_threshold, rgs_resize_fn resize, rgs_tsdf_mesh_out* out, void* scratch_user,
+                         void* cuda_stream);
+/* normals fp32 [V, 3] of any mesh (triangle indices must lie in [0, V)).  Scratch through `scratch`. */
+int32_t rgs_tsdf_vertex_normals(int64_t V, const float* vertices, int64_t F, const int32_t* triangles, float* normals, rgs_resize_fn scratch,
+                                void* scratch_user, void* cuda_stream);
 
 /* Introspection for parity tests: views into the private buffers written by rgs_forward
  * (the reference keeps the same data at BinningState::point_list / ImageState::ranges,

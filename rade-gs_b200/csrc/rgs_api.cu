@@ -4,6 +4,7 @@
 // BinningState / ImageState chunk allocator (reference: cuda_rasterizer/rasterizer_impl.cu:190-250,
 // 254-425, 429-571, 176-188; cuda_rasterizer/rasterizer_impl.h:22-94).
 #include <atomic>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -531,6 +532,162 @@ int32_t rgs_knn_mean_dist2(int32_t P, const float* points, float* mean_dist2, rg
 	if (!buf) return fail(RGS_E_ALLOC, "knn scratch callback returned NULL");
 	const cudaError_t e = launch_knn_mean_dist2(P, points, mean_dist2, buf, (cudaStream_t)cuda_stream);
 	return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, std::string("knn: ") + cudaGetErrorString(e));
+}
+
+// ---- TSDF grid (rgs_tsdf.cu) ----
+
+static bool pow2(int64_t n) { return n > 0 && (n & (n - 1)) == 0; }
+static bool finite_pos(float x) { return std::isfinite(x) && x > 0.0f; }
+
+static int tsdf_grid_check(const rgs_tsdf_grid* g) {
+	if (!g) return fail(RGS_E_INVALID, "null grid");
+	if (!finite_pos(g->voxel_size)) return fail(RGS_E_INVALID, "voxel_size must be positive and finite");
+	if (g->capacity <= 0 || g->capacity > (INT32_MAX / (RGS_TSDF_BLOCK_RES * RGS_TSDF_BLOCK_RES * RGS_TSDF_BLOCK_RES)))
+		return fail(RGS_E_INVALID, "grid capacity must be in [1, 524287] blocks");
+	if (!pow2(g->hash_slots) || g->hash_slots < 2 * g->capacity) return fail(RGS_E_INVALID, "hash_slots must be a power of two >= 2 * capacity");
+	if (!pow2(g->frame_slots) || g->frame_slots < 2 || g->frame_slots > ((int64_t)1 << 31))
+		return fail(RGS_E_INVALID, "frame_slots must be a power of two in [2, 2^31]");
+	if (!g->hash_keys || !g->hash_values || !g->tsdf || !g->weight || !g->color || !g->stamps || !g->frame_keys || !g->frame_list || !g->counters)
+		return fail(RGS_E_INVALID, "null grid array");
+	return RGS_OK;
+}
+
+static int tsdf_camera_check(const rgs_tsdf_grid* g, const rgs_tsdf_camera* c) {
+	if (!c) return fail(RGS_E_INVALID, "null camera");
+	if (c->width <= 0 || c->height <= 0) return fail(RGS_E_INVALID, "image size must be positive");
+	if (!std::isfinite(c->fx) || !std::isfinite(c->fy) || c->fx == 0.0f || c->fy == 0.0f || !std::isfinite(c->cx) || !std::isfinite(c->cy))
+		return fail(RGS_E_INVALID, "intrinsics must be finite with nonzero focal lengths");
+	for (int i = 0; i < 9; i++)
+		if (!std::isfinite(c->R[i])) return fail(RGS_E_INVALID, "extrinsic must be finite");
+	for (int i = 0; i < 3; i++)
+		if (!std::isfinite(c->t[i])) return fail(RGS_E_INVALID, "extrinsic must be finite");
+	if (!finite_pos(c->depth_scale) || !finite_pos(c->depth_max) || !finite_pos(c->trunc_voxel_multiplier))
+		return fail(RGS_E_INVALID, "depth_scale, depth_max and trunc_voxel_multiplier must be positive and finite");
+	// camera centre +- (depth_max + trunc) must stay inside the block-key range (the keys must never wrap)
+	const double reach = (double)c->depth_max + (double)c->trunc_voxel_multiplier * (double)g->voxel_size;
+	const double bs = (double)g->voxel_size * RGS_TSDF_BLOCK_RES;
+	for (int k = 0; k < 3; k++) {
+		const double ck = -((double)c->R[k] * c->t[0] + (double)c->R[3 + k] * c->t[1] + (double)c->R[6 + k] * c->t[2]);
+		const double lo = std::floor((ck - reach) / bs), hi = std::floor((ck + reach) / bs);
+		if (!(lo >= -(1 << 20) + 1 && hi <= (1 << 20) - 2))
+			return fail(RGS_E_INVALID, "camera out of the grid's key range: centre +- (depth_max + trunc) must lie within 2^20 - 2 blocks of the origin");
+	}
+	return RGS_OK;
+}
+
+// counters[0..3] to the host; fails when an earlier call left the grid incomplete
+static int tsdf_read_counters(const rgs_tsdf_grid* g, int32_t* cnt, cudaStream_t s) {
+	cudaError_t e = cudaMemcpyAsync(cnt, g->counters, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+	if (e != cudaSuccess) return fail(RGS_E_CUDA, std::string("tsdf: ") + cudaGetErrorString(e));
+	return RGS_OK;
+}
+
+static int tsdf_flags_check(const int32_t* cnt) {
+	if (cnt[2] & RGS_TSDF_BAD_COORD) return fail(RGS_E_INVALID, "tsdf: an integrate call was given a block coordinate outside [-2^20, 2^20)");
+	if (cnt[2] & RGS_TSDF_OVERFLOW) return fail(RGS_E_INVALID, "tsdf: an integrate call found no free block slot; the grid is incomplete");
+	return RGS_OK;
+}
+
+static int tsdf_cuda(cudaError_t e, const char* what) {
+	return e == cudaSuccess ? (int)RGS_OK : fail(RGS_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+}
+
+int64_t rgs_tsdf_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, const float* depth, int32_t* block_coords, int64_t* allocated,
+                       rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc == RGS_OK) rc = tsdf_camera_check(grid, cam);
+	if (rc != RGS_OK) return rc;
+	if (!depth || !block_coords || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int32_t cnt[4];
+	if ((rc = tsdf_cuda(launch_tsdf_touch(*grid, *cam, depth, cnt, s), "tsdf touch")) != RGS_OK) return rc;
+	if ((rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
+	if (allocated) *allocated = cnt[0];
+	if (cnt[3] || cnt[1] > grid->frame_slots / 2) return fail(RGS_E_CAPACITY, "tsdf touch: more blocks than the frame-local hash holds");
+	const int64_t n = cnt[1];
+	if (n == 0) return 0;
+	char* buf = scratch(scratch_user, tsdf_touch_scratch_bytes(n));
+	if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
+	if ((rc = tsdf_cuda(launch_tsdf_touch_sort(*grid, n, block_coords, buf, s), "tsdf touch")) != RGS_OK) return rc;
+	return n;
+}
+
+int32_t rgs_tsdf_integrate(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, int64_t n, const int32_t* block_coords, const float* depth,
+                           const float* color, int32_t call_id, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc == RGS_OK) rc = tsdf_camera_check(grid, cam);
+	if (rc != RGS_OK) return rc;
+	if (n < 0 || n > INT32_MAX) return fail(RGS_E_INVALID, "block count out of range");
+	if (call_id <= 0) return fail(RGS_E_INVALID, "call_id must be positive");
+	if (n == 0) return RGS_OK;
+	if (!block_coords || !depth || !color || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = scratch(scratch_user, (size_t)n * sizeof(int32_t));
+	if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
+	return tsdf_cuda(launch_tsdf_integrate(*grid, *cam, n, block_coords, depth, color, call_id, reinterpret_cast<int32_t*>(buf), (cudaStream_t)cuda_stream),
+	                 "tsdf integrate");
+}
+
+int32_t rgs_tsdf_rehash(const rgs_tsdf_grid* grid, const uint64_t* old_keys, const int32_t* old_values, int64_t old_slots, void* cuda_stream) {
+	const int rc = tsdf_grid_check(grid);
+	if (rc != RGS_OK) return rc;
+	if (old_slots < 0) return fail(RGS_E_INVALID, "negative slot count");
+	if (old_slots == 0) return RGS_OK;
+	if (!old_keys || !old_values) return fail(RGS_E_INVALID, "null pointer");
+	return tsdf_cuda(launch_tsdf_rehash(*grid, old_keys, old_values, old_slots, (cudaStream_t)cuda_stream), "tsdf rehash");
+}
+
+int64_t rgs_tsdf_active_blocks(const rgs_tsdf_grid* grid, uint64_t* keys, int32_t* pool_index, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc != RGS_OK) return rc;
+	if (!keys || !pool_index || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int32_t cnt[4];
+	if ((rc = tsdf_read_counters(grid, cnt, s)) != RGS_OK || (rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
+	const int N = cnt[0];
+	if (N == 0) return 0;
+	char* buf = scratch(scratch_user, tsdf_active_scratch_bytes(N));
+	if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
+	if ((rc = tsdf_cuda(launch_tsdf_active(*grid, N, keys, pool_index, buf, s), "tsdf active blocks")) != RGS_OK) return rc;
+	return N;
+}
+
+int32_t rgs_tsdf_extract(const rgs_tsdf_grid* grid, float weight_threshold, rgs_resize_fn resize, rgs_tsdf_mesh_out* out, void* scratch_user,
+                         void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc != RGS_OK) return rc;
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	if (std::isnan(weight_threshold)) return fail(RGS_E_INVALID, "weight_threshold is NaN");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int32_t cnt[4];
+	if ((rc = tsdf_read_counters(grid, cnt, s)) != RGS_OK || (rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
+	const int N = cnt[0];
+	int64_t totals[2] = {0, 0};
+	char* buf = nullptr;
+	if (N > 0) {
+		buf = resize(scratch_user, tsdf_extract_scratch_bytes(*grid, N));
+		if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
+		if ((rc = tsdf_cuda(launch_tsdf_extract_count(*grid, N, weight_threshold, buf, totals, s), "tsdf extract")) != RGS_OK) return rc;
+	}
+	out->num_vertices = totals[0];
+	out->num_triangles = totals[1];
+	char* v = resize(out->vertices_user, (size_t)totals[0] * 3 * sizeof(float));
+	char* c = resize(out->colors_user, (size_t)totals[0] * 3 * sizeof(float));
+	char* t = resize(out->triangles_user, (size_t)totals[1] * 3 * sizeof(int32_t));
+	if ((totals[0] > 0 && (!v || !c)) || (totals[1] > 0 && !t)) return fail(RGS_E_ALLOC, "tsdf mesh callback returned NULL");
+	if (N == 0) return RGS_OK;
+	return tsdf_cuda(launch_tsdf_extract_emit(*grid, N, buf, reinterpret_cast<float*>(v), reinterpret_cast<float*>(c), reinterpret_cast<int32_t*>(t), s),
+	                 "tsdf extract");
+}
+
+int32_t rgs_tsdf_vertex_normals(int64_t V, const float* vertices, int64_t F, const int32_t* triangles, float* normals, rgs_resize_fn scratch,
+                                void* scratch_user, void* cuda_stream) {
+	if (V < 0 || F < 0 || V > INT32_MAX || 3 * F > INT32_MAX) return fail(RGS_E_INVALID, "vertex / triangle count out of range");
+	if (V == 0) return F == 0 ? (int32_t)RGS_OK : fail(RGS_E_INVALID, "triangles without vertices");
+	if (!vertices || !normals || !scratch || (F > 0 && !triangles)) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = scratch(scratch_user, tsdf_normals_scratch_bytes(V, F));
+	if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
+	return tsdf_cuda(launch_tsdf_normals(V, vertices, F, triangles, normals, buf, (cudaStream_t)cuda_stream), "tsdf vertex normals");
 }
 
 int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt, float* dmaps,

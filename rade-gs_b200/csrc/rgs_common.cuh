@@ -282,6 +282,21 @@ void launch_integrate(const FwdParams& p, GeomView g, BinView b, ImgView img, co
 size_t knn_scratch_bytes(int P);
 cudaError_t launch_knn_mean_dist2(int P, const float* points, float* out, char* scratch, cudaStream_t s);
 
+// TSDF fusion and marching cubes (rgs_tsdf.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
+size_t tsdf_touch_scratch_bytes(int64_t n);
+cudaError_t launch_tsdf_touch(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c, const float* depth, int32_t* counters_host, cudaStream_t s);
+cudaError_t launch_tsdf_touch_sort(const rgs_tsdf_grid& g, int64_t n, int32_t* out, char* scratch, cudaStream_t s);
+cudaError_t launch_tsdf_integrate(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c, int64_t n, const int32_t* bc, const float* depth, const float* color,
+                                  int32_t call_id, int32_t* slot, cudaStream_t s);
+cudaError_t launch_tsdf_rehash(const rgs_tsdf_grid& g, const uint64_t* old_keys, const int32_t* old_vals, int64_t old_slots, cudaStream_t s);
+size_t tsdf_active_scratch_bytes(int N);
+cudaError_t launch_tsdf_active(const rgs_tsdf_grid& g, int N, uint64_t* keys, int32_t* pools, char* scratch, cudaStream_t s);
+size_t tsdf_extract_scratch_bytes(const rgs_tsdf_grid& g, int N);
+cudaError_t launch_tsdf_extract_count(const rgs_tsdf_grid& g, int N, float thr, char* scratch, int64_t* totals_host, cudaStream_t s);
+cudaError_t launch_tsdf_extract_emit(const rgs_tsdf_grid& g, int N, char* scratch, float* verts, float* colors, int32_t* tris, cudaStream_t s);
+size_t tsdf_normals_scratch_bytes(int64_t V, int64_t F);
+cudaError_t launch_tsdf_normals(int64_t V, const float* verts, int64_t F, const int32_t* tris, float* normals, char* scratch, cudaStream_t s);
+
 // fused image-side losses (rgs_image_loss.cu; SURVEY.md 8f row 2)
 void launch_ssim_l1_forward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, float* dmaps, double* sums,
                             cudaStream_t s);

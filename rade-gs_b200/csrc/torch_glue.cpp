@@ -691,6 +691,161 @@ torch::Tensor KnnMeanDist2(const torch::Tensor& points) {
 	return out;
 }
 
+// ---- TSDF voxel-block grid (rgs_tsdf_*; Python side rade_gs_b200.tsdf.VoxelBlockGrid, which owns every array) ----------------
+
+torch::Tensor grid_array(const py::object& grid, const char* name, torch::ScalarType type) {
+	torch::Tensor t = grid.attr(name).cast<torch::Tensor>();
+	TORCH_CHECK(t.is_cuda() && t.scalar_type() == type && t.is_contiguous(), "VoxelBlockGrid.", name, " must be a contiguous CUDA ", type, " tensor");
+	return t;
+}
+
+// the C view of the grid; the Python object keeps the tensors alive
+rgs_tsdf_grid tsdf_grid(const py::object& grid) {
+	rgs_tsdf_grid g;
+	torch::Tensor keys = grid_array(grid, "hash_keys", torch::kInt64), frame = grid_array(grid, "frame_keys", torch::kInt64);
+	g.voxel_size = grid.attr("voxel_size").cast<float>();
+	g.capacity = grid_array(grid, "stamps", torch::kInt32).numel();
+	g.hash_slots = keys.numel();
+	g.hash_keys = reinterpret_cast<uint64_t*>(keys.data_ptr<int64_t>());
+	g.hash_values = grid_array(grid, "hash_values", torch::kInt32).data_ptr<int32_t>();
+	g.tsdf = grid_array(grid, "tsdf", torch::kFloat32).data_ptr<float>();
+	g.weight = grid_array(grid, "weight", torch::kFloat32).data_ptr<float>();
+	g.color = grid_array(grid, "color", torch::kFloat32).data_ptr<float>();
+	g.stamps = grid_array(grid, "stamps", torch::kInt32).data_ptr<int32_t>();
+	g.frame_slots = frame.numel();
+	g.frame_keys = reinterpret_cast<uint64_t*>(frame.data_ptr<int64_t>());
+	g.frame_list = reinterpret_cast<uint64_t*>(grid_array(grid, "frame_list", torch::kInt64).data_ptr<int64_t>());
+	g.counters = grid_array(grid, "counters", torch::kInt32).data_ptr<int32_t>();
+	return g;
+}
+
+// a per-view image on the grid's device: float32, contiguous, [H, W] (depth) or [H, W, 3] (colour)
+torch::Tensor tsdf_image(const torch::Tensor& t, const torch::Tensor& like, const char* name, int channels) {
+	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
+	TORCH_CHECK(t.device() == like.device(), name, " must be on the grid's device");
+	TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32, got ", t.scalar_type());
+	TORCH_CHECK(channels == 1 ? t.dim() == 2 : (t.dim() == 3 && t.size(2) == channels), name, channels == 1 ? " must be [H, W]" : " must be [H, W, 3]",
+	            ", got ", t.sizes());
+	TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
+	return t;
+}
+
+// intrinsic [3,3] and extrinsic [4,4] as CPU float64 tensors -> the fp32 camera of the contract (one conversion, here)
+rgs_tsdf_camera tsdf_camera(const torch::Tensor& depth, const torch::Tensor& intrinsic, const torch::Tensor& extrinsic, double depth_scale, double depth_max,
+                            double trunc_voxel_multiplier) {
+	TORCH_CHECK(intrinsic.device().is_cpu() && intrinsic.scalar_type() == torch::kFloat64 && intrinsic.numel() == 9, "intrinsic must be a 3x3 matrix");
+	TORCH_CHECK(extrinsic.device().is_cpu() && extrinsic.scalar_type() == torch::kFloat64 && extrinsic.numel() == 16, "extrinsic must be a 4x4 matrix");
+	const torch::Tensor K = intrinsic.contiguous(), E = extrinsic.contiguous();
+	const double* k = K.data_ptr<double>();
+	const double* e = E.data_ptr<double>();
+	rgs_tsdf_camera c;
+	c.height = (int32_t)depth.size(0);
+	c.width = (int32_t)depth.size(1);
+	c.fx = (float)k[0];
+	c.fy = (float)k[4];
+	c.cx = (float)k[2];
+	c.cy = (float)k[5];
+	for (int r = 0; r < 3; r++) {
+		for (int q = 0; q < 3; q++) c.R[3 * r + q] = (float)e[4 * r + q];
+		c.t[r] = (float)e[4 * r + 3];
+	}
+	c.depth_scale = (float)depth_scale;
+	c.depth_max = (float)depth_max;
+	c.trunc_voxel_multiplier = (float)trunc_voxel_multiplier;
+	return c;
+}
+
+torch::Tensor tsdf_scratch(const torch::Tensor& like) { return torch::empty({0}, like.options().dtype(torch::kByte)); }
+
+// returns (number of touched blocks, or -1 when the frame-local hash is full; block coordinates int32 [n, 3]; allocated blocks)
+std::tuple<int64_t, torch::Tensor, int64_t> TsdfTouch(const py::object& grid, const torch::Tensor& depth, const torch::Tensor& intrinsic,
+                                                      const torch::Tensor& extrinsic, double depth_scale, double depth_max, double trunc_voxel_multiplier) {
+	const torch::Tensor keys = grid_array(grid, "hash_keys", torch::kInt64);
+	const c10::cuda::CUDAGuard guard(keys.device());
+	const torch::Tensor d = tsdf_image(depth, keys, "depth", 1);
+	const rgs_tsdf_grid g = tsdf_grid(grid);
+	const rgs_tsdf_camera c = tsdf_camera(d, intrinsic, extrinsic, depth_scale, depth_max, trunc_voxel_multiplier);
+	torch::Tensor out = torch::empty({g.frame_slots / 2, 3}, keys.options().dtype(torch::kInt32)), scratch = tsdf_scratch(keys);
+	int64_t allocated = 0;
+	const int64_t n = rgs_tsdf_touch(&g, &c, d.data_ptr<float>(), out.data_ptr<int32_t>(), &allocated, resize_cb, &scratch,
+	                                 at::cuda::getCurrentCUDAStream().stream());
+	if (n == RGS_E_CAPACITY) return std::make_tuple((int64_t)-1, out.narrow(0, 0, 0), allocated);
+	check(n);
+	return std::make_tuple(n, out.narrow(0, 0, n).clone(), allocated);
+}
+
+void TsdfIntegrate(const py::object& grid, const torch::Tensor& block_coords, const torch::Tensor& depth, const torch::Tensor& color,
+                   const torch::Tensor& intrinsic, const torch::Tensor& extrinsic, double depth_scale, double depth_max, double trunc_voxel_multiplier,
+                   int call_id) {
+	const torch::Tensor keys = grid_array(grid, "hash_keys", torch::kInt64);
+	const c10::cuda::CUDAGuard guard(keys.device());
+	TORCH_CHECK(block_coords.is_cuda() && block_coords.device() == keys.device(), "block_coords must be a CUDA tensor on the grid's device");
+	TORCH_CHECK(block_coords.scalar_type() == torch::kInt32 && block_coords.dim() == 2 && block_coords.size(1) == 3,
+	            "block_coords must be int32 [N, 3], got ", block_coords.scalar_type(), " ", block_coords.sizes());
+	TORCH_CHECK(block_coords.is_contiguous(), "block_coords must be contiguous");
+	const torch::Tensor d = tsdf_image(depth, keys, "depth", 1), col = tsdf_image(color, keys, "color", 3);
+	TORCH_CHECK(col.size(0) == d.size(0) && col.size(1) == d.size(1), "color and depth must have the same [H, W]");
+	const rgs_tsdf_grid g = tsdf_grid(grid);
+	const rgs_tsdf_camera c = tsdf_camera(d, intrinsic, extrinsic, depth_scale, depth_max, trunc_voxel_multiplier);
+	torch::Tensor scratch = tsdf_scratch(keys);
+	check(rgs_tsdf_integrate(&g, &c, block_coords.size(0), block_coords.data_ptr<int32_t>(), d.data_ptr<float>(), col.data_ptr<float>(), call_id, resize_cb,
+	                         &scratch, at::cuda::getCurrentCUDAStream().stream()));
+}
+
+void TsdfRehash(const py::object& grid, const torch::Tensor& old_keys, const torch::Tensor& old_values) {
+	const torch::Tensor keys = grid_array(grid, "hash_keys", torch::kInt64);
+	const c10::cuda::CUDAGuard guard(keys.device());
+	TORCH_CHECK(old_keys.is_cuda() && old_values.is_cuda() && old_keys.scalar_type() == torch::kInt64 && old_values.scalar_type() == torch::kInt32 &&
+	                old_keys.is_contiguous() && old_values.is_contiguous() && old_keys.numel() == old_values.numel(),
+	            "old hash must be contiguous CUDA int64 keys and int32 values of one length");
+	const rgs_tsdf_grid g = tsdf_grid(grid);
+	check(rgs_tsdf_rehash(&g, reinterpret_cast<const uint64_t*>(old_keys.data_ptr<int64_t>()), old_values.data_ptr<int32_t>(), old_keys.numel(),
+	                      at::cuda::getCurrentCUDAStream().stream()));
+}
+
+// returns (keys int64 [N] ascending, pool indices int32 [N])
+std::tuple<torch::Tensor, torch::Tensor> TsdfActiveBlocks(const py::object& grid) {
+	const torch::Tensor hk = grid_array(grid, "hash_keys", torch::kInt64);
+	const c10::cuda::CUDAGuard guard(hk.device());
+	const rgs_tsdf_grid g = tsdf_grid(grid);
+	torch::Tensor keys = torch::empty({g.capacity}, hk.options()), pools = torch::empty({g.capacity}, hk.options().dtype(torch::kInt32)),
+	              scratch = tsdf_scratch(hk);
+	const int64_t n = rgs_tsdf_active_blocks(&g, reinterpret_cast<uint64_t*>(keys.data_ptr<int64_t>()), pools.data_ptr<int32_t>(), resize_cb, &scratch,
+	                                         at::cuda::getCurrentCUDAStream().stream());
+	check(n);
+	return std::make_tuple(keys.narrow(0, 0, n), pools.narrow(0, 0, n));
+}
+
+// returns (vertices f32 [V,3], colors f32 [V,3], triangles int32 [F,3])
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> TsdfExtract(const py::object& grid, double weight_threshold) {
+	const torch::Tensor hk = grid_array(grid, "hash_keys", torch::kInt64);
+	const c10::cuda::CUDAGuard guard(hk.device());
+	const rgs_tsdf_grid g = tsdf_grid(grid);
+	torch::Tensor v = tsdf_scratch(hk), c = tsdf_scratch(hk), t = tsdf_scratch(hk), scratch = tsdf_scratch(hk);
+	rgs_tsdf_mesh_out out{&v, &c, &t, 0, 0};
+	check(rgs_tsdf_extract(&g, (float)weight_threshold, resize_cb, &out, &scratch, at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(v.view(torch::kFloat32).view({out.num_vertices, 3}), c.view(torch::kFloat32).view({out.num_vertices, 3}),
+	                       t.view(torch::kInt32).view({out.num_triangles, 3}));
+}
+
+torch::Tensor TsdfVertexNormals(const torch::Tensor& vertices, const torch::Tensor& triangles) {
+	TORCH_CHECK(vertices.is_cuda() && triangles.is_cuda() && vertices.device() == triangles.device(), "vertices / triangles must be CUDA tensors on one device");
+	TORCH_CHECK(vertices.scalar_type() == torch::kFloat32 && vertices.dim() == 2 && vertices.size(1) == 3 && vertices.is_contiguous(),
+	            "vertices must be contiguous float32 [V, 3]");
+	TORCH_CHECK(triangles.scalar_type() == torch::kInt32 && triangles.dim() == 2 && triangles.size(1) == 3 && triangles.is_contiguous(),
+	            "triangles must be contiguous int32 [F, 3]");
+	const c10::cuda::CUDAGuard guard(vertices.device());
+	const int64_t V = vertices.size(0), F = triangles.size(0);
+	if (F > 0) {
+		const auto mm = torch::aminmax(triangles);
+		TORCH_CHECK(std::get<0>(mm).item<int32_t>() >= 0 && std::get<1>(mm).item<int32_t>() < V, "triangle vertex index out of [0, V)");
+	}
+	torch::Tensor normals = new_empty({V, 3}, vertices.options()), scratch = tsdf_scratch(vertices);
+	check(rgs_tsdf_vertex_normals(V, vertices.data_ptr<float>(), F, triangles.data_ptr<int32_t>(), normals.data_ptr<float>(), resize_cb, &scratch,
+	                              at::cuda::getCurrentCUDAStream().stream()));
+	return normals;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -762,6 +917,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("activate_backward", &ActivateBackward);
 	m.def("densification_stats", &DensificationStats);
 	m.def("knn_mean_dist2", &KnnMeanDist2, py::arg("points"));
+	m.def("tsdf_touch", &TsdfTouch);
+	m.def("tsdf_integrate", &TsdfIntegrate);
+	m.def("tsdf_rehash", &TsdfRehash);
+	m.def("tsdf_active_blocks", &TsdfActiveBlocks);
+	m.def("tsdf_extract", &TsdfExtract);
+	m.def("tsdf_vertex_normals", &TsdfVertexNormals);
 	m.def("grad_stride", [](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });

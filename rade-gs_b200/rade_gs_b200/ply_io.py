@@ -150,3 +150,40 @@ def load_gaussian_ply(path: str, max_sh_degree: Optional[int] = None) -> Dict[st
         "filter_3D": f32(p["filter_3D"]).reshape(P, 1) if "filter_3D" in p else np.zeros((P, 1), np.float32),
         "sh_degree": deg,
     }
+
+
+def save_triangle_mesh_ply(path: str, vertices, triangles, vertex_colors=None, vertex_normals=None) -> None:
+    """Binary little-endian PLY of a triangle mesh (what ``o3d.io.write_triangle_mesh`` writes for mesh_extract.py's
+    ``recon.ply``): element ``vertex`` with float x y z nx ny nz and uchar red green blue, element ``face`` with
+    ``list uchar int vertex_indices``.  Colours in [0, 1] become floor(255 * clamp(c, 0, 1) + 0.5); absent normals or
+    colours are written as zeros.  Arrays may be numpy or torch (any device)."""
+    def arr(a, dtype):
+        if hasattr(a, "detach"):
+            a = a.detach().cpu().numpy()
+        return np.asarray(a, dtype=dtype)
+
+    v = arr(vertices, np.float32).reshape(-1, 3)
+    t = arr(triangles, np.int32).reshape(-1, 3)
+    V, Fn = len(v), len(t)
+    n = np.zeros((V, 3), np.float32) if vertex_normals is None or len(vertex_normals) == 0 else arr(vertex_normals, np.float32).reshape(V, 3)
+    c = np.zeros((V, 3), np.float64) if vertex_colors is None or len(vertex_colors) == 0 else arr(vertex_colors, np.float64).reshape(V, 3)
+    rgb = np.floor(255.0 * np.clip(c, 0.0, 1.0) + 0.5).astype(np.uint8)
+    vrec = np.empty(V, dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4"), ("red", "u1"), ("green", "u1"), ("blue", "u1")])
+    for k, name in enumerate(("x", "y", "z")):
+        vrec[name] = v[:, k]
+    for k, name in enumerate(("nx", "ny", "nz")):
+        vrec[name] = n[:, k]
+    for k, name in enumerate(("red", "green", "blue")):
+        vrec[name] = rgb[:, k]
+    frec = np.empty(Fn, dtype=[("n", "u1"), ("i", "<i4", (3,))])
+    frec["n"] = 3
+    frec["i"] = t
+    header = ["ply", "format binary_little_endian 1.0", f"element vertex {V}"] + [f"property float {a}" for a in ("x", "y", "z", "nx", "ny", "nz")]
+    header += [f"property uchar {a}" for a in ("red", "green", "blue")] + [f"element face {Fn}", "property list uchar int vertex_indices", "end_header"]
+    d = os.path.dirname(path)
+    if d:
+        os.makedirs(d, exist_ok=True)
+    with open(path, "wb") as f:
+        f.write(("\n".join(header) + "\n").encode("ascii"))
+        f.write(vrec.tobytes())
+        f.write(frec.tobytes())
