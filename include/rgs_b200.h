@@ -405,6 +405,64 @@ int32_t rgs_tsdf_extract(const rgs_tsdf_grid* grid, float weight_threshold, rgs_
 int32_t rgs_tsdf_vertex_normals(int64_t V, const float* vertices, int64_t F, const int32_t* triangles, float* normals, rgs_resize_fn scratch,
                                 void* scratch_user, void* cuda_stream);
 
+/* ---- DTU evaluation: the chamfer distances of dtu_eval/eval.py and the mask culling of evaluate_dtu_mesh.py:82-138 ----
+ * All arithmetic is IEEE fp64 with every operation rounded on its own (no FMA contraction), in the order written; a - b is
+ * one rounded subtraction.  Points are fp64 [N, 3] on the device, row-major.  The squared pair distance is
+ * d2(p, q) = (dx*dx + dy*dy) + dz*dz with dx = p.x - q.x etc., and a distance is sqrt(d2) (IEEE sqrt); this is the value
+ * scikit-learn's kd-tree reports for the same pair.  Point counts are at most 2^31 - 1.  A non-finite coordinate in a cloud
+ * handed to rgs_dtu_radius_downsample or rgs_dtu_nearest returns RGS_E_INVALID (scikit-learn's fit rejects it too). */
+
+/* Surface sampling (eval.py:54-71, sample_single_tri).  faces int32 [F, 3] index vertices fp64 [V, 3].  Per triangle, with
+ * e1 = v1 - v0, e2 = v2 - v0: l1 = sqrt((e1.x^2 + e1.y^2) + e1.z^2) (likewise l2); the cross product c = e1 x e2 with
+ * c.x = e1.y*e2.z - e1.z*e2.y, c.y = e1.z*e2.x - e1.x*e2.z, c.z = e1.x*e2.y - e1.y*e2.x; area2 = |c| as for l1.  A triangle
+ * is sampled iff area2 > 0 (a NaN area is not).  thr = density * sqrt((l1 * l2) / area2), n1 = floor(l1 / thr),
+ * n2 = floor(l2 / thr); for i = 0..n1 (outer), j = 0..n2 (inner), c0 = (i + 0.5) / max(n1, 1e-7), c1 = (j + 0.5) /
+ * max(n2, 1e-7), the point q = (e1 * c0 + e2 * c1) + v0 (per component) is emitted iff c0 + c1 < 1.  The output is the V
+ * vertices in order followed by the samples in triangle order: fp64 [V + S, 3] through resize(out->points_user, bytes).
+ * Scratch comes through resize(out->scratch_user) (about 32 bytes per face) and resize(out->rows_user) (16 bytes per sampled
+ * row).  One host read (the totals) before anything is sized by the totals; V + S > 2^31 - 1, a face index outside [0, V)
+ * or a non-finite n1 / n2 returns RGS_E_INVALID before the output is requested.  num_points receives V + S.  A triangle is
+ * counted by one thread in O(rows + columns) steps; the points themselves are written one thread each. */
+typedef struct rgs_dtu_samples_out {
+	void* points_user;
+	void* scratch_user;
+	void* rows_user;
+	int64_t num_points;
+} rgs_dtu_samples_out;
+int32_t rgs_dtu_sample_mesh(int64_t V, const double* vertices, int64_t F, const int32_t* faces, double density, rgs_resize_fn resize,
+                            rgs_dtu_samples_out* out, void* cuda_stream);
+
+/* Radius downsample (eval.py:80-94).  points fp64 [N, 3] in their processing order (the reference's shuffled order).
+ * kept[i] (uint8) = 1 iff point i lies within `radius` (d2 <= radius * radius, the product rounded once) of no kept point
+ * j < i: the greedy, lexicographically first maximal independent set in index order, which is what the reference's loop
+ * over radius_neighbors computes.  The result does not depend on thread count or scheduling.  radius must be positive and
+ * finite.  Scratch through `scratch` (about 200 bytes per point).  One host read per round; rounds (host, may be NULL)
+ * receives their number: at most the length of the longest chain of neighbours with increasing index, polylogarithmic in N
+ * for a random order. */
+int32_t rgs_dtu_radius_downsample(int64_t N, const double* points, double radius, uint8_t* kept, int32_t* rounds, rgs_resize_fn scratch,
+                                  void* scratch_user, void* cuda_stream);
+
+/* Exact 1-NN distances (eval.py:118-134, kneighbors(n_neighbors=1)).  For each query q: dist = sqrt(min_p d2(q, p)) over
+ * the M reference points, and index = the index of a reference point attaining it (which one among ties is unspecified).
+ * M >= 1 (an empty reference set returns RGS_E_INVALID); N may be 0.  Scratch through `scratch` (about 90 bytes per
+ * reference point and 24 per query).  One host read (the bounds). */
+int32_t rgs_dtu_nearest(int64_t M, const double* reference, int64_t N, const double* query, double* dist, int64_t* index, rgs_resize_fn scratch,
+                        void* scratch_user, void* cuda_stream);
+
+/* Mask dilation (evaluate_dtu_mesh.py:120-122, skimage binary_dilation(mask, disk(6))).  masks uint8 [n_views, H, W]
+ * (nonzero = set) -> dilated uint8 [n_views, H, W]: 1 iff a set pixel lies at (dx, dy) with dx^2 + dy^2 <= 36 (113 pixels);
+ * pixels outside the image are unset.  No host synchronisation. */
+int32_t rgs_dtu_dilate_masks(int32_t n_views, int32_t H, int32_t W, const uint8_t* masks, uint8_t* dilated, void* cuda_stream);
+
+/* Vertex culling (evaluate_dtu_mesh.py:82-133).  proj fp64 [n_views, 3, 4] holds rows 0..2 of K @ w2c per view, with K the
+ * reference's 4x4 intrinsic (fx, fy, W / 2, H / 2) and w2c its world_view_transform.T.  Per vertex and view:
+ * c_r = ((P_r0 x + P_r1 y) + P_r2 z) + P_r3; u = (c_0 / (c_2 + 1e-6)) / (W - 1), v likewise with H - 1; gx = (u - 0.5) * 2,
+ * gy = (v - 0.5) * 2.  The view is passed when not (-1 < gx < 1 and -1 < gy < 1); otherwise the dilated mask is read at
+ * column rint(((gx + 1) / 2) * (W - 1)), row rint(((gy + 1) / 2) * (H - 1)) (grid_sample nearest with align_corners, ties
+ * to even) and the view is passed iff it is set.  keep uint8 [V] = 1 iff every view is passed.  No host synchronisation. */
+int32_t rgs_dtu_cull_vertices(int64_t V, const double* vertices, int32_t n_views, int32_t H, int32_t W, const double* proj, const uint8_t* dilated,
+                              uint8_t* keep, void* cuda_stream);
+
 /* Introspection for parity tests: views into the private buffers written by rgs_forward
  * (the reference keeps the same data at BinningState::point_list / ImageState::ranges,
  * rasterizer_impl.cu:237-250,224-235).  Pointers are device addresses inside the given buffers. */

@@ -690,6 +690,73 @@ int32_t rgs_tsdf_vertex_normals(int64_t V, const float* vertices, int64_t F, con
 	return tsdf_cuda(launch_tsdf_normals(V, vertices, F, triangles, normals, buf, (cudaStream_t)cuda_stream), "tsdf vertex normals");
 }
 
+// ---- DTU evaluation (rgs_dtu_eval.cu) ----
+
+static int dtu_cuda(cudaError_t e, const char* what) {
+	if (e == cudaErrorInvalidValue) return fail(RGS_E_INVALID, std::string(what) + ": a point has a NaN or infinite coordinate");
+	return e == cudaSuccess ? (int)RGS_OK : fail(RGS_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+}
+
+int32_t rgs_dtu_sample_mesh(int64_t V, const double* vertices, int64_t F, const int32_t* faces, double density, rgs_resize_fn resize,
+                            rgs_dtu_samples_out* out, void* cuda_stream) {
+	if (V < 0 || F < 0 || V > INT32_MAX || F > INT32_MAX - 1) return fail(RGS_E_INVALID, "dtu sample: vertex / face count out of range");
+	if (!resize || !out || (V > 0 && !vertices) || (F > 0 && !faces)) return fail(RGS_E_INVALID, "null pointer");
+	if (!(std::isfinite(density) && density > 0.0)) return fail(RGS_E_INVALID, "dtu sample: density must be positive and finite");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int64_t totals[2] = {0, 0};   // samples, rows
+	char* buf = nullptr;
+	if (F > 0) {
+		if (V == 0) return fail(RGS_E_INVALID, "dtu sample: faces without vertices");
+		buf = resize(out->scratch_user, dtu_sample_scratch_bytes(F));
+		if (!buf) return fail(RGS_E_ALLOC, "dtu sample scratch callback returned NULL");
+		const cudaError_t e = launch_dtu_sample_count(V, vertices, F, faces, density, buf, totals, s);
+		if (e != cudaSuccess) return fail(RGS_E_CUDA, std::string("dtu sample: ") + cudaGetErrorString(e));
+		if (V + totals[0] > INT32_MAX)
+			return fail(RGS_E_INVALID, "dtu sample: more than 2^31 - 1 points (or a face index outside [0, V), or a triangle whose sample count is not finite)");
+	}
+	out->num_points = V + totals[0];
+	char* rows = totals[0] > 0 ? resize(out->rows_user, dtu_sample_rows_bytes(totals[1])) : nullptr;
+	char* pts = resize(out->points_user, (size_t)out->num_points * 3 * sizeof(double));
+	if ((totals[0] > 0 && !rows) || (out->num_points > 0 && !pts)) return fail(RGS_E_ALLOC, "dtu sample callback returned NULL");
+	if (out->num_points == 0) return RGS_OK;
+	return dtu_cuda(launch_dtu_sample_emit(V, vertices, F, faces, density, buf, totals[0], totals[1], rows, reinterpret_cast<double*>(pts), s), "dtu sample");
+}
+
+int32_t rgs_dtu_radius_downsample(int64_t N, const double* points, double radius, uint8_t* kept, int32_t* rounds, rgs_resize_fn scratch,
+                                  void* scratch_user, void* cuda_stream) {
+	if (rounds) *rounds = 0;
+	if (N < 0 || N > INT32_MAX) return fail(RGS_E_INVALID, "dtu downsample: point count out of range");
+	if (!(std::isfinite(radius) && radius > 0.0)) return fail(RGS_E_INVALID, "dtu downsample: radius must be positive and finite");
+	if (N == 0) return RGS_OK;
+	if (!points || !kept || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = scratch(scratch_user, dtu_downsample_scratch_bytes((int)N));
+	if (!buf) return fail(RGS_E_ALLOC, "dtu downsample scratch callback returned NULL");
+	return dtu_cuda(launch_dtu_downsample((int)N, points, radius, kept, buf, rounds, (cudaStream_t)cuda_stream), "dtu downsample");
+}
+
+int32_t rgs_dtu_nearest(int64_t M, const double* reference, int64_t N, const double* query, double* dist, int64_t* index, rgs_resize_fn scratch,
+                        void* scratch_user, void* cuda_stream) {
+	if (M < 0 || N < 0 || M > INT32_MAX || N > INT32_MAX) return fail(RGS_E_INVALID, "dtu nearest: point count out of range");
+	if (M == 0) return fail(RGS_E_INVALID, "dtu nearest: the reference set is empty");
+	if (!reference || !scratch || (N > 0 && (!query || !dist || !index))) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = scratch(scratch_user, dtu_nearest_scratch_bytes((int)M, (int)N));
+	if (!buf) return fail(RGS_E_ALLOC, "dtu nearest scratch callback returned NULL");
+	return dtu_cuda(launch_dtu_nearest((int)M, reference, (int)N, query, dist, index, buf, (cudaStream_t)cuda_stream), "dtu nearest");
+}
+
+int32_t rgs_dtu_dilate_masks(int32_t n_views, int32_t H, int32_t W, const uint8_t* masks, uint8_t* dilated, void* cuda_stream) {
+	if (n_views < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "dtu dilate: image size must be positive");
+	if (n_views > 0 && (!masks || !dilated)) return fail(RGS_E_INVALID, "null pointer");
+	return dtu_cuda(launch_dtu_dilate(n_views, H, W, masks, dilated, (cudaStream_t)cuda_stream), "dtu dilate");
+}
+
+int32_t rgs_dtu_cull_vertices(int64_t V, const double* vertices, int32_t n_views, int32_t H, int32_t W, const double* proj, const uint8_t* dilated,
+                              uint8_t* keep, void* cuda_stream) {
+	if (V < 0 || n_views < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "dtu cull: negative count or empty image");
+	if (V > 0 && (!vertices || !keep || (n_views > 0 && (!proj || !dilated)))) return fail(RGS_E_INVALID, "null pointer");
+	return dtu_cuda(launch_dtu_cull(V, vertices, n_views, H, W, proj, dilated, keep, (cudaStream_t)cuda_stream), "dtu cull");
+}
+
 int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt, float* dmaps,
                                  double* sums, void* cuda_stream) {
 	if (planes < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");

@@ -297,6 +297,21 @@ cudaError_t launch_tsdf_extract_emit(const rgs_tsdf_grid& g, int N, char* scratc
 size_t tsdf_normals_scratch_bytes(int64_t V, int64_t F);
 cudaError_t launch_tsdf_normals(int64_t V, const float* verts, int64_t F, const int32_t* tris, float* normals, char* scratch, cudaStream_t s);
 
+// DTU evaluation (rgs_dtu_eval.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
+size_t dtu_sample_scratch_bytes(int64_t F);
+cudaError_t launch_dtu_sample_count(int64_t V, const double* verts, int64_t F, const int32_t* faces, double density, char* scratch, int64_t* totals_host,
+                                    cudaStream_t s);
+size_t dtu_sample_rows_bytes(int64_t R);
+cudaError_t launch_dtu_sample_emit(int64_t V, const double* verts, int64_t F, const int32_t* faces, double density, char* scratch, int64_t S, int64_t R,
+                                   char* rows_scratch, double* out, cudaStream_t s);
+size_t dtu_downsample_scratch_bytes(int N);
+cudaError_t launch_dtu_downsample(int N, const double* pts, double radius, uint8_t* kept, char* scratch, int32_t* rounds, cudaStream_t s);
+size_t dtu_nearest_scratch_bytes(int M, int N);
+cudaError_t launch_dtu_nearest(int M, const double* ref, int N, const double* query, double* dist, int64_t* index, char* scratch, cudaStream_t s);
+cudaError_t launch_dtu_dilate(int n_views, int H, int W, const uint8_t* masks, uint8_t* out, cudaStream_t s);
+cudaError_t launch_dtu_cull(int64_t V, const double* verts, int n_views, int H, int W, const double* proj, const uint8_t* masks, uint8_t* keep,
+                            cudaStream_t s);
+
 // fused image-side losses (rgs_image_loss.cu; SURVEY.md 8f row 2)
 void launch_ssim_l1_forward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, float* dmaps, double* sums,
                             cudaStream_t s);

@@ -846,6 +846,82 @@ torch::Tensor TsdfVertexNormals(const torch::Tensor& vertices, const torch::Tens
 	return normals;
 }
 
+// ---- DTU evaluation (rgs_dtu_*; Python side rade_gs_b200.dtu_eval) -------------------------------------------------------
+
+torch::Tensor dtu_points(const torch::Tensor& t, const char* name) {
+	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
+	TORCH_CHECK(t.scalar_type() == torch::kFloat64 && t.dim() == 2 && t.size(1) == 3, name, " must be float64 [N, 3], got ", t.scalar_type(), " ",
+	            t.sizes());
+	return t.contiguous();
+}
+
+torch::Tensor dtu_bytes(const torch::Tensor& like) { return torch::empty({0}, like.options().dtype(torch::kByte)); }
+
+// vertices f64 [V,3], faces int32 [F,3] -> the vertices followed by the surface samples, f64 [V + S, 3]
+torch::Tensor DtuSampleMesh(const torch::Tensor& vertices, const torch::Tensor& faces, double density) {
+	const torch::Tensor v = dtu_points(vertices, "vertices");
+	TORCH_CHECK(faces.is_cuda() && faces.device() == v.device(), "faces must be a CUDA tensor on the vertices' device");
+	TORCH_CHECK(faces.scalar_type() == torch::kInt32 && faces.dim() == 2 && faces.size(1) == 3, "faces must be int32 [F, 3], got ", faces.scalar_type(), " ",
+	            faces.sizes());
+	const c10::cuda::CUDAGuard guard(v.device());
+	const torch::Tensor f = faces.contiguous();
+	torch::Tensor pts = dtu_bytes(v), scratch = dtu_bytes(v), rows = dtu_bytes(v);
+	rgs_dtu_samples_out out{&pts, &scratch, &rows, 0};
+	check(rgs_dtu_sample_mesh(v.size(0), v.data_ptr<double>(), f.size(0), f.data_ptr<int32_t>(), density, resize_cb, &out,
+	                          at::cuda::getCurrentCUDAStream().stream()));
+	return pts.view(torch::kFloat64).view({out.num_points, 3});
+}
+
+// points f64 [N,3] in processing order -> (kept bool [N], rounds)
+std::tuple<torch::Tensor, int32_t> DtuRadiusDownsample(const torch::Tensor& points, double radius) {
+	const torch::Tensor p = dtu_points(points, "points");
+	const c10::cuda::CUDAGuard guard(p.device());
+	torch::Tensor kept = new_empty({p.size(0)}, p.options().dtype(torch::kBool)), scratch = dtu_bytes(p);
+	int32_t rounds = 0;
+	check(rgs_dtu_radius_downsample(p.size(0), p.data_ptr<double>(), radius, reinterpret_cast<uint8_t*>(kept.data_ptr<bool>()), &rounds, resize_cb, &scratch,
+	                                at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(kept, rounds);
+}
+
+// reference f64 [M,3], query f64 [N,3] -> (distance f64 [N], index int64 [N])
+std::tuple<torch::Tensor, torch::Tensor> DtuNearest(const torch::Tensor& reference, const torch::Tensor& query) {
+	const torch::Tensor r = dtu_points(reference, "reference"), q = dtu_points(query, "query");
+	TORCH_CHECK(r.device() == q.device(), "reference and query must be on one device");
+	const c10::cuda::CUDAGuard guard(r.device());
+	torch::Tensor dist = new_empty({q.size(0)}, q.options()), index = new_empty({q.size(0)}, q.options().dtype(torch::kInt64)), scratch = dtu_bytes(r);
+	check(rgs_dtu_nearest(r.size(0), r.data_ptr<double>(), q.size(0), q.data_ptr<double>(), dist.data_ptr<double>(), index.data_ptr<int64_t>(), resize_cb,
+	                      &scratch, at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(dist, index);
+}
+
+// masks uint8 [n, H, W] (nonzero = set) -> disk(6) dilation, uint8 [n, H, W]
+torch::Tensor DtuDilateMasks(const torch::Tensor& masks) {
+	TORCH_CHECK(masks.is_cuda() && masks.scalar_type() == torch::kUInt8 && masks.dim() == 3, "masks must be a CUDA uint8 [n, H, W] tensor");
+	const c10::cuda::CUDAGuard guard(masks.device());
+	const torch::Tensor m = masks.contiguous();
+	torch::Tensor out = new_empty(m.sizes(), m.options());
+	check(rgs_dtu_dilate_masks((int32_t)m.size(0), (int32_t)m.size(1), (int32_t)m.size(2), m.data_ptr<uint8_t>(), out.data_ptr<uint8_t>(),
+	                           at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
+// vertices f64 [V,3], proj f64 [n,3,4], dilated uint8 [n,H,W] -> keep bool [V]
+torch::Tensor DtuCullVertices(const torch::Tensor& vertices, const torch::Tensor& proj, const torch::Tensor& dilated) {
+	const torch::Tensor v = dtu_points(vertices, "vertices");
+	TORCH_CHECK(proj.is_cuda() && proj.device() == v.device() && proj.scalar_type() == torch::kFloat64 && proj.dim() == 3 && proj.size(1) == 3 &&
+	                proj.size(2) == 4,
+	            "proj must be a CUDA float64 [n, 3, 4] tensor on the vertices' device");
+	TORCH_CHECK(dilated.is_cuda() && dilated.device() == v.device() && dilated.scalar_type() == torch::kUInt8 && dilated.dim() == 3 &&
+	                dilated.size(0) == proj.size(0),
+	            "dilated must be a CUDA uint8 [n, H, W] tensor with one mask per view");
+	const c10::cuda::CUDAGuard guard(v.device());
+	const torch::Tensor P = proj.contiguous(), m = dilated.contiguous();
+	torch::Tensor keep = new_empty({v.size(0)}, v.options().dtype(torch::kBool));
+	check(rgs_dtu_cull_vertices(v.size(0), v.data_ptr<double>(), (int32_t)P.size(0), (int32_t)m.size(1), (int32_t)m.size(2), P.data_ptr<double>(),
+	                            m.data_ptr<uint8_t>(), reinterpret_cast<uint8_t*>(keep.data_ptr<bool>()), at::cuda::getCurrentCUDAStream().stream()));
+	return keep;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -923,6 +999,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("tsdf_active_blocks", &TsdfActiveBlocks);
 	m.def("tsdf_extract", &TsdfExtract);
 	m.def("tsdf_vertex_normals", &TsdfVertexNormals);
+	m.def("dtu_sample_mesh", &DtuSampleMesh, py::arg("vertices"), py::arg("faces"), py::arg("density"));
+	m.def("dtu_radius_downsample", &DtuRadiusDownsample, py::arg("points"), py::arg("radius"));
+	m.def("dtu_nearest", &DtuNearest, py::arg("reference"), py::arg("query"));
+	m.def("dtu_dilate_masks", &DtuDilateMasks, py::arg("masks"));
+	m.def("dtu_cull_vertices", &DtuCullVertices, py::arg("vertices"), py::arg("proj"), py::arg("dilated"));
 	m.def("grad_stride", [](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });

@@ -152,6 +152,186 @@ def load_gaussian_ply(path: str, max_sh_degree: Optional[int] = None) -> Dict[st
     }
 
 
+def _read_header(f, path):
+    """(format, elements): each element {"name", "count", "props": [(name, type) or (name, (count type, item type))]}."""
+    if f.readline().strip() != b"ply":
+        raise ValueError(f"{path}: not a PLY file")
+    fmt, elements = None, []
+    while True:
+        line = f.readline()
+        if not line:
+            raise ValueError(f"{path}: unterminated PLY header")
+        tok = line.decode("ascii", "replace").split()
+        if not tok or tok[0] in ("comment", "obj_info"):
+            continue
+        if tok[0] == "format":
+            fmt = tok[1]
+        elif tok[0] == "element":
+            elements.append({"name": tok[1], "count": int(tok[2]), "props": []})
+        elif tok[0] == "property":
+            if not elements:
+                raise ValueError(f"{path}: property before any element")
+            if tok[1] == "list":
+                if tok[2] not in _PLY_TYPES or tok[3] not in _PLY_TYPES:
+                    raise ValueError(f"{path}: unknown PLY list type {tok[2]} {tok[3]}")
+                elements[-1]["props"].append((tok[4], (_PLY_TYPES[tok[2]], _PLY_TYPES[tok[3]])))
+            else:
+                if tok[1] not in _PLY_TYPES:
+                    raise ValueError(f"{path}: unknown PLY type {tok[1]}")
+                elements[-1]["props"].append((tok[2], _PLY_TYPES[tok[1]]))
+        elif tok[0] == "end_header":
+            break
+    if fmt not in ("binary_little_endian", "binary_big_endian", "ascii"):
+        raise ValueError(f"{path}: unsupported PLY format {fmt}")
+    return fmt, elements
+
+
+def _binary_element(buf, off, el, order, path):
+    """Reads one element at byte offset `off`: (dict name -> array, new offset).  A list property becomes an [count, k]
+    array when every row holds k items, else a list of arrays."""
+    props, n = el["props"], el["count"]
+    lists = [p for p in props if isinstance(p[1], tuple)]
+    if not lists or n == 0:
+        dt = np.dtype([(name, order + (t if not isinstance(t, tuple) else t[0])) for name, t in props]) if not lists else None
+        if dt is None:
+            return {name: np.zeros((0, 0)) for name, _ in props}, off
+        if off + dt.itemsize * n > len(buf):
+            raise ValueError(f"{path}: truncated {el['name']} data")
+        rec = np.frombuffer(buf, dtype=dt, count=n, offset=off)
+        return {name: np.ascontiguousarray(rec[name]) for name, _ in props}, off + dt.itemsize * n
+    # the first row's list lengths, then a fixed-size read if every row has them
+    fields, o = [], off
+    for name, t in props:
+        if isinstance(t, tuple):
+            k = int(np.frombuffer(buf, dtype=order + t[0], count=1, offset=o)[0])
+            o += np.dtype(t[0]).itemsize + k * np.dtype(t[1]).itemsize
+            fields += [(name + "\0n", order + t[0]), (name, order + t[1], (k,))]
+        else:
+            o += np.dtype(t).itemsize
+            fields.append((name, order + t))
+    dt = np.dtype(fields)
+    if off + dt.itemsize * n <= len(buf):
+        rec = np.frombuffer(buf, dtype=dt, count=n, offset=off)
+        if all((rec[name + "\0n"] == rec[name + "\0n"][0]).all() for name, _ in lists):
+            return {name: np.ascontiguousarray(rec[name]) for name, _ in props}, off + dt.itemsize * n
+    out = {name: [] for name, _ in props}   # rows of different lengths
+    for _ in range(n):
+        for name, t in props:
+            if isinstance(t, tuple):
+                k = int(np.frombuffer(buf, dtype=order + t[0], count=1, offset=off)[0])
+                off += np.dtype(t[0]).itemsize
+                out[name].append(np.frombuffer(buf, dtype=order + t[1], count=k, offset=off).copy())
+                off += k * np.dtype(t[1]).itemsize
+            else:
+                out[name].append(np.frombuffer(buf, dtype=order + t, count=1, offset=off)[0])
+                off += np.dtype(t).itemsize
+    return out, off
+
+
+def _ascii_element(tokens, pos, el, path):
+    props, n = el["props"], el["count"]
+    if not any(isinstance(t, tuple) for _, t in props):
+        k = len(props)
+        if pos + k * n > len(tokens):
+            raise ValueError(f"{path}: truncated {el['name']} data")
+        a = np.array(tokens[pos:pos + k * n], dtype=np.float64).reshape(n, k)
+        return {name: a[:, i] for i, (name, _) in enumerate(props)}, pos + k * n
+    out = {name: [] for name, _ in props}
+    for _ in range(n):
+        for name, t in props:
+            if isinstance(t, tuple):
+                k = int(tokens[pos])
+                out[name].append(np.array(tokens[pos + 1:pos + 1 + k], dtype=np.int64))
+                pos += 1 + k
+            else:
+                out[name].append(float(tokens[pos]))
+                pos += 1
+    return out, pos
+
+
+def _read_elements(path: str, wanted):
+    """The properties of the named elements of a PLY file (ascii or binary, either byte order); others are skipped."""
+    with open(path, "rb") as f:
+        fmt, elements = _read_header(f, path)
+        buf = f.read()
+    found = {}
+    if fmt == "ascii":
+        tokens, pos = buf.split(), 0
+        for el in elements:
+            data, pos = _ascii_element(tokens, pos, el, path)
+            found[el["name"]] = data
+            if all(w in found for w in wanted):
+                break
+    else:
+        order, off = ("<" if fmt == "binary_little_endian" else ">"), 0
+        for el in elements:
+            data, off = _binary_element(buf, off, el, order, path)
+            found[el["name"]] = data
+            if all(w in found for w in wanted):
+                break
+    return found
+
+
+def _xyz(found, path) -> np.ndarray:
+    v = found.get("vertex")
+    if v is None or not all(k in v for k in ("x", "y", "z")):
+        raise ValueError(f"{path}: no vertex element with x, y and z")
+    return np.stack([np.asarray(v[k], dtype=np.float64) for k in ("x", "y", "z")], axis=1).reshape(-1, 3)
+
+
+def load_point_cloud_ply(path: str) -> np.ndarray:
+    """The x y z of the ``vertex`` element as float64 [N, 3] (what ``o3d.io.read_point_cloud(...).points`` holds).  Any
+    scalar type, ascii or binary of either byte order; other properties and elements are skipped."""
+    return _xyz(_read_elements(path, ("vertex",)), path)
+
+
+def load_triangle_mesh_ply(path: str):
+    """(vertices float64 [V, 3], faces int64 [F, 3]) of a triangle mesh PLY (``o3d.io.read_triangle_mesh``): the ``face``
+    element's ``vertex_indices`` (or ``vertex_index``) list, with a uchar, ushort or int count, every face a triangle."""
+    found = _read_elements(path, ("vertex", "face"))
+    v = _xyz(found, path)
+    fe = found.get("face")
+    if fe is None:
+        return v, np.zeros((0, 3), np.int64)
+    name = "vertex_indices" if "vertex_indices" in fe else ("vertex_index" if "vertex_index" in fe else None)
+    if name is None:
+        raise ValueError(f"{path}: the face element has no vertex_indices list")
+    idx = fe[name]
+    if isinstance(idx, list):
+        if any(len(r) != 3 for r in idx):
+            raise ValueError(f"{path}: only triangle faces are supported")
+        idx = np.array(idx, dtype=np.int64).reshape(-1, 3)
+    if idx.ndim != 2 or (idx.shape[0] > 0 and idx.shape[1] != 3):
+        raise ValueError(f"{path}: only triangle faces are supported")
+    return v, np.asarray(idx, dtype=np.int64).reshape(-1, 3)
+
+
+def save_point_cloud_ply(path: str, points, colors=None) -> None:
+    """Binary little-endian PLY of a coloured point cloud (eval.py's ``vis_*.ply``): element ``vertex`` with double x y z
+    and uchar red green blue = rint(255 * clamp(c, 0, 1)) (zeros without colours).  Arrays may be numpy or torch."""
+    def arr(a):
+        if hasattr(a, "detach"):
+            a = a.detach().cpu().numpy()
+        return np.asarray(a, dtype=np.float64)
+
+    p = arr(points).reshape(-1, 3)
+    c = np.zeros_like(p) if colors is None else arr(colors).reshape(-1, 3)
+    rec = np.empty(len(p), dtype=[("x", "<f8"), ("y", "<f8"), ("z", "<f8"), ("red", "u1"), ("green", "u1"), ("blue", "u1")])
+    for k, name in enumerate(("x", "y", "z")):
+        rec[name] = p[:, k]
+    rgb = np.rint(255.0 * np.clip(c, 0.0, 1.0)).astype(np.uint8)
+    for k, name in enumerate(("red", "green", "blue")):
+        rec[name] = rgb[:, k]
+    header = ["ply", "format binary_little_endian 1.0", f"element vertex {len(p)}"] + [f"property double {a}" for a in ("x", "y", "z")]
+    header += [f"property uchar {a}" for a in ("red", "green", "blue")] + ["end_header"]
+    d = os.path.dirname(path)
+    if d:
+        os.makedirs(d, exist_ok=True)
+    with open(path, "wb") as f:
+        f.write(("\n".join(header) + "\n").encode("ascii"))
+        f.write(rec.tobytes())
+
+
 def save_triangle_mesh_ply(path: str, vertices, triangles, vertex_colors=None, vertex_normals=None) -> None:
     """Binary little-endian PLY of a triangle mesh (what ``o3d.io.write_triangle_mesh`` writes for mesh_extract.py's
     ``recon.ply``): element ``vertex`` with float x y z nx ny nz and uchar red green blue, element ``face`` with
