@@ -463,6 +463,76 @@ int32_t rgs_dtu_dilate_masks(int32_t n_views, int32_t H, int32_t W, const uint8_
 int32_t rgs_dtu_cull_vertices(int64_t V, const double* vertices, int32_t n_views, int32_t H, int32_t W, const double* proj, const uint8_t* dilated,
                               uint8_t* keep, void* cuda_stream);
 
+/* ---- Tanks and Temples evaluation: eval_tnt/run.py, registration.py and evaluation.py without Open3D ----
+ * The DTU block's arithmetic rules hold: IEEE fp64, every operation rounded on its own in the order written (no FMA
+ * contraction), points fp64 [N, 3] on the device, counts at most 2^31 - 1, and a non-finite input returns RGS_E_INVALID.
+ * Correspondences and distances come from rgs_dtu_nearest.
+ *
+ * A transform is a HOST pointer to 16 doubles, the 4x4 matrix row-major; its last row must be exactly (0 0 0 1) and every
+ * entry finite, else RGS_E_INVALID.  It maps p to p' with p'_r = ((T_r0 * x + T_r1 * y) + T_r2 * z) + T_r3 (no division by
+ * the homogeneous coordinate, which is 1).  NULL means no transform: the points are copied unchanged. */
+
+/* Polygon crop volume (Open3D's SelectionPolygonVolume): orthogonal_axis 0 / 1 / 2 for X / Y / Z; the polygon's two
+ * coordinates (u, v) are the remaining axes in increasing order ((y, z), (x, z), (x, y)).  polygon is DEVICE fp64 [K, 2],
+ * 3 <= K <= 2048, vertex k joined to vertex (k + 1) mod K.  A point w = p[orthogonal_axis] is kept iff
+ * axis_min <= w <= axis_max (inclusive at both ends) and (u, v) passes the crossing-number test: for each edge (a, b) with
+ * a.v < v <= b.v or b.v < v <= a.v (half-open, so a horizontal edge never counts and a vertex is counted once), the
+ * crossing x = a.u + ((v - a.v) * (b.u - a.u)) / (b.v - a.v) is counted iff x < u; the point is inside iff the count is
+ * odd.  Open3D's own boundary rule was not available to confirm this one: points exactly on an edge or a vertex may be
+ * decided differently there. */
+typedef struct rgs_tnt_crop_volume {
+	int32_t orthogonal_axis;
+	int32_t num_vertices;
+	double axis_min, axis_max;
+	const double* polygon;
+} rgs_tnt_crop_volume;
+
+/* Transform, then crop (registration.py:113-131, evaluation.py:75-89).  points fp64 [N, 3]; transform host [16] or NULL;
+ * volume (host struct) or NULL for no crop (every point kept).  kept uint8 [N] receives the mask over the transformed
+ * points; cropped fp64 [N, 3] receives the kept transformed points compacted in input order, *num_kept (host) their count.
+ * One thread per point with the polygon in shared memory, then CUB's stable DeviceSelect; one host read.  Scratch through
+ * `scratch` (about 40 bytes per point). */
+int32_t rgs_tnt_crop(int64_t N, const double* points, const double* transform, const rgs_tnt_crop_volume* volume, uint8_t* kept, double* cropped,
+                     int64_t* num_kept, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+
+/* In-place transform (Open3D's PointCloud::Transform, applied by the ICP after every update).  points fp64 [N, 3] are
+ * overwritten with T p as above.  No host synchronisation and no finiteness check of the points. */
+int32_t rgs_tnt_transform(int64_t N, double* points, const double* transform, void* cuda_stream);
+
+/* Voxel downsample (Open3D's VoxelDownSample).  origin = min_bound - voxel * 0.5 per axis (min_bound over all points);
+ * a point's voxel index per axis is floor((p - origin) / voxel), and the key (ix << 42) | (iy << 21) | iz.  When an axis
+ * needs more than 2^21 cells (floor((max_bound - origin) / voxel) >= 2^21) the call returns RGS_E_INVALID after one bounds
+ * pass, before any output or the sort scratch is requested.  Each voxel's mean is its sum ((0 + p_0) + p_1) + ... over its
+ * points in input order, divided by the count: the same sum Open3D's AccumulatedPoint forms, so each value matches it bit
+ * for bit.  Output in ascending key order (Open3D's is its hash map's): means fp64 [V, 3] through
+ * resize(out->means_user), counts int64 [V] through resize(out->counts_user); out->num_voxels receives V.  voxel must be
+ * positive and finite.  Scratch through resize(out->scratch_user): first 64 bytes (the bounds), then about 48 bytes per
+ * point.  Two host reads (the bounds, the voxel count).  One warp per voxel adds its points in order, so a voxel of 10^5
+ * points occupies one warp and not the launch. */
+typedef struct rgs_tnt_voxel_out {
+	void* means_user;
+	void* counts_user;
+	void* scratch_user;
+	int64_t num_voxels;
+} rgs_tnt_voxel_out;
+int32_t rgs_tnt_voxel_downsample(int64_t N, const double* points, double voxel, rgs_resize_fn resize, rgs_tnt_voxel_out* out, void* cuda_stream);
+
+/* Moments of the scaled point-to-point ICP (Open3D's TransformationEstimationPointToPoint(true), Eigen's umeyama).
+ * source fp64 [N, 3] (already transformed), target fp64 [M, 3], dist fp64 [N] and index int64 [N] from
+ * rgs_dtu_nearest(target, source).  Source point i corresponds to target point index[i] iff dist[i] < threshold (strict,
+ * as nanoflann's radius search; Open3D was not available to confirm it).  moments (HOST fp64 [19]) receives
+ *   [0] n, the correspondence count;  [1] the sum of d2(s_i, t_index[i]) over correspondences (d2 as rgs_dtu_nearest);
+ *   [2..4] ms = S_s * (1 / n);  [5..7] mt = S_t * (1 / n), with S the sums of the corresponding points;
+ *   [8..16] sigma = (1 / n) * sum (t - mt)(s - ms)^T, row-major;  [17] var_s = (1 / n) * sum ((sx^2 + sy^2) + sz^2) with s
+ *   the centred source point;  [18] 0 (the count of non-finite inputs: nonzero returns RGS_E_INVALID).
+ * Two passes (means, then centred sums), each reduced in a fixed tree: block b sums points [1024 b, 1024 b + 1024), thread
+ * t its points 1024 b + t + 256 k for k = 0..3 in that order from 0.0, then a halving tree over the 256 threads (slot t
+ * += slot t + s for s = 128, 64, .., 1); one block then sums the block results the same way (thread t: results t,
+ * t + 256, .. in order).  The shape depends on N only, so repeated calls return identical bits; no floating-point
+ * atomics.  With n = 0 every entry is 0.  Scratch through `scratch` (about 0.1 byte per point).  One host read. */
+int32_t rgs_tnt_icp_moments(int64_t N, const double* source, int64_t M, const double* target, const double* dist, const int64_t* index, double threshold,
+                            double* moments, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+
 /* Introspection for parity tests: views into the private buffers written by rgs_forward
  * (the reference keeps the same data at BinningState::point_list / ImageState::ranges,
  * rasterizer_impl.cu:237-250,224-235).  Pointers are device addresses inside the given buffers. */

@@ -757,6 +757,94 @@ int32_t rgs_dtu_cull_vertices(int64_t V, const double* vertices, int32_t n_views
 	return dtu_cuda(launch_dtu_cull(V, vertices, n_views, H, W, proj, dilated, keep, (cudaStream_t)cuda_stream), "dtu cull");
 }
 
+// ---- TNT evaluation (rgs_tnt_eval.cu) ----
+
+static int tnt_check_transform(const double* T, const char* what) {
+	if (!T) return RGS_OK;
+	for (int k = 0; k < 16; k++)
+		if (!std::isfinite(T[k])) return fail(RGS_E_INVALID, std::string(what) + ": the transform has a NaN or infinite entry");
+	if (T[12] != 0.0 || T[13] != 0.0 || T[14] != 0.0 || T[15] != 1.0) return fail(RGS_E_INVALID, std::string(what) + ": the transform's last row must be (0 0 0 1)");
+	return RGS_OK;
+}
+
+int32_t rgs_tnt_crop(int64_t N, const double* points, const double* transform, const rgs_tnt_crop_volume* volume, uint8_t* kept, double* cropped,
+                     int64_t* num_kept, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (N < 0 || N > INT32_MAX) return fail(RGS_E_INVALID, "tnt crop: point count out of range");
+	if (!num_kept) return fail(RGS_E_INVALID, "null pointer");
+	*num_kept = 0;
+	if (const int rc = tnt_check_transform(transform, "tnt crop")) return rc;
+	if (volume) {
+		if (volume->orthogonal_axis < 0 || volume->orthogonal_axis > 2) return fail(RGS_E_INVALID, "tnt crop: orthogonal_axis must be 0, 1 or 2");
+		if (volume->num_vertices < 3 || volume->num_vertices > 2048) return fail(RGS_E_INVALID, "tnt crop: the polygon needs 3 to 2048 vertices");
+		if (!volume->polygon) return fail(RGS_E_INVALID, "null pointer");
+		if (std::isnan(volume->axis_min) || std::isnan(volume->axis_max)) return fail(RGS_E_INVALID, "tnt crop: axis_min / axis_max is NaN");
+	}
+	if (N == 0) return RGS_OK;
+	if (!points || !kept || !cropped || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = scratch(scratch_user, tnt_crop_scratch_bytes((int)N));
+	if (!buf) return fail(RGS_E_ALLOC, "tnt crop scratch callback returned NULL");
+	const cudaError_t e = launch_tnt_crop((int)N, points, transform, volume ? volume->orthogonal_axis : 0, volume ? volume->axis_min : 0.0,
+	                                      volume ? volume->axis_max : 0.0, volume ? volume->num_vertices : 0, volume ? volume->polygon : nullptr, kept,
+	                                      cropped, num_kept, buf, (cudaStream_t)cuda_stream);
+	return dtu_cuda(e, "tnt crop");
+}
+
+int32_t rgs_tnt_transform(int64_t N, double* points, const double* transform, void* cuda_stream) {
+	if (N < 0 || N > INT32_MAX) return fail(RGS_E_INVALID, "tnt transform: point count out of range");
+	if (!transform) return fail(RGS_E_INVALID, "null pointer");
+	if (const int rc = tnt_check_transform(transform, "tnt transform")) return rc;
+	if (N > 0 && !points) return fail(RGS_E_INVALID, "null pointer");
+	return dtu_cuda(launch_tnt_transform(N, points, transform, (cudaStream_t)cuda_stream), "tnt transform");
+}
+
+int32_t rgs_tnt_voxel_downsample(int64_t N, const double* points, double voxel, rgs_resize_fn resize, rgs_tnt_voxel_out* out, void* cuda_stream) {
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	out->num_voxels = 0;
+	if (N < 0 || N > INT32_MAX) return fail(RGS_E_INVALID, "tnt voxel: point count out of range");
+	if (!(std::isfinite(voxel) && voxel > 0.0)) return fail(RGS_E_INVALID, "tnt voxel: voxel size must be positive and finite");
+	if (N > 0 && !points) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	double lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0}, origin[3] = {0, 0, 0};
+	if (N > 0) {
+		char* bbuf = resize(out->scratch_user, tnt_bounds_scratch_bytes());
+		if (!bbuf) return fail(RGS_E_ALLOC, "tnt voxel scratch callback returned NULL");
+		int64_t bad = 0;
+		const cudaError_t e = launch_tnt_bounds((int)N, points, bbuf, lo, hi, &bad, s);
+		if (e != cudaSuccess) return fail(RGS_E_CUDA, std::string("tnt voxel: ") + cudaGetErrorString(e));
+		if (bad) return fail(RGS_E_INVALID, "tnt voxel: a point has a NaN or infinite coordinate");
+		for (int a = 0; a < 3; a++) {
+			origin[a] = lo[a] - voxel * 0.5;
+			const double top = std::floor((hi[a] - origin[a]) / voxel);
+			if (!(top < 2097152.0)) return fail(RGS_E_INVALID, "tnt voxel: more than 2^21 voxels along an axis");
+		}
+	}
+	char* buf = N > 0 ? resize(out->scratch_user, tnt_voxel_scratch_bytes((int)N)) : nullptr;
+	if (N > 0 && !buf) return fail(RGS_E_ALLOC, "tnt voxel scratch callback returned NULL");
+	int32_t V = 0;
+	if (N > 0) {
+		const cudaError_t e = launch_tnt_voxel_sort((int)N, points, origin, voxel, buf, &V, s);
+		if (e != cudaSuccess) return fail(RGS_E_CUDA, std::string("tnt voxel: ") + cudaGetErrorString(e));
+	}
+	out->num_voxels = V;
+	char* means = resize(out->means_user, (size_t)V * 3 * sizeof(double));
+	char* counts = resize(out->counts_user, (size_t)V * sizeof(int64_t));
+	if (V > 0 && (!means || !counts)) return fail(RGS_E_ALLOC, "tnt voxel callback returned NULL");
+	if (V == 0) return RGS_OK;
+	return dtu_cuda(launch_tnt_voxel_mean((int)N, points, V, buf, reinterpret_cast<double*>(means), reinterpret_cast<int64_t*>(counts), s), "tnt voxel");
+}
+
+int32_t rgs_tnt_icp_moments(int64_t N, const double* source, int64_t M, const double* target, const double* dist, const int64_t* index, double threshold,
+                            double* moments, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (N < 0 || M < 0 || N > INT32_MAX || M > INT32_MAX) return fail(RGS_E_INVALID, "tnt moments: point count out of range");
+	if (std::isnan(threshold)) return fail(RGS_E_INVALID, "tnt moments: the threshold is NaN");
+	if (!moments || !scratch || (N > 0 && (!source || !dist || !index)) || (M > 0 && !target)) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = scratch(scratch_user, tnt_moments_scratch_bytes(N));
+	if (!buf) return fail(RGS_E_ALLOC, "tnt moments scratch callback returned NULL");
+	const cudaError_t e = launch_tnt_moments(N, source, M, target, dist, index, threshold, buf, moments, (cudaStream_t)cuda_stream);
+	if (e == cudaErrorInvalidValue) return fail(RGS_E_INVALID, "tnt moments: a point or a distance is NaN or infinite");
+	return dtu_cuda(e, "tnt moments");
+}
+
 int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt, float* dmaps,
                                  double* sums, void* cuda_stream) {
 	if (planes < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");

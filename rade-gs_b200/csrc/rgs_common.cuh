@@ -312,6 +312,20 @@ cudaError_t launch_dtu_dilate(int n_views, int H, int W, const uint8_t* masks, u
 cudaError_t launch_dtu_cull(int64_t V, const double* verts, int n_views, int H, int W, const double* proj, const uint8_t* masks, uint8_t* keep,
                             cudaStream_t s);
 
+// TNT evaluation (rgs_tnt_eval.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
+size_t tnt_crop_scratch_bytes(int N);
+cudaError_t launch_tnt_crop(int N, const double* pts, const double* xform, int axis, double axis_min, double axis_max, int K, const double* polygon,
+                            uint8_t* kept, double* cropped, int64_t* num_kept, char* scratch, cudaStream_t s);
+cudaError_t launch_tnt_transform(int64_t N, double* pts, const double* xform, cudaStream_t s);
+size_t tnt_bounds_scratch_bytes();
+size_t tnt_voxel_scratch_bytes(int N);
+cudaError_t launch_tnt_bounds(int N, const double* pts, char* scratch, double* lo, double* hi, int64_t* nonfinite, cudaStream_t s);
+cudaError_t launch_tnt_voxel_sort(int N, const double* pts, const double* origin, double voxel, char* scratch, int32_t* num_voxels, cudaStream_t s);
+cudaError_t launch_tnt_voxel_mean(int N, const double* pts, int V, char* scratch, double* means, int64_t* counts, cudaStream_t s);
+size_t tnt_moments_scratch_bytes(int64_t N);
+cudaError_t launch_tnt_moments(int64_t N, const double* src, int64_t M, const double* tgt, const double* dist, const int64_t* index, double thr,
+                               char* scratch, double* moments_host, cudaStream_t s);
+
 // fused image-side losses (rgs_image_loss.cu; SURVEY.md 8f row 2)
 void launch_ssim_l1_forward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, float* dmaps, double* sums,
                             cudaStream_t s);

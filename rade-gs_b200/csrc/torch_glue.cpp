@@ -922,6 +922,73 @@ torch::Tensor DtuCullVertices(const torch::Tensor& vertices, const torch::Tensor
 	return keep;
 }
 
+// ---- TNT evaluation (rgs_tnt_*; Python side rade_gs_b200.tnt_eval) -------------------------------------------------------
+
+// a 4x4 transform as 16 host doubles (row-major), or an empty tensor for none
+torch::Tensor tnt_host_transform(const torch::Tensor& T) {
+	if (T.numel() == 0) return T;
+	TORCH_CHECK(T.dim() == 2 && T.size(0) == 4 && T.size(1) == 4, "transform must be [4, 4], got ", T.sizes());
+	return T.to(torch::kCPU, torch::kFloat64).contiguous();
+}
+
+// points f64 [N,3], transform f64 [4,4] or empty, polygon f64 [K,2] (CUDA) or empty -> (kept bool [N], cropped f64 [n,3])
+std::tuple<torch::Tensor, torch::Tensor> TntCrop(const torch::Tensor& points, const torch::Tensor& transform, int64_t axis, double axis_min, double axis_max,
+                                                 const torch::Tensor& polygon) {
+	const torch::Tensor p = dtu_points(points, "points");
+	const c10::cuda::CUDAGuard guard(p.device());
+	const torch::Tensor T = tnt_host_transform(transform);
+	torch::Tensor poly;
+	rgs_tnt_crop_volume vol{};
+	if (polygon.numel() > 0) {
+		TORCH_CHECK(polygon.is_cuda() && polygon.device() == p.device() && polygon.scalar_type() == torch::kFloat64 && polygon.dim() == 2 &&
+		                polygon.size(1) == 2,
+		            "polygon must be a CUDA float64 [K, 2] tensor on the points' device");
+		poly = polygon.contiguous();
+		vol = rgs_tnt_crop_volume{(int32_t)axis, (int32_t)poly.size(0), axis_min, axis_max, poly.data_ptr<double>()};
+	}
+	torch::Tensor kept = new_empty({p.size(0)}, p.options().dtype(torch::kBool)), cropped = new_empty({p.size(0), 3}, p.options()), scratch = dtu_bytes(p);
+	int64_t n = 0;
+	check(rgs_tnt_crop(p.size(0), p.data_ptr<double>(), T.numel() ? T.data_ptr<double>() : nullptr, polygon.numel() ? &vol : nullptr,
+	                   reinterpret_cast<uint8_t*>(kept.data_ptr<bool>()), cropped.data_ptr<double>(), &n, resize_cb, &scratch,
+	                   at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(kept, cropped.narrow(0, 0, n));
+}
+
+// points f64 [N,3] (contiguous CUDA), overwritten with T p
+void TntTransform(torch::Tensor points, const torch::Tensor& transform) {
+	TORCH_CHECK(points.is_cuda() && points.scalar_type() == torch::kFloat64 && points.dim() == 2 && points.size(1) == 3 && points.is_contiguous(),
+	            "points must be a contiguous CUDA float64 [N, 3] tensor");
+	TORCH_CHECK(transform.numel() == 16, "transform must be [4, 4]");
+	const c10::cuda::CUDAGuard guard(points.device());
+	const torch::Tensor T = tnt_host_transform(transform);
+	check(rgs_tnt_transform(points.size(0), points.data_ptr<double>(), T.data_ptr<double>(), at::cuda::getCurrentCUDAStream().stream()));
+}
+
+// points f64 [N,3] -> (means f64 [V,3] in ascending voxel key order, counts int64 [V])
+std::tuple<torch::Tensor, torch::Tensor> TntVoxelDownsample(const torch::Tensor& points, double voxel) {
+	const torch::Tensor p = dtu_points(points, "points");
+	const c10::cuda::CUDAGuard guard(p.device());
+	torch::Tensor means = dtu_bytes(p), counts = dtu_bytes(p), scratch = dtu_bytes(p);
+	rgs_tnt_voxel_out out{&means, &counts, &scratch, 0};
+	check(rgs_tnt_voxel_downsample(p.size(0), p.data_ptr<double>(), voxel, resize_cb, &out, at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(means.narrow(0, 0, out.num_voxels * 3 * 8).view(torch::kFloat64).view({out.num_voxels, 3}),
+	                       counts.narrow(0, 0, out.num_voxels * 8).view(torch::kInt64));
+}
+
+// source f64 [N,3], target f64 [M,3], dist f64 [N], index int64 [N] -> the 18 moments (CPU float64)
+torch::Tensor TntIcpMoments(const torch::Tensor& source, const torch::Tensor& target, const torch::Tensor& dist, const torch::Tensor& index, double threshold) {
+	const torch::Tensor s = dtu_points(source, "source"), t = dtu_points(target, "target");
+	TORCH_CHECK(s.device() == t.device() && dist.device() == s.device() && index.device() == s.device(), "all inputs must be on one CUDA device");
+	TORCH_CHECK(dist.scalar_type() == torch::kFloat64 && dist.dim() == 1 && dist.size(0) == s.size(0), "dist must be float64 [N]");
+	TORCH_CHECK(index.scalar_type() == torch::kInt64 && index.dim() == 1 && index.size(0) == s.size(0), "index must be int64 [N]");
+	const c10::cuda::CUDAGuard guard(s.device());
+	const torch::Tensor d = dist.contiguous(), ix = index.contiguous();
+	torch::Tensor scratch = dtu_bytes(s), mom = torch::empty({19}, torch::TensorOptions().dtype(torch::kFloat64));
+	check(rgs_tnt_icp_moments(s.size(0), s.data_ptr<double>(), t.size(0), t.data_ptr<double>(), d.data_ptr<double>(), ix.data_ptr<int64_t>(), threshold,
+	                          mom.data_ptr<double>(), resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
+	return mom.narrow(0, 0, 18);
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1004,6 +1071,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("dtu_nearest", &DtuNearest, py::arg("reference"), py::arg("query"));
 	m.def("dtu_dilate_masks", &DtuDilateMasks, py::arg("masks"));
 	m.def("dtu_cull_vertices", &DtuCullVertices, py::arg("vertices"), py::arg("proj"), py::arg("dilated"));
+	m.def("tnt_crop", &TntCrop, py::arg("points"), py::arg("transform"), py::arg("axis"), py::arg("axis_min"), py::arg("axis_max"), py::arg("polygon"));
+	m.def("tnt_transform", &TntTransform, py::arg("points"), py::arg("transform"));
+	m.def("tnt_voxel_downsample", &TntVoxelDownsample, py::arg("points"), py::arg("voxel"));
+	m.def("tnt_icp_moments", &TntIcpMoments, py::arg("source"), py::arg("target"), py::arg("dist"), py::arg("index"), py::arg("threshold"));
 	m.def("grad_stride", [](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });
