@@ -533,6 +533,83 @@ int32_t rgs_tnt_voxel_downsample(int64_t N, const double* points, double voxel, 
 int32_t rgs_tnt_icp_moments(int64_t N, const double* source, int64_t M, const double* target, const double* dist, const int64_t* index, double threshold,
                             double* moments, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
 
+/* ---- Tetrahedra mesh extraction: mesh_extract_tetrahedra.py, utils/tetmesh.py and GaussianModel.get_tetra_points ----
+ * Arrays are fp32 / int32 / int64 on the device, row-major.  Stages 2-5 are fixed bit for bit: every fp32 operation below is
+ * one IEEE operation rounded to nearest on its own (no FMA contraction unless an fma is written), in the order written;
+ * x * 0.5 is exact. */
+
+/* Tetra points (gaussian_model.py:400-429).  xyz [P, 3], scaling [P, 3] (get_scaling_with_3D_filter), rotation [P, 4] raw
+ * (w, x, y, z), normalised here: n = sqrt(((w^2 + x^2) + y^2) + z^2), q = rotation / n, R as build_rotation.  s3 = scaling * 3.
+ * points [9P, 3]: row 8 g + k (k = 0..7) is R (c_k * s3) + xyz_g with c_k = (2 bx - 1, 2 by - 1, 2 bz - 1), k = 4 bx + 2 by + bz
+ * (trimesh.creation.box()'s vertex order, doubled); rows 8P + g are the centres xyz_g.  scales [9P] (the reference's [9P, 1]):
+ * max(s3) of the Gaussian (NaN if any is NaN) at the same rows; these are exact.  The rotated corners are not bit-fixed (the
+ * reference uses a batched matrix product): R c + xyz is evaluated in fp32 with contraction allowed. */
+int32_t rgs_tetra_points(int64_t P, const float* xyz, const float* scaling, const float* rotation, float* points, float* scales, void* cuda_stream);
+
+/* Cull SDF, one view (mesh_extract_tetrahedra.py:32-56, evaluage_cull_alpha).  alpha [N] and coord [N, 2] (pixel x, y) are
+ * integrate()'s alpha_integrated and point_coordinate; render7 [H, W] its render[7]; gt_mask [H, W] or NULL.  Inputs are not
+ * modified.  Per point:
+ *   gx = (((x * 2) + 1) / (W - 1)) - 1, gy likewise with y and H;
+ *   ix = (((gx + 1) * W) - 1) * 0.5, iy likewise with H (grid_sample, align_corners=False);
+ *   x0 = floor(ix), y0 = floor(iy), x1 = x0 + 1, y1 = y0 + 1, wx = ix - x0, ex = 1 - wx, wy = iy - y0, ey = 1 - wy;
+ *   m(x, y) = render7[y, x] * gt_mask[y, x] (render7[y, x] without a mask) when 0 <= x <= W - 1 and 0 <= y <= H - 1, else 0;
+ *   v = (((ey * ex) * m(x0, y0) + (ey * wx) * m(x1, y0)) + (wy * ex) * m(x0, y1)) + (wy * wx) * m(x1, y1);
+ *   if v > 0.5: final = NaN if alpha or final is NaN, else (final < alpha ? final : alpha); weight += 1.
+ * final [N] (start: 1) and weight int32 [N] (start: 0) are the caller's accumulators.  No host synchronisation. */
+int32_t rgs_tetra_cull_add(int64_t N, const float* alpha, const float* coord, int32_t H, int32_t W, const float* render7, const float* gt_mask,
+                           float* final_alpha, int32_t* weight, void* cuda_stream);
+/* sdf [N] = 0.5 - final where weight > 0, else -100.  No host synchronisation. */
+int32_t rgs_tetra_cull_finish(int64_t N, const float* final_alpha, const int32_t* weight, float* sdf, void* cuda_stream);
+
+/* Marching tetrahedra (utils/tetmesh.py, _unbatched_marching_tetrahedra).  points [N, 3], sdf [N], scales [N], tets int64
+ * [T, 4].  A vertex is occupied when sdf > 0; a tet is valid when 1 to 3 of its vertices are.  Every tet index must lie in
+ * [0, N): otherwise RGS_E_INVALID (found by a device flag, before any output is requested).  The edges (0,1), (0,2), (0,3),
+ * (1,2), (1,3), (2,3) of the valid tets, as (min, max) pairs, are made unique; output vertex m is the m-th edge in ascending
+ * (a, b) order whose endpoints differ in occupancy.  Outputs through resize: interp int64 [M, 2] = (a, b); ends [M, 2, 3] =
+ * (points[a], points[b]); end_sdf [M, 2]; end_scales [M, 2].  faces int64 [F, 3] come from triangle_table[code] (code = sum of
+ * 2^k over the occupied vertices k) on the tet's edge vertices: for chunk c of torch.chunk(tets, T // 2^25 + 1) when
+ * T > 2^25 (one chunk otherwise), first every 1-triangle tet of the chunk in tet order (3 entries), then every 2-triangle tet
+ * (6 entries, two faces).  This is the reference's order, chunk loop included.  N, T < 2^31 and 6 x (valid tets) < 2^31 - 256,
+ * else RGS_E_INVALID.  Scratch through resize(out->scratch_user) (about 6 bytes per tet) and resize(out->sort_user) (about
+ * 240 bytes per valid tet).  Two host reads (the valid-tet count with the index flag; M and F). */
+typedef struct rgs_tetra_march_out {
+	void* interp_user;
+	void* ends_user;
+	void* end_sdf_user;
+	void* end_scales_user;
+	void* faces_user;
+	void* scratch_user;
+	void* sort_user;
+	int64_t num_vertices, num_faces;
+} rgs_tetra_march_out;
+int32_t rgs_tetra_marching(int64_t N, const float* points, const float* sdf, const float* scales, int64_t T, const int64_t* tets, rgs_resize_fn resize,
+                           rgs_tetra_march_out* out, void* cuda_stream);
+
+/* Bisection step (mesh_extract_tetrahedra.py:92-102).  left, right [M, 3], left_sdf, right_sdf [M] are updated in place; mid
+ * [M, 3] receives the next midpoints.  With c = (l + r) * 0.5 per component: when mid_sdf [M] is given,
+ * low = (mid_sdf < 0 and left_sdf < 0) or (mid_sdf > 0 and left_sdf > 0) (so 0 and NaN go right); low: left = c,
+ * left_sdf = mid_sdf, else right = c, right_sdf = mid_sdf.  Then mid = (left + right) * 0.5.  mid_sdf NULL: only mid is
+ * written (the first midpoints).  No host synchronisation. */
+int32_t rgs_tetra_bisect(int64_t M, const float* mid_sdf, float* left, float* right, float* left_sdf, float* right_sdf, float* mid, void* cuda_stream);
+
+/* Distance / scale filter and compaction (mesh_extract_tetrahedra.py:105-112, trimesh update_vertices then update_faces).
+ * points [M, 3] (the final midpoints); ends [M, 2, 3] and end_scales [M, 2] from rgs_tetra_marching (the original edge
+ * endpoints); faces int64 [F, 3] with entries in [0, M): an entry outside it returns RGS_E_INVALID (a device flag, read with
+ * the counts).  With d = end0 - end1: vertex m is kept iff sqrt(fma(dz, dz, fma(dy, dy, dx*dx))) <= s0 + s1 (the fused
+ * multiply-adds round once each: torch.norm's order on the CPU, which decides the ties below).  Adjacent box corners along a
+ * Gaussian's longest axis are exactly s0 + s1 apart, so ties occur; torch.norm on a GPU may round them differently.  Kept vertices stay in order (also those no
+ * face uses); a face is kept iff its 3 vertices are, its entries renumbered to ranks among the kept vertices, in order.
+ * vertices fp32 [V', 3] and faces int64 [F', 3] through resize; counts in out.  Scratch through resize(out->scratch_user)
+ * (about 16 bytes per vertex and 25 per face).  One host read. */
+typedef struct rgs_tetra_filter_out {
+	void* vertices_user;
+	void* faces_user;
+	void* scratch_user;
+	int64_t num_vertices, num_faces;
+} rgs_tetra_filter_out;
+int32_t rgs_tetra_filter(int64_t M, const float* points, const float* ends, const float* end_scales, int64_t F, const int64_t* faces, rgs_resize_fn resize,
+                         rgs_tetra_filter_out* out, void* cuda_stream);
+
 /* Introspection for parity tests: views into the private buffers written by rgs_forward
  * (the reference keeps the same data at BinningState::point_list / ImageState::ranges,
  * rasterizer_impl.cu:237-250,224-235).  Pointers are device addresses inside the given buffers. */

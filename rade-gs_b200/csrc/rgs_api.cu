@@ -845,6 +845,103 @@ int32_t rgs_tnt_icp_moments(int64_t N, const double* source, int64_t M, const do
 	return dtu_cuda(e, "tnt moments");
 }
 
+// ---- tetrahedra mesh extraction (rgs_tetra.cu) ----
+
+static int tetra_cuda(cudaError_t e, const char* what) {
+	return e == cudaSuccess ? (int)RGS_OK : fail(RGS_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+}
+
+int32_t rgs_tetra_points(int64_t P, const float* xyz, const float* scaling, const float* rotation, float* points, float* scales, void* cuda_stream) {
+	if (P < 0 || 9 * P > INT32_MAX) return fail(RGS_E_INVALID, "tetra points: Gaussian count out of range");
+	if (P == 0) return RGS_OK;
+	if (!xyz || !scaling || !rotation || !points || !scales) return fail(RGS_E_INVALID, "null pointer");
+	return tetra_cuda(launch_tetra_points((int)P, xyz, scaling, rotation, points, scales, (cudaStream_t)cuda_stream), "tetra points");
+}
+
+int32_t rgs_tetra_cull_add(int64_t N, const float* alpha, const float* coord, int32_t H, int32_t W, const float* render7, const float* gt_mask,
+                           float* final_alpha, int32_t* weight, void* cuda_stream) {
+	if (N < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "tetra cull: negative point count or empty image");
+	if (N == 0) return RGS_OK;
+	if (!alpha || !coord || !render7 || !final_alpha || !weight) return fail(RGS_E_INVALID, "null pointer");
+	return tetra_cuda(launch_tetra_cull_add(N, alpha, coord, H, W, render7, gt_mask, final_alpha, weight, (cudaStream_t)cuda_stream), "tetra cull");
+}
+
+int32_t rgs_tetra_cull_finish(int64_t N, const float* final_alpha, const int32_t* weight, float* sdf, void* cuda_stream) {
+	if (N < 0) return fail(RGS_E_INVALID, "tetra cull: negative point count");
+	if (N == 0) return RGS_OK;
+	if (!final_alpha || !weight || !sdf) return fail(RGS_E_INVALID, "null pointer");
+	return tetra_cuda(launch_tetra_cull_finish(N, final_alpha, weight, sdf, (cudaStream_t)cuda_stream), "tetra cull finish");
+}
+
+int32_t rgs_tetra_marching(int64_t N, const float* points, const float* sdf, const float* scales, int64_t T, const int64_t* tets, rgs_resize_fn resize,
+                           rgs_tetra_march_out* out, void* cuda_stream) {
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	out->num_vertices = out->num_faces = 0;
+	if (N < 0 || N > INT32_MAX || T < 0 || T > INT32_MAX) return fail(RGS_E_INVALID, "tetra marching: point or tet count out of range");
+	if ((N > 0 && (!points || !sdf || !scales)) || (T > 0 && !tets)) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int32_t V = 0, M = 0, F = 0;
+	char* s1 = nullptr;
+	if (T > 0) {
+		s1 = resize(out->scratch_user, tetra_march_scratch1_bytes(T));
+		if (!s1) return fail(RGS_E_ALLOC, "tetra marching scratch callback returned NULL");
+		int32_t bad = 0;
+		if (const int rc = tetra_cuda(launch_tetra_march_valid(T, N, tets, sdf, s1, &bad, &V, s), "tetra marching")) return rc;
+		if (bad) return fail(RGS_E_INVALID, "tetra marching: a tet index lies outside [0, N)");
+		if (V > (INT32_MAX - 255) / 6) return fail(RGS_E_INVALID, "tetra marching: too many valid tets (6 x valid must stay below 2^31)");
+	}
+	char* s2 = nullptr;
+	if (V > 0) {
+		s2 = resize(out->sort_user, tetra_march_scratch2_bytes(V));
+		if (!s2) return fail(RGS_E_ALLOC, "tetra marching scratch callback returned NULL");
+		if (const int rc = tetra_cuda(launch_tetra_march_sort(T, N, tets, sdf, V, s1, s2, &M, &F, s), "tetra marching")) return rc;
+	}
+	char* interp = resize(out->interp_user, (size_t)M * 2 * sizeof(int64_t));
+	char* ends = resize(out->ends_user, (size_t)M * 6 * sizeof(float));
+	char* end_sdf = resize(out->end_sdf_user, (size_t)M * 2 * sizeof(float));
+	char* end_scl = resize(out->end_scales_user, (size_t)M * 2 * sizeof(float));
+	char* faces = resize(out->faces_user, (size_t)F * 3 * sizeof(int64_t));
+	if ((M > 0 && (!interp || !ends || !end_sdf || !end_scl)) || (F > 0 && !faces)) return fail(RGS_E_ALLOC, "tetra marching callback returned NULL");
+	out->num_vertices = M;
+	out->num_faces = F;
+	if (V == 0) return RGS_OK;
+	return tetra_cuda(launch_tetra_march_emit(T, points, sdf, scales, V, s1, s2, N, reinterpret_cast<int64_t*>(interp), reinterpret_cast<float*>(ends),
+	                                          reinterpret_cast<float*>(end_sdf), reinterpret_cast<float*>(end_scl), reinterpret_cast<int64_t*>(faces), s),
+	                  "tetra marching");
+}
+
+int32_t rgs_tetra_bisect(int64_t M, const float* mid_sdf, float* left, float* right, float* left_sdf, float* right_sdf, float* mid, void* cuda_stream) {
+	if (M < 0) return fail(RGS_E_INVALID, "tetra bisect: negative vertex count");
+	if (M == 0) return RGS_OK;
+	if (!left || !right || !mid || (mid_sdf && (!left_sdf || !right_sdf))) return fail(RGS_E_INVALID, "null pointer");
+	return tetra_cuda(launch_tetra_bisect(M, mid_sdf, left, right, left_sdf, right_sdf, mid, (cudaStream_t)cuda_stream), "tetra bisect");
+}
+
+int32_t rgs_tetra_filter(int64_t M, const float* points, const float* ends, const float* end_scales, int64_t F, const int64_t* faces, rgs_resize_fn resize,
+                         rgs_tetra_filter_out* out, void* cuda_stream) {
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	out->num_vertices = out->num_faces = 0;
+	if (M < 0 || M > INT32_MAX || F < 0 || F > INT32_MAX) return fail(RGS_E_INVALID, "tetra filter: vertex or face count out of range");
+	if ((M > 0 && (!points || !ends || !end_scales)) || (F > 0 && !faces)) return fail(RGS_E_INVALID, "null pointer");
+	if (M == 0 && F > 0) return fail(RGS_E_INVALID, "tetra filter: faces without vertices");
+	char* verts = resize(out->vertices_user, (size_t)M * 3 * sizeof(float));
+	char* fout = resize(out->faces_user, (size_t)F * 3 * sizeof(int64_t));
+	if ((M > 0 && !verts) || (F > 0 && !fout)) return fail(RGS_E_ALLOC, "tetra filter callback returned NULL");
+	if (M == 0) return RGS_OK;
+	char* buf = resize(out->scratch_user, tetra_filter_scratch_bytes((int)M, F));
+	if (!buf) return fail(RGS_E_ALLOC, "tetra filter scratch callback returned NULL");
+	int64_t nv = 0, nf = 0;
+	int32_t bad = 0;
+	if (const int rc = tetra_cuda(launch_tetra_filter((int)M, points, ends, end_scales, F, faces, buf, reinterpret_cast<float*>(verts),
+	                                                  reinterpret_cast<int64_t*>(fout), &nv, &nf, &bad, (cudaStream_t)cuda_stream),
+	                              "tetra filter"))
+		return rc;
+	if (bad) return fail(RGS_E_INVALID, "tetra filter: a face index lies outside [0, M)");
+	out->num_vertices = nv;
+	out->num_faces = nf;
+	return RGS_OK;
+}
+
 int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt, float* dmaps,
                                  double* sums, void* cuda_stream) {
 	if (planes < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");

@@ -326,6 +326,24 @@ size_t tnt_moments_scratch_bytes(int64_t N);
 cudaError_t launch_tnt_moments(int64_t N, const double* src, int64_t M, const double* tgt, const double* dist, const int64_t* index, double thr,
                                char* scratch, double* moments_host, cudaStream_t s);
 
+// Tetrahedra mesh extraction (rgs_tetra.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
+cudaError_t launch_tetra_points(int P, const float* xyz, const float* scaling, const float* rotation, float* points, float* scales, cudaStream_t s);
+cudaError_t launch_tetra_cull_add(int64_t N, const float* alpha, const float* coord, int H, int W, const float* render7, const float* gt_mask, float* fin,
+                                  int32_t* weight, cudaStream_t s);
+cudaError_t launch_tetra_cull_finish(int64_t N, const float* fin, const int32_t* weight, float* sdf, cudaStream_t s);
+size_t tetra_march_scratch1_bytes(int64_t T);
+size_t tetra_march_scratch2_bytes(int V);
+cudaError_t launch_tetra_march_valid(int64_t T, int64_t N, const int64_t* tets, const float* sdf, char* scratch1, int32_t* bad, int32_t* num_valid,
+                                     cudaStream_t s);
+cudaError_t launch_tetra_march_sort(int64_t T, int64_t N, const int64_t* tets, const float* sdf, int V, const char* scratch1, char* scratch2,
+                                    int32_t* num_vertices, int32_t* num_faces, cudaStream_t s);
+cudaError_t launch_tetra_march_emit(int64_t T, const float* points, const float* sdf, const float* scales, int V, const char* scratch1, char* scratch2,
+                                    int64_t N, int64_t* interp, float* ends, float* end_sdf, float* end_scl, int64_t* faces, cudaStream_t s);
+cudaError_t launch_tetra_bisect(int64_t M, const float* mid_sdf, float* left, float* right, float* left_sdf, float* right_sdf, float* mid, cudaStream_t s);
+size_t tetra_filter_scratch_bytes(int M, int64_t F);
+cudaError_t launch_tetra_filter(int M, const float* points, const float* ends, const float* end_scl, int64_t F, const int64_t* faces, char* scratch,
+                                float* out_vertices, int64_t* out_faces, int64_t* num_vertices, int64_t* num_faces, int32_t* bad, cudaStream_t s);
+
 // fused image-side losses (rgs_image_loss.cu; SURVEY.md 8f row 2)
 void launch_ssim_l1_forward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, float* dmaps, double* sums,
                             cudaStream_t s);

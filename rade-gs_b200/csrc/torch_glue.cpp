@@ -989,6 +989,127 @@ torch::Tensor TntIcpMoments(const torch::Tensor& source, const torch::Tensor& ta
 	return mom.narrow(0, 0, 18);
 }
 
+// ---- tetrahedra mesh extraction (rgs_tetra_*; Python side rade_gs_b200.tetra) ----------------------------------------------
+
+// a CUDA float32 tensor with `inner` elements per row (inner 0: one-dimensional), on `like`'s device when given
+torch::Tensor tetra_f32(const torch::Tensor& t, int64_t inner, const char* name, const torch::Tensor* like = nullptr) {
+	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
+	TORCH_CHECK(!like || t.device() == like->device(), name, " must be on the same device as the other inputs");
+	TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32, got ", t.scalar_type());
+	if (inner == 0) {
+		TORCH_CHECK(t.dim() == 1, name, " must be one-dimensional, got ", t.sizes());
+	} else {
+		TORCH_CHECK(t.dim() >= 1 && t.numel() == t.size(0) * inner, name, " must hold ", inner, " values per row, got ", t.sizes());
+	}
+	return t.contiguous();
+}
+
+// xyz, scaling f32 [P,3], rotation f32 [P,4] -> (points f32 [9P,3], scales f32 [9P,1])
+std::tuple<torch::Tensor, torch::Tensor> TetraPoints(const torch::Tensor& xyz, const torch::Tensor& scaling, const torch::Tensor& rotation) {
+	const torch::Tensor x = tetra_f32(xyz, 3, "xyz"), s = tetra_f32(scaling, 3, "scaling", &x), r = tetra_f32(rotation, 4, "rotation", &x);
+	TORCH_CHECK(s.size(0) == x.size(0) && r.size(0) == x.size(0), "xyz, scaling and rotation must have one row per Gaussian");
+	const c10::cuda::CUDAGuard guard(x.device());
+	const int64_t P = x.size(0);
+	torch::Tensor pts = new_empty({9 * P, 3}, x.options()), scl = new_empty({9 * P, 1}, x.options());
+	check(rgs_tetra_points(P, x.data_ptr<float>(), s.data_ptr<float>(), r.data_ptr<float>(), pts.data_ptr<float>(), scl.data_ptr<float>(),
+	                       at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(pts, scl);
+}
+
+// accumulates one view into final_alpha f32 [N] and weight int32 [N] (contiguous, in place)
+void TetraCullAdd(const torch::Tensor& alpha, const torch::Tensor& coord, const torch::Tensor& render7, const torch::Tensor& gt_mask, torch::Tensor final_alpha,
+                  torch::Tensor weight) {
+	TORCH_CHECK(final_alpha.is_cuda() && final_alpha.scalar_type() == torch::kFloat32 && final_alpha.dim() == 1 && final_alpha.is_contiguous(),
+	            "final_alpha must be a contiguous CUDA float32 [N] tensor");
+	const int64_t N = final_alpha.size(0);
+	TORCH_CHECK(weight.device() == final_alpha.device() && weight.scalar_type() == torch::kInt32 && weight.dim() == 1 && weight.size(0) == N &&
+	                weight.is_contiguous(),
+	            "weight must be a contiguous int32 [N] tensor on final_alpha's device");
+	const torch::Tensor a = tetra_f32(alpha.reshape({-1}), 0, "alpha_integrated", &final_alpha), c = tetra_f32(coord, 2, "point_coordinate", &final_alpha);
+	TORCH_CHECK(a.size(0) == N && c.size(0) == N, "alpha_integrated and point_coordinate must have one row per point (", N, ")");
+	TORCH_CHECK(render7.dim() == 2, "render7 must be [H, W], got ", render7.sizes());
+	const torch::Tensor r7 = tetra_f32(render7, render7.size(1), "render7", &final_alpha);
+	torch::Tensor gt;
+	if (gt_mask.numel() > 0) {
+		gt = tetra_f32(gt_mask.reshape({-1}), 0, "gt_mask", &final_alpha);
+		TORCH_CHECK(gt.size(0) == r7.numel(), "gt_mask must have the image's H x W values, got ", gt_mask.sizes());
+	}
+	const c10::cuda::CUDAGuard guard(final_alpha.device());
+	check(rgs_tetra_cull_add(N, a.data_ptr<float>(), c.data_ptr<float>(), (int32_t)r7.size(0), (int32_t)r7.size(1), r7.data_ptr<float>(),
+	                         gt.defined() ? gt.data_ptr<float>() : nullptr, final_alpha.data_ptr<float>(), weight.data_ptr<int32_t>(),
+	                         at::cuda::getCurrentCUDAStream().stream()));
+}
+
+torch::Tensor TetraCullFinish(const torch::Tensor& final_alpha, const torch::Tensor& weight) {
+	const torch::Tensor f = tetra_f32(final_alpha, 0, "final_alpha");
+	TORCH_CHECK(weight.device() == f.device() && weight.scalar_type() == torch::kInt32 && weight.dim() == 1 && weight.size(0) == f.size(0),
+	            "weight must be int32 [N] on final_alpha's device");
+	const c10::cuda::CUDAGuard guard(f.device());
+	const torch::Tensor w = weight.contiguous();
+	torch::Tensor sdf = new_empty({f.size(0)}, f.options());
+	check(rgs_tetra_cull_finish(f.size(0), f.data_ptr<float>(), w.data_ptr<int32_t>(), sdf.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+	return sdf;
+}
+
+// points f32 [N,3], sdf f32 [N], scales f32 [N] or [N,1], tets int64 [T,4]
+//   -> (ends f32 [M,2,3], end_sdf f32 [M,2,1], end_scales f32 [M,2,1], faces int64 [F,3], interp_v int64 [M,2])
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> TetraMarching(const torch::Tensor& points, const torch::Tensor& sdf,
+                                                                                                   const torch::Tensor& scales, const torch::Tensor& tets) {
+	const torch::Tensor p = tetra_f32(points, 3, "vertices"), d = tetra_f32(sdf.reshape({-1}), 0, "sdf", &p), s = tetra_f32(scales.reshape({-1}), 0, "scales", &p);
+	TORCH_CHECK(d.size(0) == p.size(0) && s.size(0) == p.size(0), "sdf and scales must have one value per vertex");
+	TORCH_CHECK(tets.is_cuda() && tets.device() == p.device() && tets.scalar_type() == torch::kInt64 && tets.dim() == 2 && tets.size(1) == 4,
+	            "tets must be a CUDA int64 [T, 4] tensor on the vertices' device, got ", tets.scalar_type(), " ", tets.sizes());
+	const c10::cuda::CUDAGuard guard(p.device());
+	const torch::Tensor t = tets.contiguous();
+	torch::Tensor interp = dtu_bytes(p), ends = dtu_bytes(p), esdf = dtu_bytes(p), escl = dtu_bytes(p), faces = dtu_bytes(p), scratch = dtu_bytes(p),
+	              sort = dtu_bytes(p);
+	rgs_tetra_march_out out{&interp, &ends, &esdf, &escl, &faces, &scratch, &sort, 0, 0};
+	check(rgs_tetra_marching(p.size(0), p.data_ptr<float>(), d.data_ptr<float>(), s.data_ptr<float>(), t.size(0), t.data_ptr<int64_t>(), resize_cb, &out,
+	                         at::cuda::getCurrentCUDAStream().stream()));
+	const int64_t M = out.num_vertices, F = out.num_faces;
+	auto view = [](const torch::Tensor& b, int64_t n, torch::ScalarType ty, at::IntArrayRef shape) {
+		return b.narrow(0, 0, n * (ty == torch::kInt64 ? 8 : 4)).view(ty).view(shape);
+	};
+	return std::make_tuple(view(ends, M * 6, torch::kFloat32, {M, 2, 3}), view(esdf, M * 2, torch::kFloat32, {M, 2, 1}),
+	                       view(escl, M * 2, torch::kFloat32, {M, 2, 1}), view(faces, F * 3, torch::kInt64, {F, 3}), view(interp, M * 2, torch::kInt64, {M, 2}));
+}
+
+// one bisection step in place: left, right f32 [M,3], left_sdf, right_sdf f32 [M] (or [M,1]), mid f32 [M,3]; mid_sdf f32 [M] or empty
+void TetraBisect(const torch::Tensor& mid_sdf, torch::Tensor left, torch::Tensor right, torch::Tensor left_sdf, torch::Tensor right_sdf, torch::Tensor mid) {
+	const int64_t M = left.size(0);
+	for (const torch::Tensor* t : {&left, &right, &mid})
+		TORCH_CHECK(t->is_cuda() && t->device() == left.device() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == M * 3,
+		            "left, right and mid must be contiguous CUDA float32 [M, 3] tensors on one device");
+	for (const torch::Tensor* t : {&left_sdf, &right_sdf})
+		TORCH_CHECK(t->device() == left.device() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == M,
+		            "left_sdf and right_sdf must be contiguous float32 [M] tensors on the points' device");
+	torch::Tensor m;
+	if (mid_sdf.numel() > 0) {
+		m = tetra_f32(mid_sdf.reshape({-1}), 0, "mid_sdf", &left);
+		TORCH_CHECK(m.size(0) == M, "mid_sdf must have one value per vertex (", M, "), got ", mid_sdf.sizes());
+	}
+	const c10::cuda::CUDAGuard guard(left.device());
+	check(rgs_tetra_bisect(M, m.defined() ? m.data_ptr<float>() : nullptr, left.data_ptr<float>(), right.data_ptr<float>(), left_sdf.data_ptr<float>(),
+	                       right_sdf.data_ptr<float>(), mid.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+}
+
+// points f32 [M,3], ends f32 [M,2,3], end_scales f32 [M,2(,1)], faces int64 [F,3] -> (vertices f32 [V',3], faces int64 [F',3])
+std::tuple<torch::Tensor, torch::Tensor> TetraFilter(const torch::Tensor& points, const torch::Tensor& ends, const torch::Tensor& end_scales,
+                                                     const torch::Tensor& faces) {
+	const torch::Tensor p = tetra_f32(points, 3, "points"), e = tetra_f32(ends, 6, "ends", &p), s = tetra_f32(end_scales, 2, "end_scales", &p);
+	TORCH_CHECK(e.size(0) == p.size(0) && s.size(0) == p.size(0), "ends and end_scales must have one row per vertex");
+	TORCH_CHECK(faces.is_cuda() && faces.device() == p.device() && faces.scalar_type() == torch::kInt64 && faces.dim() == 2 && faces.size(1) == 3,
+	            "faces must be a CUDA int64 [F, 3] tensor on the points' device, got ", faces.scalar_type(), " ", faces.sizes());
+	const c10::cuda::CUDAGuard guard(p.device());
+	const torch::Tensor f = faces.contiguous();
+	torch::Tensor verts = dtu_bytes(p), fout = dtu_bytes(p), scratch = dtu_bytes(p);
+	rgs_tetra_filter_out out{&verts, &fout, &scratch, 0, 0};
+	check(rgs_tetra_filter(p.size(0), p.data_ptr<float>(), e.data_ptr<float>(), s.data_ptr<float>(), f.size(0), f.data_ptr<int64_t>(), resize_cb, &out,
+	                       at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(verts.narrow(0, 0, out.num_vertices * 12).view(torch::kFloat32).view({out.num_vertices, 3}),
+	                       fout.narrow(0, 0, out.num_faces * 24).view(torch::kInt64).view({out.num_faces, 3}));
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1075,7 +1196,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("tnt_transform", &TntTransform, py::arg("points"), py::arg("transform"));
 	m.def("tnt_voxel_downsample", &TntVoxelDownsample, py::arg("points"), py::arg("voxel"));
 	m.def("tnt_icp_moments", &TntIcpMoments, py::arg("source"), py::arg("target"), py::arg("dist"), py::arg("index"), py::arg("threshold"));
-	m.def("grad_stride", [](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
+	m.def("tetra_points", &TetraPoints, py::arg("xyz"), py::arg("scaling"), py::arg("rotation"));
+	m.def("tetra_cull_add", &TetraCullAdd, py::arg("alpha"), py::arg("coord"), py::arg("render7"), py::arg("gt_mask"), py::arg("final_alpha"), py::arg("weight"));
+	m.def("tetra_cull_finish", &TetraCullFinish, py::arg("final_alpha"), py::arg("weight"));
+	m.def("tetra_marching", &TetraMarching, py::arg("vertices"), py::arg("sdf"), py::arg("scales"), py::arg("tets"));
+	m.def("tetra_bisect", &TetraBisect, py::arg("mid_sdf"), py::arg("left"), py::arg("right"), py::arg("left_sdf"), py::arg("right_sdf"), py::arg("mid"));
+	m.def("tetra_filter", &TetraFilter, py::arg("points"), py::arg("ends"), py::arg("end_scales"), py::arg("faces"));
+	m.def("grad_stride",[](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });
 	m.def("abi_version", []() { return rgs_abi_version(); });
