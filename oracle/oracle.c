@@ -830,8 +830,10 @@ void orc_preprocess_backward(const orc_scene* s, const orc_geom* g, const orc_sg
 /* ---- integrate_gaussians_to_points (SURVEY.md 8f row 3) ---------------------------------------------------------
  * computeCov2D<INTE> extras, forward.cu:187-235: the inverse covariance in (pixel x, pixel y, ray depth) space.  The
  * reference leaves it unassigned for ill-conditioned covariances (its else-branch fills a shadowed local, :214); those
- * Gaussians get condition = 0 and zeros here.  invraycov [P,6] must arrive zero-filled (rasterize_points.cu:317). */
-void orc_inte_geometry(const orc_scene* s, const orc_geom* g, float* invraycov, uint8_t* condition) {
+ * Gaussians get condition = 0 and zeros here.  invraycov [P,6] must arrive zero-filled (rasterize_points.cu:317).
+ * sigma_inv, if not NULL ([P,12], zero-filled), receives the Sigma^-1 each Gaussian in front of the near plane was given, in
+ * the layout this build keeps it: 9 floats column-major, then the flag bits (1 well-conditioned, 2 solver converged). */
+void orc_inte_geometry(const orc_scene* s, const orc_geom* g, float* invraycov, uint8_t* condition, float* sigma_inv) {
 	const float focal_y = s->H / (2.0f * s->tan_fovy), focal_x = s->W / (2.0f * s->tan_fovx);
 	const float* V = s->viewmatrix;
 	for (int idx = 0; idx < s->P; idx++) {
@@ -847,6 +849,12 @@ void orc_inte_geometry(const orc_scene* s, const orc_geom* g, float* invraycov, 
 		m3 Wm = m3_make(V[0], V[4], V[8], V[1], V[5], V[9], V[2], V[6], V[10]);
 		sig_inv si = sigma_inverse(cov6);
 		condition[idx] = (uint8_t)si.well;
+		if (sigma_inv) {
+			float* so = sigma_inv + 12 * idx;
+			for (int c = 0; c < 3; c++) for (int k = 0; k < 3; k++) so[3 * c + k] = si.inv.c[c][k];
+			const int32_t flags = (si.well ? 1 : 0) | (si.solved ? 2 : 0);
+			memcpy(so + 9, &flags, sizeof(flags));
+		}
 		m3 cci = m3_mul(m3_mul(m3_t(Wm), si.inv), Wm);
 		v3 uvh = v3_make(txtz, tytz, 1), uvh_mn = v3_normalize(m3_mulv(cci, uvh));
 		if (isnan(uvh_mn.v[0]) || !si.solved || !si.well) continue;

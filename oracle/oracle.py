@@ -233,8 +233,9 @@ def integrate(inp: Inputs, points3D) -> dict:
     b = binning(W, H, g["radii"], g["means2D"], g["depths"], g["tiles_touched"])
     invraycov = np.zeros((P, 6), np.float32)
     condition = np.zeros(P, np.uint8)
+    sigma_inv = np.zeros((P, 12), np.float32)  # what orc_inte_geometry used: 9 floats column-major, the flag bits in float 9
     sc, cg = inp.c_scene(), _c_geom(g)
-    lib().orc_inte_geometry(C.byref(sc), C.byref(cg), _p(invraycov, _f32p), _p(condition, _u8p))
+    lib().orc_inte_geometry(C.byref(sc), C.byref(cg), _p(invraycov, _f32p), _p(condition, _u8p), _p(sigma_inv, _f32p))
     out = dict(color=np.zeros((9, H, W), np.float32), alpha_integrated=np.ones(PN, np.float32), color_integrated=np.zeros((PN, 3), np.float32),
                point_coordinate=np.zeros((PN, 2), np.float32), point_sdf=np.full(PN, -1000.0, np.float32))
     co = _IntegrateOut(_p(out["color"], _f32p), _p(out["alpha_integrated"], _f32p), _p(out["color_integrated"], _f32p),
@@ -245,7 +246,7 @@ def integrate(inp: Inputs, points3D) -> dict:
     over = lib().orc_integrate(C.c_int(W), C.c_int(H), C.c_float(inp.tanfovx), C.c_float(inp.tanfovy), _p(inp.bg, _f32p), _p(ranges, _u32p),
                                _p(pl, _u32p), C.byref(cg), _p(invraycov, _f32p), _p(condition, _u8p), C.c_int(PN), _p(points3D, _f32p),
                                _p(inp.viewmatrix, _f32p), C.byref(co))
-    out.update(radii=g["radii"], num_rendered=b["num_rendered"], invraycov=invraycov, condition=condition, overflowed=int(over), geom=g, binning=b)
+    out.update(radii=g["radii"], num_rendered=b["num_rendered"], invraycov=invraycov, condition=condition, sigma_inv=sigma_inv, overflowed=int(over), geom=g, binning=b)
     return out
 
 

@@ -104,7 +104,7 @@ def ours_views(fwd: dict, sc) -> dict:
     tiles_touched = g.take(P, torch.int32, 4)
     g.take(P, torch.int32, 4)  # backward preprocess's row list
     clamped = g.take(P, torch.uint8, 1)
-    g.take(P * 12, torch.float32, 4)  # Sigma^-1 kept for backward
+    sigma_inv = g.take(P * 12, torch.float32, 4).view(P, 12)  # Sigma^-1 kept for backward: 9 floats column-major, flag bits in float 9
     b = _Cursor(fwd["binning"])
     point_list = b.take(R, torch.int32, 4)
     keys = b.take(R, torch.int64, 8)
@@ -120,7 +120,7 @@ def ours_views(fwd: dict, sc) -> dict:
     accum_depth = i.take(N if depth else 0, torch.float32, 4).view(-1, sc.width)
     normal_length = i.take(N if (coord or depth) else 0, torch.float32, 4).view(-1, sc.width)
     accum_coord = i.take(3 * N if coord else 0, torch.float32, 4).view(-1, sc.height, sc.width)
-    return dict(totals=totals, records=rec, depths=depths, tiles_touched=tiles_touched, clamped=clamped, point_list=point_list,
+    return dict(totals=totals, records=rec, sigma_inv=sigma_inv, depths=depths, tiles_touched=tiles_touched, clamped=clamped, point_list=point_list,
                 keys=keys, hitmask=hitmask, ranges=ranges, chunk_base=chunk_base, n_contrib=n_contrib,
                 accum_depth=(accum_depth if depth else None), normal_length=(normal_length if (coord or depth) else None),
                 accum_coord=(accum_coord if coord else None),
