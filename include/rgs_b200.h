@@ -275,6 +275,38 @@ int32_t rgs_normal_consistency(int32_t H, int32_t W, int32_t from_depth, float i
                                float w_expected, float w_median, double* loss_sum, float* d_normal, float* d_expected,
                                float* d_median, void* cuda_stream);
 
+/* ---- decoupled-appearance L1 loss (train.py:37-58 with GOF's AppearanceNetwork, scene/appearance_network.py) ----
+ * The image is planar fp32 [3, H0, W0], H0, W0 >= 32.  The crop is H = H0 / 32 * 32 rows by W = W0 / 32 * 32 columns at
+ * top = H0 / 2 - H / 2, left = W0 / 2 - W / 2.  The network's head (conv1, up1..up4) is the caller's; these functions run the
+ * rest.  up4 is the head's output [16, H/2, W/2].  w2 [16,16,3,3], b2 [16], w3 [3,16,3,3], b3 [3] are conv2 and conv3.  All
+ * arithmetic is fp32 (FFMA, no tensor cores); sums are fixed-order, so every output is bit-reproducible from run to run.
+ *
+ * rgs_appearance_downsample: down [3, H/32, W/32] = bilinear, align_corners=True, of the crop.  Source index = s * dst in fp32
+ *   with s = (in - 1) / (out - 1) in fp32, or 0 when out == 1 (torch's rule); taps i0 = (int)src and i0 + 1 (i0 itself at
+ *   the last input row), weights 1 - l and l with l = src - i0.
+ * rgs_appearance_downsample_backward: d_image += the transpose of that map applied to d_down (read-modify-write: the taps of
+ *   different samples are disjoint).  No host synchronisation.
+ * rgs_appearance_l1_forward: X = up4 upsampled x2 (bilinear, align_corners=True, same index rule) to [16, H, W];
+ *   A = relu(conv2(X) + b2); M = sigmoid(conv3(A) + b3) = 1 / (1 + exp(-s)); both convolutions 3x3 with zero padding at the
+ *   crop's border.  loss[0] = mean over the 3 H W crop elements of |M * crop(image) - crop(gt)|, summed per CTA in fp32 per
+ *   tile, across tiles and CTAs in fp64, in a fixed order.  act [16, H, W] (NULL when no backward follows) receives A;
+ *   transformed [3, H, W] (may be NULL) receives M * crop(image).  partials: RGS_APPEARANCE_CTAS doubles of scratch.
+ * rgs_appearance_l1_backward: the gradients of upstream * loss, upstream a DEVICE scalar (NULL: 1).  d_image [3, H0, W0] is fully
+ *   written: sgn(t - gt) * (upstream / (3 H W)) * M inside the crop (sgn(0) = 0), zero outside; the downsample's share is added
+ *   afterwards by rgs_appearance_downsample_backward.  d_up4 [16, H/2, W/2] goes through sigmoid' = M (1 - M), conv3^T, the ReLU
+ *   mask (A > 0), conv2^T and the upsample's transpose as a gather.  d_w2, d_b2, d_w3, d_b3 are the weight and bias gradients:
+ *   each of RGS_APPEARANCE_CTAS CTAs owns a fixed set of tiles and writes one fp64 row of RGS_APPEARANCE_GRAD_FLOATS partial sums
+ *   into partials; the rows are summed in row order.  act is forward's output.  d_x: [16, H, W] floats of scratch. */
+#define RGS_APPEARANCE_CTAS 264
+#define RGS_APPEARANCE_GRAD_FLOATS 2755
+int32_t rgs_appearance_downsample(int32_t H0, int32_t W0, const float* image, float* down, void* cuda_stream);
+int32_t rgs_appearance_downsample_backward(int32_t H0, int32_t W0, const float* d_down, float* d_image, void* cuda_stream);
+int32_t rgs_appearance_l1_forward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* w2, const float* b2,
+                                  const float* w3, const float* b3, float* act, float* transformed, double* partials, float* loss, void* cuda_stream);
+int32_t rgs_appearance_l1_backward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* act, const float* w2,
+                                   const float* w3, const float* b3, const float* upstream, float* d_image, float* d_up4, float* d_w2, float* d_b2,
+                                   float* d_w3, float* d_b3, double* partials, float* d_x, void* cuda_stream);
+
 /* ---- initial Gaussian scales: simple_knn's distCUDA2 (reference scene/gaussian_model.py:20, :315-316) ----
  * points [P,3] (device, fp32) -> mean_dist2 [P] (device): the mean of the squared Euclidean distances from point i to its 3 nearest
  * OTHER points, where "other" is decided by index (an exact duplicate of i is a neighbour at distance 0).  Exact in fp32: every pair

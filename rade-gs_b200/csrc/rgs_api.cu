@@ -981,6 +981,43 @@ int32_t rgs_normal_consistency(int32_t H, int32_t W, int32_t from_depth, float i
 	return after_launch();
 }
 
+static int32_t appearance_size(int32_t H0, int32_t W0) {
+	if (H0 < 32 || W0 < 32) return fail(RGS_E_INVALID, "appearance loss: the image must be at least 32 x 32");
+	if ((int64_t)H0 * W0 > (int64_t)1 << 28) return fail(RGS_E_INVALID, "appearance loss: image too large");
+	return RGS_OK;
+}
+
+static int32_t appearance_status(cudaError_t e) { return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, cudaGetErrorString(e)); }
+
+int32_t rgs_appearance_downsample(int32_t H0, int32_t W0, const float* image, float* down, void* cuda_stream) {
+	if (const int32_t rc = appearance_size(H0, W0)) return rc;
+	if (!image || !down) return fail(RGS_E_INVALID, "null pointer");
+	return appearance_status(launch_appearance_downsample(H0, W0, image, down, (cudaStream_t)cuda_stream));
+}
+
+int32_t rgs_appearance_downsample_backward(int32_t H0, int32_t W0, const float* d_down, float* d_image, void* cuda_stream) {
+	if (const int32_t rc = appearance_size(H0, W0)) return rc;
+	if (!d_down || !d_image) return fail(RGS_E_INVALID, "null pointer");
+	return appearance_status(launch_appearance_downsample_backward(H0, W0, d_down, d_image, (cudaStream_t)cuda_stream));
+}
+
+int32_t rgs_appearance_l1_forward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* w2, const float* b2,
+                                  const float* w3, const float* b3, float* act, float* transformed, double* partials, float* loss, void* cuda_stream) {
+	if (const int32_t rc = appearance_size(H0, W0)) return rc;
+	if (!image || !gt || !up4 || !w2 || !b2 || !w3 || !b3 || !partials || !loss) return fail(RGS_E_INVALID, "null pointer");
+	return appearance_status(launch_appearance_l1_forward(H0, W0, image, gt, up4, w2, b2, w3, b3, act, transformed, partials, loss, (cudaStream_t)cuda_stream));
+}
+
+int32_t rgs_appearance_l1_backward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* act, const float* w2,
+                                   const float* w3, const float* b3, const float* upstream, float* d_image, float* d_up4, float* d_w2, float* d_b2,
+                                   float* d_w3, float* d_b3, double* partials, float* d_x, void* cuda_stream) {
+	if (const int32_t rc = appearance_size(H0, W0)) return rc;
+	if (!image || !gt || !up4 || !act || !w2 || !w3 || !b3 || !d_image || !d_up4 || !d_w2 || !d_b2 || !d_w3 || !d_b3 || !partials || !d_x)
+		return fail(RGS_E_INVALID, "null pointer");
+	return appearance_status(launch_appearance_l1_backward(H0, W0, image, gt, up4, act, w2, w3, b3, upstream, d_image, d_up4, d_w2, d_b2, d_w3, d_b3, partials,
+	                                                       d_x, (cudaStream_t)cuda_stream));
+}
+
 int32_t rgs_debug_get_views(const rgs_camera* cam, int32_t P, int64_t num_rendered, const char* geom_buffer, const char* binning_buffer,
                             const char* image_buffer, rgs_debug_views* views) {
 	if (!cam || !views) return fail(RGS_E_INVALID, "null pointer");

@@ -353,4 +353,13 @@ void launch_normal_consistency(int H, int W, bool from_depth, float inv_fx, floa
                                const float* map_e, const float* map_m, float w_e, float w_m, double* loss_sum, float* d_normal, float* d_e, float* d_m,
                                cudaStream_t s);
 
+// decoupled-appearance L1 loss (rgs_appearance.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
+cudaError_t launch_appearance_downsample(int H0, int W0, const float* img, float* down, cudaStream_t s);
+cudaError_t launch_appearance_downsample_backward(int H0, int W0, const float* d_down, float* d_img, cudaStream_t s);
+cudaError_t launch_appearance_l1_forward(int H0, int W0, const float* img, const float* gt, const float* up4, const float* w2, const float* b2, const float* w3,
+                                         const float* b3, float* act, float* out, double* partials, float* loss, cudaStream_t s);
+cudaError_t launch_appearance_l1_backward(int H0, int W0, const float* img, const float* gt, const float* up4, const float* act, const float* w2, const float* w3,
+                                          const float* b3, const float* upstream, float* d_img, float* d_up4, float* d_w2, float* d_b2, float* d_w3,
+                                          float* d_b3, double* partials, float* d_x, cudaStream_t s);
+
 }  // namespace rgs

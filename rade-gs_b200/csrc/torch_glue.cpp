@@ -675,6 +675,110 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> NormalCon
 	return std::make_tuple(loss, dn, de.view(map_expected.sizes()), dm.view(map_median.sizes()));
 }
 
+// ---- decoupled-appearance L1 loss (train.py:37-58; rgs_appearance_*) -------------------------------------------------------
+
+void appearance_image(const torch::Tensor& t, const char* name) {
+	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
+	TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32");
+	TORCH_CHECK(t.dim() == 3 && t.size(0) == 3, name, " must be [3, H, W]");
+	TORCH_CHECK(t.size(1) >= 32 && t.size(2) >= 32, "appearance loss: the image must be at least 32 x 32, got ", t.sizes());
+}
+
+// image [3,H0,W0] -> the center crop's bilinear downsample [3, H/32, W/32]
+torch::Tensor AppearanceDownsample(const torch::Tensor& image) {
+	appearance_image(image, "image");
+	const c10::cuda::CUDAGuard guard(image.device());
+	const torch::Tensor a = image.contiguous();
+	const int H0 = a.size(1), W0 = a.size(2);
+	torch::Tensor down = new_empty({3, H0 / 32, W0 / 32}, a.options());
+	check(rgs_appearance_downsample(H0, W0, a.data_ptr<float>(), down.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+	return down;
+}
+
+// d_image += the downsample's transpose applied to d_down (in place)
+void AppearanceDownsampleBackward(const torch::Tensor& d_down, torch::Tensor& d_image) {
+	appearance_image(d_image, "d_image");
+	TORCH_CHECK(d_image.is_contiguous(), "d_image must be contiguous");
+	const int H0 = d_image.size(1), W0 = d_image.size(2);
+	torch::Tensor g = image_input(d_down, d_image, "d_down");
+	TORCH_CHECK(g.numel() == 3 * (int64_t)(H0 / 32) * (W0 / 32), "d_down does not belong to this image");
+	const c10::cuda::CUDAGuard guard(d_image.device());
+	check(rgs_appearance_downsample_backward(H0, W0, g.data_ptr<float>(), d_image.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+}
+
+struct AppearanceArgs {
+	torch::Tensor image, gt, up4, w2, b2, w3, b3;
+	int H0, W0;
+};
+
+AppearanceArgs appearance_args(const torch::Tensor& image, const torch::Tensor& gt, const torch::Tensor& up4, const torch::Tensor& w2, const torch::Tensor& b2,
+                               const torch::Tensor& w3, const torch::Tensor& b3) {
+	appearance_image(image, "image");
+	AppearanceArgs a;
+	a.image = image.contiguous();
+	a.H0 = image.size(1);
+	a.W0 = image.size(2);
+	TORCH_CHECK(gt.sizes() == image.sizes(), "gt must have the image's shape");
+	a.gt = image_input(gt, image, "gt");
+	const int64_t H = a.H0 / 32 * 32, W = a.W0 / 32 * 32;
+	a.up4 = image_input(up4, image, "up4 output");
+	TORCH_CHECK(a.up4.numel() == 16 * (H / 2) * (W / 2), "up4 output must be [1, 16, ", H / 2, ", ", W / 2, "], got ", up4.sizes());
+	a.w2 = image_input(w2, image, "conv2 weight");
+	a.b2 = image_input(b2, image, "conv2 bias");
+	a.w3 = image_input(w3, image, "conv3 weight");
+	a.b3 = image_input(b3, image, "conv3 bias");
+	TORCH_CHECK(a.w2.sizes() == torch::IntArrayRef({16, 16, 3, 3}) && a.b2.numel() == 16, "conv2 must be 16 -> 16 with 3x3 kernels");
+	TORCH_CHECK(a.w3.sizes() == torch::IntArrayRef({3, 16, 3, 3}) && a.b3.numel() == 3, "conv3 must be 16 -> 3 with 3x3 kernels");
+	return a;
+}
+
+// returns (loss [] float32, act [16, H, W] or empty, transformed [3, H, W] or empty)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> AppearanceL1Forward(const torch::Tensor& image, const torch::Tensor& gt, const torch::Tensor& up4,
+                                                                             const torch::Tensor& w2, const torch::Tensor& b2, const torch::Tensor& w3,
+                                                                             const torch::Tensor& b3, const bool need_act, const bool want_transformed) {
+	const AppearanceArgs a = appearance_args(image, gt, up4, w2, b2, w3, b3);
+	const c10::cuda::CUDAGuard guard(a.image.device());
+	const int64_t H = a.H0 / 32 * 32, W = a.W0 / 32 * 32;
+	const auto o = a.image.options();
+	torch::Tensor act = need_act ? new_empty({16, H, W}, o) : torch::empty({0}, o);
+	torch::Tensor out = want_transformed ? new_empty({3, H, W}, o) : torch::empty({0}, o);
+	torch::Tensor partials = new_empty({RGS_APPEARANCE_CTAS}, o.dtype(torch::kFloat64));
+	torch::Tensor loss = new_empty({}, o);
+	check(rgs_appearance_l1_forward(a.H0, a.W0, a.image.data_ptr<float>(), a.gt.data_ptr<float>(), a.up4.data_ptr<float>(), a.w2.data_ptr<float>(),
+	                                a.b2.data_ptr<float>(), a.w3.data_ptr<float>(), a.b3.data_ptr<float>(), need_act ? act.data_ptr<float>() : nullptr,
+	                                want_transformed ? out.data_ptr<float>() : nullptr, partials.data_ptr<double>(), loss.data_ptr<float>(),
+	                                at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(loss, act, out);
+}
+
+// returns (d_image [3,H0,W0] (crop term only), d_up4 shaped like up4, d_w2, d_b2, d_w3, d_b3)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> AppearanceL1Backward(
+    const torch::Tensor& image, const torch::Tensor& gt, const torch::Tensor& up4, const torch::Tensor& act, const torch::Tensor& w2, const torch::Tensor& b2,
+    const torch::Tensor& w3, const torch::Tensor& b3, const torch::Tensor& upstream) {
+	const AppearanceArgs a = appearance_args(image, gt, up4, w2, b2, w3, b3);
+	const c10::cuda::CUDAGuard guard(a.image.device());
+	const int64_t H = a.H0 / 32 * 32, W = a.W0 / 32 * 32;
+	const torch::Tensor ac = image_input(act, image, "activations");
+	TORCH_CHECK(ac.numel() == 16 * H * W, "activations do not belong to this image");
+	const float* up_ptr = nullptr;
+	torch::Tensor up;
+	if (upstream.defined() && upstream.numel() != 0) {
+		TORCH_CHECK(upstream.numel() == 1, "appearance loss backward: upstream gradient must be a scalar");
+		up = image_input(upstream, image, "upstream gradient");
+		up_ptr = up.data_ptr<float>();
+	}
+	const auto o = a.image.options();
+	torch::Tensor d_img = new_empty(a.image.sizes(), o), d_up4 = new_empty(up4.sizes(), o);
+	torch::Tensor d_w2 = new_empty(w2.sizes(), o), d_b2 = new_empty(b2.sizes(), o), d_w3 = new_empty(w3.sizes(), o), d_b3 = new_empty(b3.sizes(), o);
+	torch::Tensor partials = new_empty({RGS_APPEARANCE_CTAS, RGS_APPEARANCE_GRAD_FLOATS}, o.dtype(torch::kFloat64));
+	torch::Tensor d_x = new_empty({16, H, W}, o);
+	check(rgs_appearance_l1_backward(a.H0, a.W0, a.image.data_ptr<float>(), a.gt.data_ptr<float>(), a.up4.data_ptr<float>(), ac.data_ptr<float>(),
+	                                 a.w2.data_ptr<float>(), a.w3.data_ptr<float>(), a.b3.data_ptr<float>(), up_ptr, d_img.data_ptr<float>(),
+	                                 d_up4.data_ptr<float>(), d_w2.data_ptr<float>(), d_b2.data_ptr<float>(), d_w3.data_ptr<float>(), d_b3.data_ptr<float>(),
+	                                 partials.data_ptr<double>(), d_x.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(d_img, d_up4, d_w2, d_b2, d_w3, d_b3);
+}
+
 // simple_knn's distCUDA2 (reference scene/gaussian_model.py:315-316): points [P,3] float32 on a CUDA device -> [P] float32,
 // the mean squared distance to the 3 nearest other points (rgs_knn_mean_dist2).  Non-contiguous input is accepted.
 torch::Tensor KnnMeanDist2(const torch::Tensor& points) {
@@ -1177,6 +1281,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("ssim_l1_backward", &SsimL1Backward, py::arg("img"), py::arg("gt"), py::arg("dmaps"), py::arg("w_ssim"), py::arg("w_l1"), py::arg("upstream"),
 	      py::arg("row_lo") = 0, py::arg("row_hi") = -1);
 	m.def("normal_consistency", &NormalConsistency);
+	m.def("appearance_downsample", &AppearanceDownsample, py::arg("image"));
+	m.def("appearance_downsample_backward", &AppearanceDownsampleBackward, py::arg("d_down"), py::arg("d_image"));
+	m.def("appearance_l1_forward", &AppearanceL1Forward, py::arg("image"), py::arg("gt"), py::arg("up4"), py::arg("w2"), py::arg("b2"), py::arg("w3"),
+	      py::arg("b3"), py::arg("need_act"), py::arg("want_transformed"));
+	m.def("appearance_l1_backward", &AppearanceL1Backward, py::arg("image"), py::arg("gt"), py::arg("up4"), py::arg("act"), py::arg("w2"), py::arg("b2"),
+	      py::arg("w3"), py::arg("b3"), py::arg("upstream"));
 	m.def("activate_forward", &ActivateForward);
 	m.def("activate_backward", &ActivateBackward);
 	m.def("densification_stats", &DensificationStats);
