@@ -63,6 +63,23 @@ static int fail(int code, const std::string& msg) {
 		if (_e != cudaSuccess) return fail(RGS_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
 	} while (0)
 
+// A launcher's result as a status of entry `what`.  The DTU and TNT launchers report a non-finite input point as
+// cudaErrorInvalidValue; they pass `invalid`, the message that turns it into RGS_E_INVALID.
+static int cuda_status(cudaError_t e, const char* what, const char* invalid = nullptr) {
+	if (e == cudaSuccess) return RGS_OK;
+	if (invalid && e == cudaErrorInvalidValue) return fail(RGS_E_INVALID, std::string(what) + ": " + invalid);
+	return fail(RGS_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+}
+
+static const char* const kNonFinitePoint = "a point has a NaN or infinite coordinate";
+
+// `bytes` from the caller's resize callback into `buf`.  NULL is a failure only when bytes were asked for: an empty
+// output may come back as NULL.
+static int grow(rgs_resize_fn fn, void* user, size_t bytes, char*& buf, const char* what) {
+	buf = fn(user, bytes);
+	return buf || bytes == 0 ? (int)RGS_OK : fail(RGS_E_ALLOC, std::string(what) + " callback returned NULL");
+}
+
 // After each stage in debug mode: synchronise and surface the error, like CHECK_CUDA (auxiliary.h:404-411).
 static int debug_sync(const rgs_camera* cam, cudaStream_t s, const char* stage) {
 	cudaError_t e = cudaGetLastError();
@@ -216,14 +233,14 @@ static int64_t forward_to_binning(const rgs_camera* cam, const FwdParams& p, int
 	// image-side scratch first: needed even when there is nothing to draw (background fill)
 	size_t img_bytes = 0;
 	carve_img(nullptr, p.grid_x, p.grid_y, N, p.coord, p.depth, &img_bytes);
-	char* img_ptr = bufs->image(bufs->image_user, img_bytes);
-	if (!img_ptr) return fail(RGS_E_ALLOC, "image buffer callback returned NULL");
+	char* img_ptr;
+	if ((rc = grow(bufs->image, bufs->image_user, img_bytes, img_ptr, "image buffer")) != RGS_OK) return rc;
 	img = carve_img(img_ptr, p.grid_x, p.grid_y, N, p.coord, p.depth, nullptr);
 
 	size_t geom_bytes = 0;
 	carve_geom(nullptr, P, p.coord, &geom_bytes);
-	char* geom_ptr = bufs->geom(bufs->geom_user, geom_bytes);
-	if (!geom_ptr) return fail(RGS_E_ALLOC, "geometry buffer callback returned NULL");
+	char* geom_ptr;
+	if ((rc = grow(bufs->geom, bufs->geom_user, geom_bytes, geom_ptr, "geometry buffer")) != RGS_OK) return rc;
 	g = carve_geom(geom_ptr, P, p.coord, nullptr);
 
 	int64_t R = 0;
@@ -244,8 +261,8 @@ static int64_t forward_to_binning(const rgs_camera* cam, const FwdParams& p, int
 	}
 	size_t bin_bytes = 0;
 	carve_bin(nullptr, (size_t)R, tiles, &bin_bytes);
-	char* bin_ptr = bufs->binning(bufs->binning_user, bin_bytes);
-	if (!bin_ptr) return fail(RGS_E_ALLOC, "binning buffer callback returned NULL");
+	char* bin_ptr;
+	if ((rc = grow(bufs->binning, bufs->binning_user, bin_bytes, bin_ptr, "binning buffer")) != RGS_OK) return rc;
 	b = carve_bin(bin_ptr, (size_t)R, tiles, nullptr);
 	// forward-render writes a ballot word only for the chunks a warp actually tested; backward masks every position at or
 	// behind the warp's last contributor, so the unwritten words never matter -- zero them anyway (<= R bytes) so that no
@@ -310,10 +327,7 @@ int64_t rgs_integrate(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_
 	size_t bytes = 0;
 	for (int pass = 0; pass < 2; pass++) {
 		char* base = nullptr;
-		if (pass == 1) {
-			base = point_buffer(point_buffer_user, bytes);
-			if (!base) return fail(RGS_E_ALLOC, "point buffer callback returned NULL");
-		}
+		if (pass == 1 && (rc = grow(point_buffer, point_buffer_user, bytes, base, "point buffer")) != RGS_OK) return rc;
 		Carver cv(base);
 		v.PN = PN;
 		v.points3D = io->points3D;
@@ -442,8 +456,9 @@ int32_t rgs_backward(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_b
 	if (!grad_scratch) return fail(RGS_E_INVALID, "null scratch callback");
 	if (!out) return fail(RGS_E_INVALID, "null gradient accumulator / outputs");
 	const size_t bytes = (size_t)gs->P * grad_floats(cam->require_coord != 0) * sizeof(float);
-	float* acc = reinterpret_cast<float*>(grad_scratch(grad_scratch_user, bytes));
-	if (!acc) return fail(RGS_E_ALLOC, "gradient scratch callback returned NULL");
+	char* acc_bytes;
+	if (const int rc = grow(grad_scratch, grad_scratch_user, bytes, acc_bytes, "gradient scratch")) return rc;
+	float* acc = reinterpret_cast<float*>(acc_bytes);
 	cudaStream_t s = (cudaStream_t)cuda_stream;
 	// The zero-fill of the dense gradient tensors (pure HBM writes, ~280 MB at 1 M Gaussians) runs on a side stream underneath the
 	// issue-bound backward blend; everything queued on `s` before this call is ordered before it (the tensors may be recycled memory).
@@ -470,9 +485,7 @@ int32_t rgs_mark_visible(int32_t P, const float* means3D, const float* viewmatri
 	if (P == 0) return RGS_OK;
 	if (!means3D || !viewmatrix || !present) return fail(RGS_E_INVALID, "null pointer");
 	launch_mark_visible(P, means3D, viewmatrix, present, (cudaStream_t)cuda_stream);
-	cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess) return fail(RGS_E_CUDA, cudaGetErrorString(e));
-	return RGS_OK;
+	return cuda_status(cudaGetLastError(), "mark visible");
 }
 
 int32_t rgs_activate_forward(int32_t P, const float* raw_scaling, const float* raw_opacity, const float* raw_rotation, const float* filter_3D,
@@ -481,8 +494,7 @@ int32_t rgs_activate_forward(int32_t P, const float* raw_scaling, const float* r
 	if (P == 0) return RGS_OK;
 	if (!raw_scaling || !raw_opacity || !raw_rotation || !filter_3D || !scales || !opacity || !rotations) return fail(RGS_E_INVALID, "null pointer");
 	launch_activate_forward(P, raw_scaling, raw_opacity, raw_rotation, filter_3D, scales, opacity, rotations, (cudaStream_t)cuda_stream);
-	cudaError_t e = cudaGetLastError();
-	return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, cudaGetErrorString(e));
+	return cuda_status(cudaGetLastError(), "activate forward");
 }
 
 int32_t rgs_activate_backward(int32_t P, const float* raw_scaling, const float* raw_opacity, const float* raw_rotation, const float* filter_3D,
@@ -495,8 +507,7 @@ int32_t rgs_activate_backward(int32_t P, const float* raw_scaling, const float* 
 		return fail(RGS_E_INVALID, "null pointer");
 	launch_activate_backward(P, raw_scaling, raw_opacity, raw_rotation, filter_3D, g_scales, g_opacity, g_rotations, d_raw_scaling, d_raw_opacity,
 	                         d_raw_rotation, (cudaStream_t)cuda_stream);
-	cudaError_t e = cudaGetLastError();
-	return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, cudaGetErrorString(e));
+	return cuda_status(cudaGetLastError(), "activate backward");
 }
 
 int32_t rgs_densification_stats(int32_t P, const float* means2D_grad, const int32_t* radii, float* grad_accum, float* grad_accum_abs,
@@ -505,13 +516,7 @@ int32_t rgs_densification_stats(int32_t P, const float* means2D_grad, const int3
 	if (P == 0) return RGS_OK;
 	if (!means2D_grad || !radii || !grad_accum || !grad_accum_abs || !grad_accum_abs_max || !denom) return fail(RGS_E_INVALID, "null pointer");
 	launch_densification_stats(P, means2D_grad, radii, grad_accum, grad_accum_abs, grad_accum_abs_max, denom, max_radii2D, (cudaStream_t)cuda_stream);
-	cudaError_t e = cudaGetLastError();
-	return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, cudaGetErrorString(e));
-}
-
-static int32_t after_launch() {
-	cudaError_t e = cudaGetLastError();
-	return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, cudaGetErrorString(e));
+	return cuda_status(cudaGetLastError(), "densification stats");
 }
 
 int32_t rgs_compute_3d_filter(int32_t P, const float* xyz, int32_t n_cams, const float* cams, float focal_length, float* filter_3D,
@@ -521,17 +526,16 @@ int32_t rgs_compute_3d_filter(int32_t P, const float* xyz, int32_t n_cams, const
 	if (!xyz || !filter_3D || !max_distance || (n_cams > 0 && !cams)) return fail(RGS_E_INVALID, "null pointer");
 	if (!(focal_length > 0.0f)) return fail(RGS_E_INVALID, "focal_length must be positive");
 	launch_compute_3d_filter(P, xyz, n_cams, cams, focal_length, filter_3D, max_distance, (cudaStream_t)cuda_stream);
-	return after_launch();
+	return cuda_status(cudaGetLastError(), "compute 3d filter");
 }
 
 int32_t rgs_knn_mean_dist2(int32_t P, const float* points, float* mean_dist2, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
 	if (P < 0) return fail(RGS_E_INVALID, "negative point count");
 	if (P == 0) return RGS_OK;
 	if (!points || !mean_dist2 || !scratch) return fail(RGS_E_INVALID, "null pointer");
-	char* buf = scratch(scratch_user, knn_scratch_bytes(P));
-	if (!buf) return fail(RGS_E_ALLOC, "knn scratch callback returned NULL");
-	const cudaError_t e = launch_knn_mean_dist2(P, points, mean_dist2, buf, (cudaStream_t)cuda_stream);
-	return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, std::string("knn: ") + cudaGetErrorString(e));
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, knn_scratch_bytes(P), buf, "knn scratch")) return rc;
+	return cuda_status(launch_knn_mean_dist2(P, points, mean_dist2, buf, (cudaStream_t)cuda_stream), "knn");
 }
 
 // ---- TSDF grid (rgs_tsdf.cu) ----
@@ -579,18 +583,13 @@ static int tsdf_camera_check(const rgs_tsdf_grid* g, const rgs_tsdf_camera* c) {
 static int tsdf_read_counters(const rgs_tsdf_grid* g, int32_t* cnt, cudaStream_t s) {
 	cudaError_t e = cudaMemcpyAsync(cnt, g->counters, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
 	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-	if (e != cudaSuccess) return fail(RGS_E_CUDA, std::string("tsdf: ") + cudaGetErrorString(e));
-	return RGS_OK;
+	return cuda_status(e, "tsdf");
 }
 
 static int tsdf_flags_check(const int32_t* cnt) {
 	if (cnt[2] & RGS_TSDF_BAD_COORD) return fail(RGS_E_INVALID, "tsdf: an integrate call was given a block coordinate outside [-2^20, 2^20)");
 	if (cnt[2] & RGS_TSDF_OVERFLOW) return fail(RGS_E_INVALID, "tsdf: an integrate call found no free block slot; the grid is incomplete");
 	return RGS_OK;
-}
-
-static int tsdf_cuda(cudaError_t e, const char* what) {
-	return e == cudaSuccess ? (int)RGS_OK : fail(RGS_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
 }
 
 int64_t rgs_tsdf_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, const float* depth, int32_t* block_coords, int64_t* allocated,
@@ -601,15 +600,15 @@ int64_t rgs_tsdf_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, co
 	if (!depth || !block_coords || !scratch) return fail(RGS_E_INVALID, "null pointer");
 	const cudaStream_t s = (cudaStream_t)cuda_stream;
 	int32_t cnt[4];
-	if ((rc = tsdf_cuda(launch_tsdf_touch(*grid, *cam, depth, cnt, s), "tsdf touch")) != RGS_OK) return rc;
+	if ((rc = cuda_status(launch_tsdf_touch(*grid, *cam, depth, cnt, s), "tsdf touch")) != RGS_OK) return rc;
 	if ((rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
 	if (allocated) *allocated = cnt[0];
 	if (cnt[3] || cnt[1] > grid->frame_slots / 2) return fail(RGS_E_CAPACITY, "tsdf touch: more blocks than the frame-local hash holds");
 	const int64_t n = cnt[1];
 	if (n == 0) return 0;
-	char* buf = scratch(scratch_user, tsdf_touch_scratch_bytes(n));
-	if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
-	if ((rc = tsdf_cuda(launch_tsdf_touch_sort(*grid, n, block_coords, buf, s), "tsdf touch")) != RGS_OK) return rc;
+	char* buf;
+	if ((rc = grow(scratch, scratch_user, tsdf_touch_scratch_bytes(n), buf, "tsdf scratch")) != RGS_OK) return rc;
+	if ((rc = cuda_status(launch_tsdf_touch_sort(*grid, n, block_coords, buf, s), "tsdf touch")) != RGS_OK) return rc;
 	return n;
 }
 
@@ -622,9 +621,9 @@ int32_t rgs_tsdf_integrate(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam
 	if (call_id <= 0) return fail(RGS_E_INVALID, "call_id must be positive");
 	if (n == 0) return RGS_OK;
 	if (!block_coords || !depth || !color || !scratch) return fail(RGS_E_INVALID, "null pointer");
-	char* buf = scratch(scratch_user, (size_t)n * sizeof(int32_t));
-	if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
-	return tsdf_cuda(launch_tsdf_integrate(*grid, *cam, n, block_coords, depth, color, call_id, reinterpret_cast<int32_t*>(buf), (cudaStream_t)cuda_stream),
+	char* buf;
+	if ((rc = grow(scratch, scratch_user, (size_t)n * sizeof(int32_t), buf, "tsdf scratch")) != RGS_OK) return rc;
+	return cuda_status(launch_tsdf_integrate(*grid, *cam, n, block_coords, depth, color, call_id, reinterpret_cast<int32_t*>(buf), (cudaStream_t)cuda_stream),
 	                 "tsdf integrate");
 }
 
@@ -634,7 +633,7 @@ int32_t rgs_tsdf_rehash(const rgs_tsdf_grid* grid, const uint64_t* old_keys, con
 	if (old_slots < 0) return fail(RGS_E_INVALID, "negative slot count");
 	if (old_slots == 0) return RGS_OK;
 	if (!old_keys || !old_values) return fail(RGS_E_INVALID, "null pointer");
-	return tsdf_cuda(launch_tsdf_rehash(*grid, old_keys, old_values, old_slots, (cudaStream_t)cuda_stream), "tsdf rehash");
+	return cuda_status(launch_tsdf_rehash(*grid, old_keys, old_values, old_slots, (cudaStream_t)cuda_stream), "tsdf rehash");
 }
 
 int64_t rgs_tsdf_active_blocks(const rgs_tsdf_grid* grid, uint64_t* keys, int32_t* pool_index, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
@@ -646,9 +645,9 @@ int64_t rgs_tsdf_active_blocks(const rgs_tsdf_grid* grid, uint64_t* keys, int32_
 	if ((rc = tsdf_read_counters(grid, cnt, s)) != RGS_OK || (rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
 	const int N = cnt[0];
 	if (N == 0) return 0;
-	char* buf = scratch(scratch_user, tsdf_active_scratch_bytes(N));
-	if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
-	if ((rc = tsdf_cuda(launch_tsdf_active(*grid, N, keys, pool_index, buf, s), "tsdf active blocks")) != RGS_OK) return rc;
+	char* buf;
+	if ((rc = grow(scratch, scratch_user, tsdf_active_scratch_bytes(N), buf, "tsdf scratch")) != RGS_OK) return rc;
+	if ((rc = cuda_status(launch_tsdf_active(*grid, N, keys, pool_index, buf, s), "tsdf active blocks")) != RGS_OK) return rc;
 	return N;
 }
 
@@ -665,18 +664,18 @@ int32_t rgs_tsdf_extract(const rgs_tsdf_grid* grid, float weight_threshold, rgs_
 	int64_t totals[2] = {0, 0};
 	char* buf = nullptr;
 	if (N > 0) {
-		buf = resize(scratch_user, tsdf_extract_scratch_bytes(*grid, N));
-		if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
-		if ((rc = tsdf_cuda(launch_tsdf_extract_count(*grid, N, weight_threshold, buf, totals, s), "tsdf extract")) != RGS_OK) return rc;
+		if ((rc = grow(resize, scratch_user, tsdf_extract_scratch_bytes(*grid, N), buf, "tsdf scratch")) != RGS_OK) return rc;
+		if ((rc = cuda_status(launch_tsdf_extract_count(*grid, N, weight_threshold, buf, totals, s), "tsdf extract")) != RGS_OK) return rc;
 	}
 	out->num_vertices = totals[0];
 	out->num_triangles = totals[1];
-	char* v = resize(out->vertices_user, (size_t)totals[0] * 3 * sizeof(float));
-	char* c = resize(out->colors_user, (size_t)totals[0] * 3 * sizeof(float));
-	char* t = resize(out->triangles_user, (size_t)totals[1] * 3 * sizeof(int32_t));
-	if ((totals[0] > 0 && (!v || !c)) || (totals[1] > 0 && !t)) return fail(RGS_E_ALLOC, "tsdf mesh callback returned NULL");
+	char *v, *c, *t;
+	if ((rc = grow(resize, out->vertices_user, (size_t)totals[0] * 3 * sizeof(float), v, "tsdf mesh")) != RGS_OK ||
+	    (rc = grow(resize, out->colors_user, (size_t)totals[0] * 3 * sizeof(float), c, "tsdf mesh")) != RGS_OK ||
+	    (rc = grow(resize, out->triangles_user, (size_t)totals[1] * 3 * sizeof(int32_t), t, "tsdf mesh")) != RGS_OK)
+		return rc;
 	if (N == 0) return RGS_OK;
-	return tsdf_cuda(launch_tsdf_extract_emit(*grid, N, buf, reinterpret_cast<float*>(v), reinterpret_cast<float*>(c), reinterpret_cast<int32_t*>(t), s),
+	return cuda_status(launch_tsdf_extract_emit(*grid, N, buf, reinterpret_cast<float*>(v), reinterpret_cast<float*>(c), reinterpret_cast<int32_t*>(t), s),
 	                 "tsdf extract");
 }
 
@@ -685,17 +684,12 @@ int32_t rgs_tsdf_vertex_normals(int64_t V, const float* vertices, int64_t F, con
 	if (V < 0 || F < 0 || V > INT32_MAX || 3 * F > INT32_MAX) return fail(RGS_E_INVALID, "vertex / triangle count out of range");
 	if (V == 0) return F == 0 ? (int32_t)RGS_OK : fail(RGS_E_INVALID, "triangles without vertices");
 	if (!vertices || !normals || !scratch || (F > 0 && !triangles)) return fail(RGS_E_INVALID, "null pointer");
-	char* buf = scratch(scratch_user, tsdf_normals_scratch_bytes(V, F));
-	if (!buf) return fail(RGS_E_ALLOC, "tsdf scratch callback returned NULL");
-	return tsdf_cuda(launch_tsdf_normals(V, vertices, F, triangles, normals, buf, (cudaStream_t)cuda_stream), "tsdf vertex normals");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, tsdf_normals_scratch_bytes(V, F), buf, "tsdf scratch")) return rc;
+	return cuda_status(launch_tsdf_normals(V, vertices, F, triangles, normals, buf, (cudaStream_t)cuda_stream), "tsdf vertex normals");
 }
 
 // ---- DTU evaluation (rgs_dtu_eval.cu) ----
-
-static int dtu_cuda(cudaError_t e, const char* what) {
-	if (e == cudaErrorInvalidValue) return fail(RGS_E_INVALID, std::string(what) + ": a point has a NaN or infinite coordinate");
-	return e == cudaSuccess ? (int)RGS_OK : fail(RGS_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-}
 
 int32_t rgs_dtu_sample_mesh(int64_t V, const double* vertices, int64_t F, const int32_t* faces, double density, rgs_resize_fn resize,
                             rgs_dtu_samples_out* out, void* cuda_stream) {
@@ -703,23 +697,24 @@ int32_t rgs_dtu_sample_mesh(int64_t V, const double* vertices, int64_t F, const 
 	if (!resize || !out || (V > 0 && !vertices) || (F > 0 && !faces)) return fail(RGS_E_INVALID, "null pointer");
 	if (!(std::isfinite(density) && density > 0.0)) return fail(RGS_E_INVALID, "dtu sample: density must be positive and finite");
 	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int rc;
 	int64_t totals[2] = {0, 0};   // samples, rows
 	char* buf = nullptr;
 	if (F > 0) {
 		if (V == 0) return fail(RGS_E_INVALID, "dtu sample: faces without vertices");
-		buf = resize(out->scratch_user, dtu_sample_scratch_bytes(F));
-		if (!buf) return fail(RGS_E_ALLOC, "dtu sample scratch callback returned NULL");
-		const cudaError_t e = launch_dtu_sample_count(V, vertices, F, faces, density, buf, totals, s);
-		if (e != cudaSuccess) return fail(RGS_E_CUDA, std::string("dtu sample: ") + cudaGetErrorString(e));
+		if ((rc = grow(resize, out->scratch_user, dtu_sample_scratch_bytes(F), buf, "dtu sample scratch")) != RGS_OK ||
+		    (rc = cuda_status(launch_dtu_sample_count(V, vertices, F, faces, density, buf, totals, s), "dtu sample")) != RGS_OK)
+			return rc;
 		if (V + totals[0] > INT32_MAX)
 			return fail(RGS_E_INVALID, "dtu sample: more than 2^31 - 1 points (or a face index outside [0, V), or a triangle whose sample count is not finite)");
 	}
 	out->num_points = V + totals[0];
-	char* rows = totals[0] > 0 ? resize(out->rows_user, dtu_sample_rows_bytes(totals[1])) : nullptr;
-	char* pts = resize(out->points_user, (size_t)out->num_points * 3 * sizeof(double));
-	if ((totals[0] > 0 && !rows) || (out->num_points > 0 && !pts)) return fail(RGS_E_ALLOC, "dtu sample callback returned NULL");
+	char *rows = nullptr, *pts;
+	if ((totals[0] > 0 && (rc = grow(resize, out->rows_user, dtu_sample_rows_bytes(totals[1]), rows, "dtu sample")) != RGS_OK) ||
+	    (rc = grow(resize, out->points_user, (size_t)out->num_points * 3 * sizeof(double), pts, "dtu sample")) != RGS_OK)
+		return rc;
 	if (out->num_points == 0) return RGS_OK;
-	return dtu_cuda(launch_dtu_sample_emit(V, vertices, F, faces, density, buf, totals[0], totals[1], rows, reinterpret_cast<double*>(pts), s), "dtu sample");
+	return cuda_status(launch_dtu_sample_emit(V, vertices, F, faces, density, buf, totals[0], totals[1], rows, reinterpret_cast<double*>(pts), s), "dtu sample", kNonFinitePoint);
 }
 
 int32_t rgs_dtu_radius_downsample(int64_t N, const double* points, double radius, uint8_t* kept, int32_t* rounds, rgs_resize_fn scratch,
@@ -729,9 +724,9 @@ int32_t rgs_dtu_radius_downsample(int64_t N, const double* points, double radius
 	if (!(std::isfinite(radius) && radius > 0.0)) return fail(RGS_E_INVALID, "dtu downsample: radius must be positive and finite");
 	if (N == 0) return RGS_OK;
 	if (!points || !kept || !scratch) return fail(RGS_E_INVALID, "null pointer");
-	char* buf = scratch(scratch_user, dtu_downsample_scratch_bytes((int)N));
-	if (!buf) return fail(RGS_E_ALLOC, "dtu downsample scratch callback returned NULL");
-	return dtu_cuda(launch_dtu_downsample((int)N, points, radius, kept, buf, rounds, (cudaStream_t)cuda_stream), "dtu downsample");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, dtu_downsample_scratch_bytes((int)N), buf, "dtu downsample scratch")) return rc;
+	return cuda_status(launch_dtu_downsample((int)N, points, radius, kept, buf, rounds, (cudaStream_t)cuda_stream), "dtu downsample", kNonFinitePoint);
 }
 
 int32_t rgs_dtu_nearest(int64_t M, const double* reference, int64_t N, const double* query, double* dist, int64_t* index, rgs_resize_fn scratch,
@@ -739,22 +734,22 @@ int32_t rgs_dtu_nearest(int64_t M, const double* reference, int64_t N, const dou
 	if (M < 0 || N < 0 || M > INT32_MAX || N > INT32_MAX) return fail(RGS_E_INVALID, "dtu nearest: point count out of range");
 	if (M == 0) return fail(RGS_E_INVALID, "dtu nearest: the reference set is empty");
 	if (!reference || !scratch || (N > 0 && (!query || !dist || !index))) return fail(RGS_E_INVALID, "null pointer");
-	char* buf = scratch(scratch_user, dtu_nearest_scratch_bytes((int)M, (int)N));
-	if (!buf) return fail(RGS_E_ALLOC, "dtu nearest scratch callback returned NULL");
-	return dtu_cuda(launch_dtu_nearest((int)M, reference, (int)N, query, dist, index, buf, (cudaStream_t)cuda_stream), "dtu nearest");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, dtu_nearest_scratch_bytes((int)M, (int)N), buf, "dtu nearest scratch")) return rc;
+	return cuda_status(launch_dtu_nearest((int)M, reference, (int)N, query, dist, index, buf, (cudaStream_t)cuda_stream), "dtu nearest", kNonFinitePoint);
 }
 
 int32_t rgs_dtu_dilate_masks(int32_t n_views, int32_t H, int32_t W, const uint8_t* masks, uint8_t* dilated, void* cuda_stream) {
 	if (n_views < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "dtu dilate: image size must be positive");
 	if (n_views > 0 && (!masks || !dilated)) return fail(RGS_E_INVALID, "null pointer");
-	return dtu_cuda(launch_dtu_dilate(n_views, H, W, masks, dilated, (cudaStream_t)cuda_stream), "dtu dilate");
+	return cuda_status(launch_dtu_dilate(n_views, H, W, masks, dilated, (cudaStream_t)cuda_stream), "dtu dilate", kNonFinitePoint);
 }
 
 int32_t rgs_dtu_cull_vertices(int64_t V, const double* vertices, int32_t n_views, int32_t H, int32_t W, const double* proj, const uint8_t* dilated,
                               uint8_t* keep, void* cuda_stream) {
 	if (V < 0 || n_views < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "dtu cull: negative count or empty image");
 	if (V > 0 && (!vertices || !keep || (n_views > 0 && (!proj || !dilated)))) return fail(RGS_E_INVALID, "null pointer");
-	return dtu_cuda(launch_dtu_cull(V, vertices, n_views, H, W, proj, dilated, keep, (cudaStream_t)cuda_stream), "dtu cull");
+	return cuda_status(launch_dtu_cull(V, vertices, n_views, H, W, proj, dilated, keep, (cudaStream_t)cuda_stream), "dtu cull", kNonFinitePoint);
 }
 
 // ---- TNT evaluation (rgs_tnt_eval.cu) ----
@@ -781,12 +776,12 @@ int32_t rgs_tnt_crop(int64_t N, const double* points, const double* transform, c
 	}
 	if (N == 0) return RGS_OK;
 	if (!points || !kept || !cropped || !scratch) return fail(RGS_E_INVALID, "null pointer");
-	char* buf = scratch(scratch_user, tnt_crop_scratch_bytes((int)N));
-	if (!buf) return fail(RGS_E_ALLOC, "tnt crop scratch callback returned NULL");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, tnt_crop_scratch_bytes((int)N), buf, "tnt crop scratch")) return rc;
 	const cudaError_t e = launch_tnt_crop((int)N, points, transform, volume ? volume->orthogonal_axis : 0, volume ? volume->axis_min : 0.0,
 	                                      volume ? volume->axis_max : 0.0, volume ? volume->num_vertices : 0, volume ? volume->polygon : nullptr, kept,
 	                                      cropped, num_kept, buf, (cudaStream_t)cuda_stream);
-	return dtu_cuda(e, "tnt crop");
+	return cuda_status(e, "tnt crop", kNonFinitePoint);
 }
 
 int32_t rgs_tnt_transform(int64_t N, double* points, const double* transform, void* cuda_stream) {
@@ -794,7 +789,7 @@ int32_t rgs_tnt_transform(int64_t N, double* points, const double* transform, vo
 	if (!transform) return fail(RGS_E_INVALID, "null pointer");
 	if (const int rc = tnt_check_transform(transform, "tnt transform")) return rc;
 	if (N > 0 && !points) return fail(RGS_E_INVALID, "null pointer");
-	return dtu_cuda(launch_tnt_transform(N, points, transform, (cudaStream_t)cuda_stream), "tnt transform");
+	return cuda_status(launch_tnt_transform(N, points, transform, (cudaStream_t)cuda_stream), "tnt transform", kNonFinitePoint);
 }
 
 int32_t rgs_tnt_voxel_downsample(int64_t N, const double* points, double voxel, rgs_resize_fn resize, rgs_tnt_voxel_out* out, void* cuda_stream) {
@@ -804,13 +799,14 @@ int32_t rgs_tnt_voxel_downsample(int64_t N, const double* points, double voxel, 
 	if (!(std::isfinite(voxel) && voxel > 0.0)) return fail(RGS_E_INVALID, "tnt voxel: voxel size must be positive and finite");
 	if (N > 0 && !points) return fail(RGS_E_INVALID, "null pointer");
 	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int rc;
 	double lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0}, origin[3] = {0, 0, 0};
 	if (N > 0) {
-		char* bbuf = resize(out->scratch_user, tnt_bounds_scratch_bytes());
-		if (!bbuf) return fail(RGS_E_ALLOC, "tnt voxel scratch callback returned NULL");
+		char* bbuf;
 		int64_t bad = 0;
-		const cudaError_t e = launch_tnt_bounds((int)N, points, bbuf, lo, hi, &bad, s);
-		if (e != cudaSuccess) return fail(RGS_E_CUDA, std::string("tnt voxel: ") + cudaGetErrorString(e));
+		if ((rc = grow(resize, out->scratch_user, tnt_bounds_scratch_bytes(), bbuf, "tnt voxel scratch")) != RGS_OK ||
+		    (rc = cuda_status(launch_tnt_bounds((int)N, points, bbuf, lo, hi, &bad, s), "tnt voxel")) != RGS_OK)
+			return rc;
 		if (bad) return fail(RGS_E_INVALID, "tnt voxel: a point has a NaN or infinite coordinate");
 		for (int a = 0; a < 3; a++) {
 			origin[a] = lo[a] - voxel * 0.5;
@@ -818,19 +814,18 @@ int32_t rgs_tnt_voxel_downsample(int64_t N, const double* points, double voxel, 
 			if (!(top < 2097152.0)) return fail(RGS_E_INVALID, "tnt voxel: more than 2^21 voxels along an axis");
 		}
 	}
-	char* buf = N > 0 ? resize(out->scratch_user, tnt_voxel_scratch_bytes((int)N)) : nullptr;
-	if (N > 0 && !buf) return fail(RGS_E_ALLOC, "tnt voxel scratch callback returned NULL");
+	char* buf = nullptr;
 	int32_t V = 0;
-	if (N > 0) {
-		const cudaError_t e = launch_tnt_voxel_sort((int)N, points, origin, voxel, buf, &V, s);
-		if (e != cudaSuccess) return fail(RGS_E_CUDA, std::string("tnt voxel: ") + cudaGetErrorString(e));
-	}
+	if (N > 0 && ((rc = grow(resize, out->scratch_user, tnt_voxel_scratch_bytes((int)N), buf, "tnt voxel scratch")) != RGS_OK ||
+	              (rc = cuda_status(launch_tnt_voxel_sort((int)N, points, origin, voxel, buf, &V, s), "tnt voxel")) != RGS_OK))
+		return rc;
 	out->num_voxels = V;
-	char* means = resize(out->means_user, (size_t)V * 3 * sizeof(double));
-	char* counts = resize(out->counts_user, (size_t)V * sizeof(int64_t));
-	if (V > 0 && (!means || !counts)) return fail(RGS_E_ALLOC, "tnt voxel callback returned NULL");
+	char *means, *counts;
+	if ((rc = grow(resize, out->means_user, (size_t)V * 3 * sizeof(double), means, "tnt voxel")) != RGS_OK ||
+	    (rc = grow(resize, out->counts_user, (size_t)V * sizeof(int64_t), counts, "tnt voxel")) != RGS_OK)
+		return rc;
 	if (V == 0) return RGS_OK;
-	return dtu_cuda(launch_tnt_voxel_mean((int)N, points, V, buf, reinterpret_cast<double*>(means), reinterpret_cast<int64_t*>(counts), s), "tnt voxel");
+	return cuda_status(launch_tnt_voxel_mean((int)N, points, V, buf, reinterpret_cast<double*>(means), reinterpret_cast<int64_t*>(counts), s), "tnt voxel", kNonFinitePoint);
 }
 
 int32_t rgs_tnt_icp_moments(int64_t N, const double* source, int64_t M, const double* target, const double* dist, const int64_t* index, double threshold,
@@ -838,24 +833,19 @@ int32_t rgs_tnt_icp_moments(int64_t N, const double* source, int64_t M, const do
 	if (N < 0 || M < 0 || N > INT32_MAX || M > INT32_MAX) return fail(RGS_E_INVALID, "tnt moments: point count out of range");
 	if (std::isnan(threshold)) return fail(RGS_E_INVALID, "tnt moments: the threshold is NaN");
 	if (!moments || !scratch || (N > 0 && (!source || !dist || !index)) || (M > 0 && !target)) return fail(RGS_E_INVALID, "null pointer");
-	char* buf = scratch(scratch_user, tnt_moments_scratch_bytes(N));
-	if (!buf) return fail(RGS_E_ALLOC, "tnt moments scratch callback returned NULL");
-	const cudaError_t e = launch_tnt_moments(N, source, M, target, dist, index, threshold, buf, moments, (cudaStream_t)cuda_stream);
-	if (e == cudaErrorInvalidValue) return fail(RGS_E_INVALID, "tnt moments: a point or a distance is NaN or infinite");
-	return dtu_cuda(e, "tnt moments");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, tnt_moments_scratch_bytes(N), buf, "tnt moments scratch")) return rc;
+	return cuda_status(launch_tnt_moments(N, source, M, target, dist, index, threshold, buf, moments, (cudaStream_t)cuda_stream), "tnt moments",
+	                   "a point or a distance is NaN or infinite");
 }
 
 // ---- tetrahedra mesh extraction (rgs_tetra.cu) ----
-
-static int tetra_cuda(cudaError_t e, const char* what) {
-	return e == cudaSuccess ? (int)RGS_OK : fail(RGS_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-}
 
 int32_t rgs_tetra_points(int64_t P, const float* xyz, const float* scaling, const float* rotation, float* points, float* scales, void* cuda_stream) {
 	if (P < 0 || 9 * P > INT32_MAX) return fail(RGS_E_INVALID, "tetra points: Gaussian count out of range");
 	if (P == 0) return RGS_OK;
 	if (!xyz || !scaling || !rotation || !points || !scales) return fail(RGS_E_INVALID, "null pointer");
-	return tetra_cuda(launch_tetra_points((int)P, xyz, scaling, rotation, points, scales, (cudaStream_t)cuda_stream), "tetra points");
+	return cuda_status(launch_tetra_points((int)P, xyz, scaling, rotation, points, scales, (cudaStream_t)cuda_stream), "tetra points");
 }
 
 int32_t rgs_tetra_cull_add(int64_t N, const float* alpha, const float* coord, int32_t H, int32_t W, const float* render7, const float* gt_mask,
@@ -863,14 +853,14 @@ int32_t rgs_tetra_cull_add(int64_t N, const float* alpha, const float* coord, in
 	if (N < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "tetra cull: negative point count or empty image");
 	if (N == 0) return RGS_OK;
 	if (!alpha || !coord || !render7 || !final_alpha || !weight) return fail(RGS_E_INVALID, "null pointer");
-	return tetra_cuda(launch_tetra_cull_add(N, alpha, coord, H, W, render7, gt_mask, final_alpha, weight, (cudaStream_t)cuda_stream), "tetra cull");
+	return cuda_status(launch_tetra_cull_add(N, alpha, coord, H, W, render7, gt_mask, final_alpha, weight, (cudaStream_t)cuda_stream), "tetra cull");
 }
 
 int32_t rgs_tetra_cull_finish(int64_t N, const float* final_alpha, const int32_t* weight, float* sdf, void* cuda_stream) {
 	if (N < 0) return fail(RGS_E_INVALID, "tetra cull: negative point count");
 	if (N == 0) return RGS_OK;
 	if (!final_alpha || !weight || !sdf) return fail(RGS_E_INVALID, "null pointer");
-	return tetra_cuda(launch_tetra_cull_finish(N, final_alpha, weight, sdf, (cudaStream_t)cuda_stream), "tetra cull finish");
+	return cuda_status(launch_tetra_cull_finish(N, final_alpha, weight, sdf, (cudaStream_t)cuda_stream), "tetra cull finish");
 }
 
 int32_t rgs_tetra_marching(int64_t N, const float* points, const float* sdf, const float* scales, int64_t T, const int64_t* tets, rgs_resize_fn resize,
@@ -880,32 +870,34 @@ int32_t rgs_tetra_marching(int64_t N, const float* points, const float* sdf, con
 	if (N < 0 || N > INT32_MAX || T < 0 || T > INT32_MAX) return fail(RGS_E_INVALID, "tetra marching: point or tet count out of range");
 	if ((N > 0 && (!points || !sdf || !scales)) || (T > 0 && !tets)) return fail(RGS_E_INVALID, "null pointer");
 	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int rc;
 	int32_t V = 0, M = 0, F = 0;
 	char* s1 = nullptr;
 	if (T > 0) {
-		s1 = resize(out->scratch_user, tetra_march_scratch1_bytes(T));
-		if (!s1) return fail(RGS_E_ALLOC, "tetra marching scratch callback returned NULL");
 		int32_t bad = 0;
-		if (const int rc = tetra_cuda(launch_tetra_march_valid(T, N, tets, sdf, s1, &bad, &V, s), "tetra marching")) return rc;
+		if ((rc = grow(resize, out->scratch_user, tetra_march_scratch1_bytes(T), s1, "tetra marching scratch")) != RGS_OK ||
+		    (rc = cuda_status(launch_tetra_march_valid(T, N, tets, sdf, s1, &bad, &V, s), "tetra marching")) != RGS_OK)
+			return rc;
 		if (bad) return fail(RGS_E_INVALID, "tetra marching: a tet index lies outside [0, N)");
 		if (V > (INT32_MAX - 255) / 6) return fail(RGS_E_INVALID, "tetra marching: too many valid tets (6 x valid must stay below 2^31)");
 	}
 	char* s2 = nullptr;
 	if (V > 0) {
-		s2 = resize(out->sort_user, tetra_march_scratch2_bytes(V));
-		if (!s2) return fail(RGS_E_ALLOC, "tetra marching scratch callback returned NULL");
-		if (const int rc = tetra_cuda(launch_tetra_march_sort(T, N, tets, sdf, V, s1, s2, &M, &F, s), "tetra marching")) return rc;
+		if ((rc = grow(resize, out->sort_user, tetra_march_scratch2_bytes(V), s2, "tetra marching scratch")) != RGS_OK ||
+		    (rc = cuda_status(launch_tetra_march_sort(T, N, tets, sdf, V, s1, s2, &M, &F, s), "tetra marching")) != RGS_OK)
+			return rc;
 	}
-	char* interp = resize(out->interp_user, (size_t)M * 2 * sizeof(int64_t));
-	char* ends = resize(out->ends_user, (size_t)M * 6 * sizeof(float));
-	char* end_sdf = resize(out->end_sdf_user, (size_t)M * 2 * sizeof(float));
-	char* end_scl = resize(out->end_scales_user, (size_t)M * 2 * sizeof(float));
-	char* faces = resize(out->faces_user, (size_t)F * 3 * sizeof(int64_t));
-	if ((M > 0 && (!interp || !ends || !end_sdf || !end_scl)) || (F > 0 && !faces)) return fail(RGS_E_ALLOC, "tetra marching callback returned NULL");
+	char *interp, *ends, *end_sdf, *end_scl, *faces;
+	if ((rc = grow(resize, out->interp_user, (size_t)M * 2 * sizeof(int64_t), interp, "tetra marching")) != RGS_OK ||
+	    (rc = grow(resize, out->ends_user, (size_t)M * 6 * sizeof(float), ends, "tetra marching")) != RGS_OK ||
+	    (rc = grow(resize, out->end_sdf_user, (size_t)M * 2 * sizeof(float), end_sdf, "tetra marching")) != RGS_OK ||
+	    (rc = grow(resize, out->end_scales_user, (size_t)M * 2 * sizeof(float), end_scl, "tetra marching")) != RGS_OK ||
+	    (rc = grow(resize, out->faces_user, (size_t)F * 3 * sizeof(int64_t), faces, "tetra marching")) != RGS_OK)
+		return rc;
 	out->num_vertices = M;
 	out->num_faces = F;
 	if (V == 0) return RGS_OK;
-	return tetra_cuda(launch_tetra_march_emit(T, points, sdf, scales, V, s1, s2, N, reinterpret_cast<int64_t*>(interp), reinterpret_cast<float*>(ends),
+	return cuda_status(launch_tetra_march_emit(T, points, sdf, scales, V, s1, s2, N, reinterpret_cast<int64_t*>(interp), reinterpret_cast<float*>(ends),
 	                                          reinterpret_cast<float*>(end_sdf), reinterpret_cast<float*>(end_scl), reinterpret_cast<int64_t*>(faces), s),
 	                  "tetra marching");
 }
@@ -914,7 +906,7 @@ int32_t rgs_tetra_bisect(int64_t M, const float* mid_sdf, float* left, float* ri
 	if (M < 0) return fail(RGS_E_INVALID, "tetra bisect: negative vertex count");
 	if (M == 0) return RGS_OK;
 	if (!left || !right || !mid || (mid_sdf && (!left_sdf || !right_sdf))) return fail(RGS_E_INVALID, "null pointer");
-	return tetra_cuda(launch_tetra_bisect(M, mid_sdf, left, right, left_sdf, right_sdf, mid, (cudaStream_t)cuda_stream), "tetra bisect");
+	return cuda_status(launch_tetra_bisect(M, mid_sdf, left, right, left_sdf, right_sdf, mid, (cudaStream_t)cuda_stream), "tetra bisect");
 }
 
 int32_t rgs_tetra_filter(int64_t M, const float* points, const float* ends, const float* end_scales, int64_t F, const int64_t* faces, rgs_resize_fn resize,
@@ -924,17 +916,18 @@ int32_t rgs_tetra_filter(int64_t M, const float* points, const float* ends, cons
 	if (M < 0 || M > INT32_MAX || F < 0 || F > INT32_MAX) return fail(RGS_E_INVALID, "tetra filter: vertex or face count out of range");
 	if ((M > 0 && (!points || !ends || !end_scales)) || (F > 0 && !faces)) return fail(RGS_E_INVALID, "null pointer");
 	if (M == 0 && F > 0) return fail(RGS_E_INVALID, "tetra filter: faces without vertices");
-	char* verts = resize(out->vertices_user, (size_t)M * 3 * sizeof(float));
-	char* fout = resize(out->faces_user, (size_t)F * 3 * sizeof(int64_t));
-	if ((M > 0 && !verts) || (F > 0 && !fout)) return fail(RGS_E_ALLOC, "tetra filter callback returned NULL");
+	char *verts, *fout, *buf;
+	int rc;
+	if ((rc = grow(resize, out->vertices_user, (size_t)M * 3 * sizeof(float), verts, "tetra filter")) != RGS_OK ||
+	    (rc = grow(resize, out->faces_user, (size_t)F * 3 * sizeof(int64_t), fout, "tetra filter")) != RGS_OK)
+		return rc;
 	if (M == 0) return RGS_OK;
-	char* buf = resize(out->scratch_user, tetra_filter_scratch_bytes((int)M, F));
-	if (!buf) return fail(RGS_E_ALLOC, "tetra filter scratch callback returned NULL");
 	int64_t nv = 0, nf = 0;
 	int32_t bad = 0;
-	if (const int rc = tetra_cuda(launch_tetra_filter((int)M, points, ends, end_scales, F, faces, buf, reinterpret_cast<float*>(verts),
-	                                                  reinterpret_cast<int64_t*>(fout), &nv, &nf, &bad, (cudaStream_t)cuda_stream),
-	                              "tetra filter"))
+	if ((rc = grow(resize, out->scratch_user, tetra_filter_scratch_bytes((int)M, F), buf, "tetra filter scratch")) != RGS_OK ||
+	    (rc = cuda_status(launch_tetra_filter((int)M, points, ends, end_scales, F, faces, buf, reinterpret_cast<float*>(verts),
+	                                          reinterpret_cast<int64_t*>(fout), &nv, &nf, &bad, (cudaStream_t)cuda_stream),
+	                      "tetra filter")) != RGS_OK)
 		return rc;
 	if (bad) return fail(RGS_E_INVALID, "tetra filter: a face index lies outside [0, M)");
 	out->num_vertices = nv;
@@ -949,7 +942,7 @@ int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t r
 	if (!img || !gt || !sums) return fail(RGS_E_INVALID, "null pointer");
 	if (planes > 65535) return fail(RGS_E_INVALID, "too many image planes");
 	launch_ssim_l1_forward(planes, H, W, row_lo, row_hi, img, gt, dmaps, sums, (cudaStream_t)cuda_stream);
-	return after_launch();
+	return cuda_status(cudaGetLastError(), "ssim l1 forward");
 }
 
 int32_t rgs_ssim_l1_backward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt,
@@ -959,7 +952,7 @@ int32_t rgs_ssim_l1_backward_rows(int32_t planes, int32_t H, int32_t W, int32_t 
 	if (!img || !gt || !dmaps || !d_img) return fail(RGS_E_INVALID, "null pointer");
 	if (planes > 65535) return fail(RGS_E_INVALID, "too many image planes");
 	launch_ssim_l1_backward(planes, H, W, row_lo, row_hi, img, gt, dmaps, w_ssim, w_l1, upstream, d_img, (cudaStream_t)cuda_stream);
-	return after_launch();
+	return cuda_status(cudaGetLastError(), "ssim l1 backward");
 }
 
 int32_t rgs_ssim_l1_forward(int32_t planes, int32_t H, int32_t W, const float* img, const float* gt, float* dmaps, double* sums, void* cuda_stream) {
@@ -978,7 +971,7 @@ int32_t rgs_normal_consistency(int32_t H, int32_t W, int32_t from_depth, float i
 	if (!rendered_normal || !map_expected || !map_median || !loss_sum || !d_normal || !d_expected || !d_median) return fail(RGS_E_INVALID, "null pointer");
 	launch_normal_consistency(H, W, from_depth != 0, inv_fx, inv_fy, cx, cy, rendered_normal, map_expected, map_median, w_expected, w_median, loss_sum,
 	                          d_normal, d_expected, d_median, (cudaStream_t)cuda_stream);
-	return after_launch();
+	return cuda_status(cudaGetLastError(), "normal consistency");
 }
 
 static int32_t appearance_size(int32_t H0, int32_t W0) {
@@ -987,25 +980,24 @@ static int32_t appearance_size(int32_t H0, int32_t W0) {
 	return RGS_OK;
 }
 
-static int32_t appearance_status(cudaError_t e) { return e == cudaSuccess ? (int32_t)RGS_OK : fail(RGS_E_CUDA, cudaGetErrorString(e)); }
-
 int32_t rgs_appearance_downsample(int32_t H0, int32_t W0, const float* image, float* down, void* cuda_stream) {
 	if (const int32_t rc = appearance_size(H0, W0)) return rc;
 	if (!image || !down) return fail(RGS_E_INVALID, "null pointer");
-	return appearance_status(launch_appearance_downsample(H0, W0, image, down, (cudaStream_t)cuda_stream));
+	return cuda_status(launch_appearance_downsample(H0, W0, image, down, (cudaStream_t)cuda_stream), "appearance downsample");
 }
 
 int32_t rgs_appearance_downsample_backward(int32_t H0, int32_t W0, const float* d_down, float* d_image, void* cuda_stream) {
 	if (const int32_t rc = appearance_size(H0, W0)) return rc;
 	if (!d_down || !d_image) return fail(RGS_E_INVALID, "null pointer");
-	return appearance_status(launch_appearance_downsample_backward(H0, W0, d_down, d_image, (cudaStream_t)cuda_stream));
+	return cuda_status(launch_appearance_downsample_backward(H0, W0, d_down, d_image, (cudaStream_t)cuda_stream), "appearance downsample backward");
 }
 
 int32_t rgs_appearance_l1_forward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* w2, const float* b2,
                                   const float* w3, const float* b3, float* act, float* transformed, double* partials, float* loss, void* cuda_stream) {
 	if (const int32_t rc = appearance_size(H0, W0)) return rc;
 	if (!image || !gt || !up4 || !w2 || !b2 || !w3 || !b3 || !partials || !loss) return fail(RGS_E_INVALID, "null pointer");
-	return appearance_status(launch_appearance_l1_forward(H0, W0, image, gt, up4, w2, b2, w3, b3, act, transformed, partials, loss, (cudaStream_t)cuda_stream));
+	return cuda_status(launch_appearance_l1_forward(H0, W0, image, gt, up4, w2, b2, w3, b3, act, transformed, partials, loss, (cudaStream_t)cuda_stream),
+	                   "appearance l1 forward");
 }
 
 int32_t rgs_appearance_l1_backward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* act, const float* w2,
@@ -1014,8 +1006,9 @@ int32_t rgs_appearance_l1_backward(int32_t H0, int32_t W0, const float* image, c
 	if (const int32_t rc = appearance_size(H0, W0)) return rc;
 	if (!image || !gt || !up4 || !act || !w2 || !w3 || !b3 || !d_image || !d_up4 || !d_w2 || !d_b2 || !d_w3 || !d_b3 || !partials || !d_x)
 		return fail(RGS_E_INVALID, "null pointer");
-	return appearance_status(launch_appearance_l1_backward(H0, W0, image, gt, up4, act, w2, w3, b3, upstream, d_image, d_up4, d_w2, d_b2, d_w3, d_b3, partials,
-	                                                       d_x, (cudaStream_t)cuda_stream));
+	return cuda_status(launch_appearance_l1_backward(H0, W0, image, gt, up4, act, w2, w3, b3, upstream, d_image, d_up4, d_w2, d_b2, d_w3, d_b3, partials,
+	                                                 d_x, (cudaStream_t)cuda_stream),
+	                   "appearance l1 backward");
 }
 
 int32_t rgs_debug_get_views(const rgs_camera* cam, int32_t P, int64_t num_rendered, const char* geom_buffer, const char* binning_buffer,

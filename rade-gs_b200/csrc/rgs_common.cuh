@@ -41,6 +41,19 @@ enum GradSlot {
 __host__ __device__ inline int rec_floats(bool coord) { return coord ? REC_FLOATS_COORD : REC_FLOATS_BASE; }
 __host__ __device__ inline int grad_floats(bool coord) { return coord ? GRAD_FLOATS_COORD : GRAD_FLOATS_BASE; }
 
+// host launchers: return the first failing CUDA call's status to the C ABI, which maps it to RGS_E_CUDA
+#define RGS_TRY(expr)                     \
+	do {                                  \
+		cudaError_t _e = (expr);          \
+		if (_e != cudaSuccess) return _e; \
+	} while (0)
+
+inline int pow2_at_least(int n) {
+	int p = 1;
+	while (p < n) p <<= 1;
+	return p;
+}
+
 // ---- buffer carving (128-byte aligned sub-arrays out of one resizable byte buffer) ----------------
 struct Carver {
 	char* base;

@@ -568,19 +568,7 @@ __global__ void __launch_bounds__(256) cull_kernel(int64_t V, const double* __re
 	keep[i] = ok;
 }
 
-int pow2_at_least(int n) {
-	int p = 1;
-	while (p < n) p <<= 1;
-	return p;
-}
-
 }  // namespace
-
-#define DTU_TRY(expr)                     \
-	do {                                  \
-		cudaError_t _e = (expr);          \
-		if (_e != cudaSuccess) return _e; \
-	} while (0)
 
 // ---- sampling ----
 
@@ -617,13 +605,13 @@ cudaError_t launch_dtu_sample_count(int64_t V, const double* verts, int64_t F, c
 	sample_count_kernel<<<(unsigned)((F + 1 + 127) / 128), 128, 0, s>>>(V, verts, F, faces, density, k.pts, k.rows);
 	count_launch();
 	size_t temp = k.temp_bytes;
-	DTU_TRY(cub::DeviceScan::ExclusiveSum(k.temp, temp, k.pts, k.pts_off, (int)(F + 1), s));
+	RGS_TRY(cub::DeviceScan::ExclusiveSum(k.temp, temp, k.pts, k.pts_off, (int)(F + 1), s));
 	temp = k.temp_bytes;
-	DTU_TRY(cub::DeviceScan::ExclusiveSum(k.temp, temp, k.rows, k.rows_off, (int)(F + 1), s));
+	RGS_TRY(cub::DeviceScan::ExclusiveSum(k.temp, temp, k.rows, k.rows_off, (int)(F + 1), s));
 	count_launch(2);
-	DTU_TRY(cudaMemcpyAsync(totals_host, k.pts_off + F, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-	DTU_TRY(cudaMemcpyAsync(totals_host + 1, k.rows_off + F, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-	DTU_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(totals_host, k.pts_off + F, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaMemcpyAsync(totals_host + 1, k.rows_off + F, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	return cudaGetLastError();
 }
 
@@ -638,7 +626,7 @@ size_t dtu_sample_rows_bytes(int64_t R) {
 cudaError_t launch_dtu_sample_emit(int64_t V, const double* verts, int64_t F, const int32_t* faces, double density, char* scratch, int64_t S, int64_t R,
                                    char* rows_scratch, double* out, cudaStream_t s) {
 	SampleScratch k = carve_sample(scratch, F, nullptr);
-	if (V > 0) DTU_TRY(cudaMemcpyAsync(out, verts, (size_t)V * 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+	if (V > 0) RGS_TRY(cudaMemcpyAsync(out, verts, (size_t)V * 3 * sizeof(double), cudaMemcpyDeviceToDevice, s));
 	if (S == 0) return cudaGetLastError();
 	Carver c(rows_scratch);
 	int64_t* row_first = c.take<int64_t>(R);
@@ -699,10 +687,10 @@ size_t dtu_downsample_scratch_bytes(int N) {
 // returns cudaErrorInvalidValue when a point is not finite (checked on the host after the bounds pass)
 cudaError_t launch_dtu_downsample(int N, const double* pts, double radius, uint8_t* kept, char* scratch, int32_t* rounds, cudaStream_t s) {
 	DsScratch k = carve_ds(scratch, N, nullptr);
-	DTU_TRY(reset_bounds(k.bits, 1, s));
+	RGS_TRY(reset_bounds(k.bits, 1, s));
 	launch_bounds(N, pts, k.bits, s);
 	Bounds b;
-	DTU_TRY(fetch_bounds(k.bits, &b, 1, s));
+	RGS_TRY(fetch_bounds(k.bits, &b, 1, s));
 	if (b.nonfinite) return cudaErrorInvalidValue;
 	// cell edge slightly above r, so the 27-cell filter stays conservative under rounding; coarser when the cloud spans more
 	// than 2^21 - 2 cells on an axis (larger cells only make the filter looser)
@@ -717,10 +705,10 @@ cudaError_t launch_dtu_downsample(int N, const double* pts, double radius, uint8
 	ds_key_kernel<<<blocks, 256, 0, s>>>(N, pts, g, k.keys_in, k.ids_in);
 	count_launch();
 	size_t temp = k.temp_bytes;
-	DTU_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.keys_in, k.keys_out, k.ids_in, k.ids_out, N, 0, 63, s));
+	RGS_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.keys_in, k.keys_out, k.ids_in, k.ids_out, N, 0, 63, s));
 	ds_pack_kernel<<<blocks, 256, 0, s>>>(N, pts, k.keys_out, k.ids_out, k.packed, k.head);
 	temp = k.temp_bytes;
-	DTU_TRY(cub::DeviceScan::InclusiveSum(k.temp, temp, k.head, k.cell_incl, N, s));
+	RGS_TRY(cub::DeviceScan::InclusiveSum(k.temp, temp, k.head, k.cell_incl, N, s));
 	ds_cells_kernel<<<blocks, 256, 0, s>>>(N, k.keys_out, k.head, k.cell_incl, k.cell_of_pt, k.cell_key, k.cell_start, k.counters + 1);
 	ds_neighbours_kernel<<<blocks, 256, 0, s>>>(k.counters + 1, k.cell_key, k.nbr);
 	ds_iota_kernel<<<blocks, 256, 0, s>>>(N, k.list_a, k.state);
@@ -729,12 +717,12 @@ cudaError_t launch_dtu_downsample(int N, const double* pts, double radius, uint8
 	int n = N, r = 0;
 	int32_t *cur = k.list_a, *nxt = k.list_b;
 	while (n > 0) {
-		DTU_TRY(cudaMemsetAsync(k.counters, 0, sizeof(int32_t), s));
+		RGS_TRY(cudaMemsetAsync(k.counters, 0, sizeof(int32_t), s));
 		ds_round_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(n, cur, k.packed, k.ids_out, k.cell_of_pt, k.cell_start, k.nbr, r2, k.state, nxt,
 		                                                            k.counters);
 		count_launch();
-		DTU_TRY(cudaMemcpyAsync(&n, k.counters, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-		DTU_TRY(cudaStreamSynchronize(s));
+		RGS_TRY(cudaMemcpyAsync(&n, k.counters, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+		RGS_TRY(cudaStreamSynchronize(s));
 		std::swap(cur, nxt);
 		r++;
 	}
@@ -788,16 +776,16 @@ size_t dtu_nearest_scratch_bytes(int M, int N) {
 
 cudaError_t launch_dtu_nearest(int M, const double* ref, int N, const double* query, double* dist, int64_t* index, char* scratch, cudaStream_t s) {
 	NnScratch k = carve_nn(scratch, M, N, nullptr);
-	DTU_TRY(reset_bounds(k.bits, 2, s));
+	RGS_TRY(reset_bounds(k.bits, 2, s));
 	launch_bounds(M, ref, k.bits, s);
 	launch_bounds(N, query, k.bits + 8, s);
 	Bounds b[2];
-	DTU_TRY(fetch_bounds(k.bits, b, 2, s));
+	RGS_TRY(fetch_bounds(k.bits, b, 2, s));
 	if (b[0].nonfinite || b[1].nonfinite) return cudaErrorInvalidValue;
 
 	nn_morton_kernel<<<(M + 255) / 256, 256, 0, s>>>(M, ref, k.bits, k.keys_in, k.ids_in);
 	size_t temp = k.temp_bytes;
-	DTU_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.keys_in, k.keys_out, k.ids_in, k.ids_out, M, 0, 63, s));
+	RGS_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.keys_in, k.keys_out, k.ids_in, k.ids_out, M, 0, 63, s));
 	const int L = (M + NN_LEAF - 1) / NN_LEAF, Lp = pow2_at_least(L);
 	nn_leaf_kernel<<<(Lp + 7) / 8, 256, 0, s>>>(M, L, Lp, ref, k.ids_out, k.packed, k.node_lo, k.node_hi);
 	count_launch(3);
@@ -808,7 +796,7 @@ cudaError_t launch_dtu_nearest(int M, const double* ref, int N, const double* qu
 	if (N == 0) return cudaGetLastError();
 	nn_morton_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, query, k.bits + 8, k.qkeys_in, k.qids_in);
 	temp = k.temp_bytes;
-	DTU_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.qkeys_in, k.qkeys_out, k.qids_in, k.qids_out, N, 0, 63, s));
+	RGS_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.qkeys_in, k.qkeys_out, k.qids_in, k.qids_out, N, 0, 63, s));
 	const int warps = (N + 31) / 32;
 	nn_query_kernel<<<(warps + NN_WARPS - 1) / NN_WARPS, NN_WARPS * 32, 0, s>>>(N, query, k.qids_out, M, Lp, k.packed, k.ids_out, k.node_lo, k.node_hi, dist,
 	                                                                            index);

@@ -276,12 +276,6 @@ __global__ void __launch_bounds__(KNN_WARPS * 32) knn_query_kernel(int P, int F,
 }
 
 int leaves_of(int F) { return (F + KNN_LEAF - 1) / KNN_LEAF; }
-int pow2_at_least(int n) {
-	int p = 1;
-	while (p < n) p <<= 1;
-	return p;
-}
-
 struct KnnScratch {
 	uint32_t* bits;
 	uint64_t *keys_in, *keys_out;
@@ -321,29 +315,23 @@ size_t knn_scratch_bytes(int P) {
 	return total;
 }
 
-#define KNN_TRY(expr)                             \
-	do {                                          \
-		cudaError_t _e = (expr);                  \
-		if (_e != cudaSuccess) return _e;         \
-	} while (0)
-
 cudaError_t launch_knn_mean_dist2(int P, const float* points, float* out, char* scratch, cudaStream_t s) {
 	KnnScratch k = carve_knn(scratch, P, nullptr);
 	// bounds: min words start at the largest ordered value, max words and the count at zero
-	KNN_TRY(cudaMemsetAsync(k.bits, 0xff, 3 * sizeof(uint32_t), s));
-	KNN_TRY(cudaMemsetAsync(k.bits + 3, 0, 5 * sizeof(uint32_t), s));
+	RGS_TRY(cudaMemsetAsync(k.bits, 0xff, 3 * sizeof(uint32_t), s));
+	RGS_TRY(cudaMemsetAsync(k.bits + 3, 0, 5 * sizeof(uint32_t), s));
 	const int bounds_blocks = std::min((P + 255) / 256, 4 * sm_count());
 	knn_bounds_kernel<<<bounds_blocks, 256, 0, s>>>(P, points, k.bits);
 	count_launch();
 	// the finite count sizes the tree: one blocking read
 	uint32_t F = 0;
-	KNN_TRY(cudaMemcpyAsync(&F, k.bits + 6, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-	KNN_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(&F, k.bits + 6, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 
 	knn_morton_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, points, k.bits, k.keys_in, k.ids_in);
 	count_launch();
 	size_t temp = k.sort_temp_bytes;
-	KNN_TRY(cub::DeviceRadixSort::SortPairs(k.sort_temp, temp, k.keys_in, k.keys_out, k.ids_in, k.ids_out, P, 0, 64, s));
+	RGS_TRY(cub::DeviceRadixSort::SortPairs(k.sort_temp, temp, k.keys_in, k.keys_out, k.ids_in, k.ids_out, P, 0, 64, s));
 	count_launch();
 	const int L = leaves_of((int)F), Lp = pow2_at_least(L > 0 ? L : 1);
 	if (F > 0) {

@@ -23,12 +23,6 @@ namespace rgs {
 
 namespace {
 
-#define TET_TRY(expr)                     \
-	do {                                  \
-		cudaError_t _e = (expr);          \
-		if (_e != cudaSuccess) return _e; \
-	} while (0)
-
 // utils/tetmesh.py: triangle_table, num_triangles_table and base_tet_edges
 __constant__ int8_t c_tri_table[16][6] = {
 	{-1, -1, -1, -1, -1, -1}, {1, 0, 2, -1, -1, -1}, {4, 0, 3, -1, -1, -1}, {1, 4, 2, 1, 3, 4},
@@ -407,14 +401,14 @@ cudaError_t launch_tetra_march_valid(int64_t T, int64_t N, const int64_t* tets, 
                                      cudaStream_t s) {
 	Carver c(scratch1);
 	TetScratch1 k = carve1(c, T);
-	TET_TRY(cudaMemsetAsync(k.counters, 0, 2 * sizeof(int32_t), s));
+	RGS_TRY(cudaMemsetAsync(k.counters, 0, 2 * sizeof(int32_t), s));
 	tetra_code_kernel<<<(unsigned)((T + 255) / 256), 256, 0, s>>>(T, N, tets, sdf, k.code, k.valid, k.counters);
 	size_t temp = k.temp_bytes;
-	TET_TRY(cub::DeviceSelect::Flagged(k.temp, temp, thrust::counting_iterator<int32_t>(0), k.valid, k.ids, k.counters + 1, (int)T, s));
+	RGS_TRY(cub::DeviceSelect::Flagged(k.temp, temp, thrust::counting_iterator<int32_t>(0), k.valid, k.ids, k.counters + 1, (int)T, s));
 	count_launch(2);
 	int32_t h[2];
-	TET_TRY(cudaMemcpyAsync(h, k.counters, sizeof(h), cudaMemcpyDeviceToHost, s));
-	TET_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(h, k.counters, sizeof(h), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	*bad = h[0];
 	*num_valid = h[1];
 	return cudaGetLastError();
@@ -428,26 +422,26 @@ cudaError_t launch_tetra_march_sort(int64_t T, int64_t N, const int64_t* tets, c
 	const int E = 6 * V, nb = bits_for(N);
 	tetra_edge_key_kernel<<<(unsigned)((E + 255) / 256), 256, 0, s>>>(V, k1.ids, tets, nb, k.keys_in, k.pos_in);
 	size_t temp = k.temp_bytes;
-	TET_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.keys_in, k.keys_out, k.pos_in, k.pos_out, E, 0, 2 * nb, s));
+	RGS_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.keys_in, k.keys_out, k.pos_in, k.pos_out, E, 0, 2 * nb, s));
 	tetra_cross_head_kernel<<<(unsigned)((E + 255) / 256), 256, 0, s>>>(E, k.keys_out, nb, sdf, k.head);
 	temp = k.temp_bytes;
-	TET_TRY(cub::DeviceScan::InclusiveSum(k.temp, temp, k.head, k.incl, E, s));
+	RGS_TRY(cub::DeviceScan::InclusiveSum(k.temp, temp, k.head, k.incl, E, s));
 	// torch.chunk(tets, T // CHUNK + 1) when T > CHUNK: chunks of ceil(T / n) tets
 	const int64_t n_chunks = T > CHUNK ? T / CHUNK + 1 : 1;
 	const int64_t chunk_len = std::max<int64_t>(1, (T + n_chunks - 1) / n_chunks);
 	const int64_t groups = 2 * ((T + chunk_len - 1) / chunk_len);
 	tetra_group_kernel<<<(unsigned)((V + 255) / 256), 256, 0, s>>>(V, k1.ids, k1.code, chunk_len, k.group_in, k.vid_in);
 	temp = k.temp_bytes;
-	TET_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.group_in, k.group_out, k.vid_in, k.vid_out, V, 0, bits_for(groups), s));
+	RGS_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.group_in, k.group_out, k.vid_in, k.vid_out, V, 0, bits_for(groups), s));
 	tetra_ntri_kernel<<<(unsigned)((V + 255) / 256), 256, 0, s>>>(V, k.vid_out, k1.ids, k1.code, k.ntri);
 	temp = k.temp_bytes;
-	TET_TRY(cub::DeviceScan::ExclusiveSum(k.temp, temp, k.ntri, k.face_off, V, s));
+	RGS_TRY(cub::DeviceScan::ExclusiveSum(k.temp, temp, k.ntri, k.face_off, V, s));
 	count_launch(7);
 	int32_t h[3];
-	TET_TRY(cudaMemcpyAsync(h, k.incl + (E - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-	TET_TRY(cudaMemcpyAsync(h + 1, k.face_off + (V - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-	TET_TRY(cudaMemcpyAsync(h + 2, k.ntri + (V - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-	TET_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(h, k.incl + (E - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaMemcpyAsync(h + 1, k.face_off + (V - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaMemcpyAsync(h + 2, k.ntri + (V - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	*num_vertices = h[0];
 	*num_faces = h[1] + h[2];
 	return cudaGetLastError();
@@ -509,24 +503,24 @@ cudaError_t launch_tetra_filter(int M, const float* points, const float* ends, c
                                 float* out_vertices, int64_t* out_faces, int64_t* num_vertices, int64_t* num_faces, int32_t* bad, cudaStream_t s) {
 	Carver c(scratch);
 	FilterScratch k = carve_filter(c, M, F);
-	TET_TRY(cudaMemsetAsync(k.count32, 0, 2 * sizeof(int32_t), s));
+	RGS_TRY(cudaMemsetAsync(k.count32, 0, 2 * sizeof(int32_t), s));
 	tetra_keep_kernel<<<(unsigned)((M + 255) / 256), 256, 0, s>>>(M, ends, end_scl, k.keep);
 	size_t temp = k.temp_bytes;
-	TET_TRY(cub::DeviceScan::ExclusiveSum(k.temp, temp, k.keep, k.excl, M, s));
+	RGS_TRY(cub::DeviceScan::ExclusiveSum(k.temp, temp, k.keep, k.excl, M, s));
 	temp = k.temp_bytes;
-	TET_TRY(cub::DeviceSelect::Flagged(k.temp, temp, reinterpret_cast<const P3f*>(points), k.keep, reinterpret_cast<P3f*>(out_vertices), k.count32, M, s));
+	RGS_TRY(cub::DeviceSelect::Flagged(k.temp, temp, reinterpret_cast<const P3f*>(points), k.keep, reinterpret_cast<P3f*>(out_vertices), k.count32, M, s));
 	int64_t h[2] = {0, 0};
 	if (F > 0) {
 		tetra_face_keep_kernel<<<(unsigned)((F + 255) / 256), 256, 0, s>>>(F, faces, k.keep, k.excl, M, k.remapped, k.fkeep, k.count32 + 1);
 		temp = k.temp_bytes;
-		TET_TRY(cub::DeviceSelect::Flagged(k.temp, temp, k.remapped, k.fkeep, reinterpret_cast<Tri*>(out_faces), k.count64, F, s));
+		RGS_TRY(cub::DeviceSelect::Flagged(k.temp, temp, k.remapped, k.fkeep, reinterpret_cast<Tri*>(out_faces), k.count64, F, s));
 		count_launch(2);
-		TET_TRY(cudaMemcpyAsync(h + 1, k.count64, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+		RGS_TRY(cudaMemcpyAsync(h + 1, k.count64, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
 	}
 	count_launch(3);
 	int32_t h32[2];
-	TET_TRY(cudaMemcpyAsync(h32, k.count32, sizeof(h32), cudaMemcpyDeviceToHost, s));
-	TET_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(h32, k.count32, sizeof(h32), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	*num_vertices = h32[0];
 	*bad = h32[1];
 	*num_faces = h[1];

@@ -327,12 +327,6 @@ __global__ void __launch_bounds__(MOM_THREADS) tnt_mom_final_kernel(int64_t P, c
 
 }  // namespace
 
-#define TNT_TRY(expr)                     \
-	do {                                  \
-		cudaError_t _e = (expr);          \
-		if (_e != cudaSuccess) return _e; \
-	} while (0)
-
 static Xform make_xform(const double* T) {
 	Xform x;
 	for (int k = 0; k < 12; k++) x.m[k] = T ? T[k] : 0.0;
@@ -372,7 +366,7 @@ size_t tnt_crop_scratch_bytes(int N) {
 cudaError_t launch_tnt_crop(int N, const double* pts, const double* xform, int axis, double axis_min, double axis_max, int K, const double* polygon,
                             uint8_t* kept, double* cropped, int64_t* num_kept, char* scratch, cudaStream_t s) {
 	CropScratch k = carve_crop(scratch, N, nullptr);
-	TNT_TRY(cudaMemsetAsync(k.bad, 0, sizeof(unsigned long long), s));
+	RGS_TRY(cudaMemsetAsync(k.bad, 0, sizeof(unsigned long long), s));
 	CropParams c;
 	c.has_xform = xform != nullptr;
 	c.has_volume = polygon != nullptr;
@@ -383,12 +377,12 @@ cudaError_t launch_tnt_crop(int N, const double* pts, const double* xform, int a
 	tnt_crop_kernel<<<(unsigned)((N + 255) / 256), 256, 2 * (size_t)c.K * sizeof(double), s>>>(N, pts, make_xform(xform), c, polygon, k.moved, kept, k.bad);
 	count_launch();
 	size_t temp = k.temp_bytes;
-	TNT_TRY(cub::DeviceSelect::Flagged(k.temp, temp, k.moved, kept, reinterpret_cast<P3*>(cropped), k.num, N, s));
+	RGS_TRY(cub::DeviceSelect::Flagged(k.temp, temp, k.moved, kept, reinterpret_cast<P3*>(cropped), k.num, N, s));
 	count_launch();
 	unsigned long long h[2];
-	TNT_TRY(cudaMemcpyAsync(&h[0], k.num, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-	TNT_TRY(cudaMemcpyAsync(&h[1], k.bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-	TNT_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(&h[0], k.num, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaMemcpyAsync(&h[1], k.bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	*num_kept = (int64_t)h[0];
 	if (h[1]) return cudaErrorInvalidValue;
 	return cudaGetLastError();
@@ -439,14 +433,14 @@ size_t tnt_voxel_scratch_bytes(int N) {
 
 cudaError_t launch_tnt_bounds(int N, const double* pts, char* scratch, double* lo, double* hi, int64_t* nonfinite, cudaStream_t s) {
 	unsigned long long* bits = reinterpret_cast<unsigned long long*>(scratch);
-	TNT_TRY(cudaMemsetAsync(bits, 0xff, 3 * sizeof(unsigned long long), s));
-	TNT_TRY(cudaMemsetAsync(bits + 3, 0, 5 * sizeof(unsigned long long), s));
+	RGS_TRY(cudaMemsetAsync(bits, 0xff, 3 * sizeof(unsigned long long), s));
+	RGS_TRY(cudaMemsetAsync(bits + 3, 0, 5 * sizeof(unsigned long long), s));
 	const int blocks = (int)std::min<int64_t>((N + 255) / 256, 4 * sm_count());
 	tnt_bounds_kernel<<<blocks, 256, 0, s>>>(N, pts, bits);
 	count_launch();
 	unsigned long long h[8];
-	TNT_TRY(cudaMemcpyAsync(h, bits, sizeof(h), cudaMemcpyDeviceToHost, s));
-	TNT_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(h, bits, sizeof(h), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	for (int a = 0; a < 3; a++) {
 		lo[a] = ord2d(h[a]);
 		hi[a] = ord2d(h[3 + a]);
@@ -463,14 +457,14 @@ cudaError_t launch_tnt_voxel_sort(int N, const double* pts, const double* origin
 	const unsigned blocks = (unsigned)((N + 255) / 256);
 	tnt_voxel_key_kernel<<<blocks, 256, 0, s>>>(N, pts, g, k.keys_in, k.ids_in);
 	size_t temp = k.temp_bytes;
-	TNT_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.keys_in, k.keys_out, k.ids_in, k.ids_out, N, 0, 3 * VOXEL_BITS, s));
+	RGS_TRY(cub::DeviceRadixSort::SortPairs(k.temp, temp, k.keys_in, k.keys_out, k.ids_in, k.ids_out, N, 0, 3 * VOXEL_BITS, s));
 	tnt_voxel_head_kernel<<<blocks, 256, 0, s>>>(N, k.keys_out, k.head);
 	temp = k.temp_bytes;
-	TNT_TRY(cub::DeviceScan::InclusiveSum(k.temp, temp, k.head, k.incl, N, s));
+	RGS_TRY(cub::DeviceScan::InclusiveSum(k.temp, temp, k.head, k.incl, N, s));
 	tnt_voxel_start_kernel<<<blocks, 256, 0, s>>>(N, k.head, k.incl, k.start);
 	count_launch(5);
-	TNT_TRY(cudaMemcpyAsync(num_voxels, k.incl + (N - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-	TNT_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(num_voxels, k.incl + (N - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	return cudaGetLastError();
 }
 
@@ -498,7 +492,7 @@ cudaError_t launch_tnt_moments(int64_t N, const double* src, int64_t M, const do
 	double* mom = c.take<double>(32);
 	double* partial = c.take<double>((size_t)P * MOM_B);
 	if (N == 0) {
-		TNT_TRY(cudaMemsetAsync(partial, 0, (size_t)MOM_B * sizeof(double), s));
+		RGS_TRY(cudaMemsetAsync(partial, 0, (size_t)MOM_B * sizeof(double), s));
 	} else {
 		tnt_mom_a_kernel<<<(unsigned)P, MOM_THREADS, 0, s>>>(N, src, M, tgt, dist, index, thr, partial);
 		count_launch();
@@ -510,8 +504,8 @@ cudaError_t launch_tnt_moments(int64_t N, const double* src, int64_t M, const do
 	}
 	tnt_mom_final_kernel<MOM_B><<<1, MOM_THREADS, 0, s>>>(P, partial, mom);
 	count_launch(2);
-	TNT_TRY(cudaMemcpyAsync(moments_host, mom, 19 * sizeof(double), cudaMemcpyDeviceToHost, s));
-	TNT_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(moments_host, mom, 19 * sizeof(double), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	if (moments_host[18] != 0.0) return cudaErrorInvalidValue;
 	return cudaGetLastError();
 }

@@ -550,12 +550,6 @@ unsigned blocks_for(int64_t n) { return (unsigned)((n + 255) / 256); }
 
 }  // namespace
 
-#define TSDF_TRY(expr)                            \
-	do {                                          \
-		cudaError_t _e = (expr);                  \
-		if (_e != cudaSuccess) return _e;         \
-	} while (0)
-
 // ---- host launchers (argument checks are in rgs_api.cu) ---------------------------------------------------------------
 
 Cam make_cam(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c) {
@@ -588,14 +582,14 @@ size_t tsdf_touch_scratch_bytes(int64_t n) {
 // phase 1: the frame-local hash and list; counters_host receives counters[0..3] (the one host read of a view)
 cudaError_t launch_tsdf_touch(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c, const float* depth, int32_t* counters_host, cudaStream_t s) {
 	const Cam k = make_cam(g, c);
-	TSDF_TRY(cudaMemsetAsync(g.frame_keys, 0xff, (size_t)g.frame_slots * sizeof(uint64_t), s));
-	TSDF_TRY(cudaMemsetAsync(g.counters + 1, 0, sizeof(int32_t), s));
-	TSDF_TRY(cudaMemsetAsync(g.counters + 3, 0, sizeof(int32_t), s));
+	RGS_TRY(cudaMemsetAsync(g.frame_keys, 0xff, (size_t)g.frame_slots * sizeof(uint64_t), s));
+	RGS_TRY(cudaMemsetAsync(g.counters + 1, 0, sizeof(int32_t), s));
+	RGS_TRY(cudaMemsetAsync(g.counters + 3, 0, sizeof(int32_t), s));
 	const int64_t P = (int64_t)c.width * c.height;
 	tsdf_touch_kernel<<<blocks_for(P), 256, 0, s>>>(k, depth, g.frame_keys, (uint64_t)g.frame_slots - 1, g.frame_list, g.frame_slots / 2, g.counters);
 	count_launch();
-	TSDF_TRY(cudaGetLastError());
-	TSDF_TRY(cudaMemcpyAsync(counters_host, g.counters, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaGetLastError());
+	RGS_TRY(cudaMemcpyAsync(counters_host, g.counters, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
 	return cudaStreamSynchronize(s);
 }
 
@@ -606,7 +600,7 @@ cudaError_t launch_tsdf_touch_sort(const rgs_tsdf_grid& g, int64_t n, int32_t* o
 	Carver cv(scratch);
 	uint64_t* sorted = cv.take<uint64_t>(n);
 	char* tmp = cv.take<char>(temp);
-	TSDF_TRY(cub::DeviceRadixSort::SortKeys(tmp, temp, g.frame_list, sorted, (int)n, 0, 63, s));
+	RGS_TRY(cub::DeviceRadixSort::SortKeys(tmp, temp, g.frame_list, sorted, (int)n, 0, 63, s));
 	count_launch();
 	tsdf_decode_kernel<<<blocks_for(n), 256, 0, s>>>((int)n, sorted, out);
 	count_launch();
@@ -638,9 +632,9 @@ size_t tsdf_active_scratch_bytes(int N) {
 cudaError_t launch_tsdf_active(const rgs_tsdf_grid& g, int N, uint64_t* keys, int32_t* pools, char* scratch, cudaStream_t s) {
 	Carver cv(scratch);
 	const ActiveScratch a = carve_active(cv, N);
-	TSDF_TRY(sort_active(g, a, N, s));
-	TSDF_TRY(cudaMemcpyAsync(keys, a.keys_out, (size_t)N * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
-	TSDF_TRY(cudaMemcpyAsync(pools, a.vals_out, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+	RGS_TRY(sort_active(g, a, N, s));
+	RGS_TRY(cudaMemcpyAsync(keys, a.keys_out, (size_t)N * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
+	RGS_TRY(cudaMemcpyAsync(pools, a.vals_out, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
 	return cudaSuccess;
 }
 
@@ -684,25 +678,25 @@ size_t tsdf_extract_scratch_bytes(const rgs_tsdf_grid& g, int N) {
 cudaError_t launch_tsdf_extract_count(const rgs_tsdf_grid& g, int N, float thr, char* scratch, int64_t* totals_host, cudaStream_t s) {
 	const int64_t M = (int64_t)N * BV;
 	ExtractScratch x = carve_extract(scratch, g, N, nullptr);
-	TSDF_TRY(sort_active(g, x.a, N, s));
+	RGS_TRY(sort_active(g, x.a, N, s));
 	tsdf_inverse_kernel<<<blocks_for(N), 256, 0, s>>>(N, x.a.vals_out, x.inv);
 	tsdf_neighbours_kernel<<<blocks_for((int64_t)N * 27), 256, 0, s>>>(g, N, x.a.keys_out, x.inv, x.nbr);
 	tsdf_state_kernel<<<blocks_for(M), 256, 0, s>>>(g, M, x.a.vals_out, thr, x.st);
 	tsdf_cell_kernel<<<blocks_for(M), 256, 0, s>>>(M, x.nbr, x.st, x.cell);
 	tsdf_count_kernel<<<blocks_for(M), 256, 0, s>>>(M, x.nbr, x.st, x.cell, x.vmask, x.vcnt, x.tcnt);
 	count_launch(5);
-	TSDF_TRY(cudaGetLastError());
+	RGS_TRY(cudaGetLastError());
 	size_t temp = x.scan_temp_bytes;
-	TSDF_TRY(cub::DeviceScan::ExclusiveSum(x.scan_temp, temp, x.vcnt, x.voff, M, s));
+	RGS_TRY(cub::DeviceScan::ExclusiveSum(x.scan_temp, temp, x.vcnt, x.voff, M, s));
 	temp = x.scan_temp_bytes;
-	TSDF_TRY(cub::DeviceScan::ExclusiveSum(x.scan_temp, temp, x.tcnt, x.toff, M, s));
+	RGS_TRY(cub::DeviceScan::ExclusiveSum(x.scan_temp, temp, x.tcnt, x.toff, M, s));
 	count_launch(2);
 	int32_t tail[4];
-	TSDF_TRY(cudaMemcpyAsync(tail, x.voff + M - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-	TSDF_TRY(cudaMemcpyAsync(tail + 1, x.vcnt + M - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-	TSDF_TRY(cudaMemcpyAsync(tail + 2, x.toff + M - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-	TSDF_TRY(cudaMemcpyAsync(tail + 3, x.tcnt + M - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-	TSDF_TRY(cudaStreamSynchronize(s));
+	RGS_TRY(cudaMemcpyAsync(tail, x.voff + M - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaMemcpyAsync(tail + 1, x.vcnt + M - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaMemcpyAsync(tail + 2, x.toff + M - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaMemcpyAsync(tail + 3, x.tcnt + M - 1, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+	RGS_TRY(cudaStreamSynchronize(s));
 	totals_host[0] = (int64_t)tail[0] + tail[1];
 	totals_host[1] = (int64_t)tail[2] + tail[3];
 	return cudaSuccess;
@@ -751,8 +745,8 @@ size_t tsdf_normals_scratch_bytes(int64_t V, int64_t F) {
 cudaError_t launch_tsdf_normals(int64_t V, const float* verts, int64_t F, const int32_t* tris, float* normals, char* scratch, cudaStream_t s) {
 	const int64_t F3 = 3 * F;
 	NormalsScratch x = carve_normals(scratch, V, F3, nullptr);
-	TSDF_TRY(cudaMemsetAsync(x.first, 0, (size_t)V * sizeof(int32_t), s));
-	TSDF_TRY(cudaMemsetAsync(x.last, 0, (size_t)V * sizeof(int32_t), s));
+	RGS_TRY(cudaMemsetAsync(x.first, 0, (size_t)V * sizeof(int32_t), s));
+	RGS_TRY(cudaMemsetAsync(x.last, 0, (size_t)V * sizeof(int32_t), s));
 	if (F3 > 0) {
 		tsdf_pairs_kernel<<<blocks_for(F3), 256, 0, s>>>(F3, tris, x.vk_in, x.tv_in);
 		count_launch();
@@ -760,7 +754,7 @@ cudaError_t launch_tsdf_normals(int64_t V, const float* verts, int64_t F, const 
 		while (bits < 32 && ((int64_t)1 << bits) < V) bits++;
 		size_t temp = x.sort_temp_bytes;
 		// radix sort is stable: each vertex's entries stay in ascending triangle order
-		TSDF_TRY(cub::DeviceRadixSort::SortPairs(x.sort_temp, temp, x.vk_in, x.vk_out, x.tv_in, x.tv_out, (int)F3, 0, bits, s));
+		RGS_TRY(cub::DeviceRadixSort::SortPairs(x.sort_temp, temp, x.vk_in, x.vk_out, x.tv_in, x.tv_out, (int)F3, 0, bits, s));
 		count_launch();
 		tsdf_ranges_kernel<<<blocks_for(F3), 256, 0, s>>>(F3, x.vk_out, x.first, x.last);
 		count_launch();

@@ -27,11 +27,49 @@ namespace {
 
 const float* opt_ptr(const torch::Tensor& t) { return t.numel() == 0 ? nullptr : t.data_ptr<float>(); }
 
+const char* dtype_name(torch::ScalarType t) {
+	switch (t) {
+		case torch::kFloat32: return "float32";
+		case torch::kFloat64: return "float64";
+		case torch::kInt32: return "int32";
+		case torch::kInt64: return "int64";
+		case torch::kUInt8: return "uint8";
+		default: return c10::toString(t);
+	}
+}
+
+// COPY hands the kernels a contiguous copy when needed; REJECT refuses a non-contiguous tensor instead, for tensors the
+// kernels write in place and for the arrays the TSDF grid owns.
+enum Contiguity { COPY, REJECT };
+
+// The check of one tensor argument: `dtype`, sizes matching `dims` (-1 matches any size; no dims: any shape; `shape` is the
+// pattern as messages print it, e.g. "[H, W, 3]"), on a CUDA device, `like`'s device when given.
+torch::Tensor arg(const torch::Tensor& t, const char* name, torch::ScalarType dtype, std::initializer_list<int64_t> dims = {}, const char* shape = "",
+                  const torch::Tensor* like = nullptr, Contiguity mode = COPY) {
+	TORCH_CHECK(t.scalar_type() == dtype, name, " must be ", dtype_name(dtype), ", got ", t.scalar_type());
+	bool fits = dims.size() == 0 || t.dim() == (int64_t)dims.size();
+	for (int64_t i = 0; fits && i < (int64_t)dims.size(); i++) fits = dims.begin()[i] < 0 || t.size(i) == dims.begin()[i];
+	TORCH_CHECK(fits, name, " must be ", shape, ", got ", t.sizes());
+	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
+	TORCH_CHECK(!like || t.device() == like->device(), name, " must be on the same device as the other inputs");
+	if (mode == COPY) return t.contiguous();
+	TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
+	return t;
+}
+
+// the rasterizer's optional float32 inputs: an empty tensor (torch.Tensor([]) on the CPU) is absent and stays so
 torch::Tensor as_input(const torch::Tensor& t, const torch::Tensor& like, const char* name) {
-	if (t.numel() == 0) return t;  // absent (torch.Tensor([]) on the CPU), stays absent
-	TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32");
-	TORCH_CHECK(t.device() == like.device(), name, " must be on the same device as means3D");
-	return t.contiguous();
+	return t.numel() == 0 ? t : arg(t, name, torch::kFloat32, {}, "", &like);
+}
+
+// an empty byte tensor on `like`'s device, for the C ABI's resize callback to grow
+torch::Tensor bytes(const torch::Tensor& like) { return torch::empty({0}, like.options().dtype(torch::kByte)); }
+
+// the first n rows of `dtype` values shaped `k` in a byte buffer the C ABI resized
+torch::Tensor rows(const torch::Tensor& buffer, torch::ScalarType dtype, int64_t n, std::initializer_list<int64_t> k) {
+	std::vector<int64_t> shape{n};
+	shape.insert(shape.end(), k);
+	return buffer.narrow(0, 0, c10::multiply_integers(shape) * (int64_t)c10::elementSize(dtype)).view(dtype).view(shape);
 }
 
 // Debug aid (`_C.set_poison(byte)`, tests only): every scratch buffer and every empty()-allocated output is filled with
@@ -63,8 +101,8 @@ void check(int64_t rc) {
 
 // The rasterizer has no CPU fallback: refuse host tensors, then run on the device of means3D.
 c10::cuda::CUDAGuard cuda_guard(const torch::Tensor& means3D, const torch::Tensor* points3D = nullptr) {
-	TORCH_CHECK(means3D.is_cuda() && (!points3D || points3D->is_cuda()),
-	            points3D ? "means3D / points3D must be CUDA tensors" : "means3D must be a CUDA tensor", ": this rasterizer has no CPU path");
+	TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor: no CPU path");
+	TORCH_CHECK(!points3D || points3D->is_cuda(), "points3D must be a CUDA tensor: no CPU path");
 	return c10::cuda::CUDAGuard(means3D.device());
 }
 
@@ -160,7 +198,6 @@ FwdResult forward_impl(const torch::Tensor& background, const torch::Tensor& mea
 	const int H = image_height, W = image_width;
 	auto int_opts = means3D.options().dtype(torch::kInt32);
 	auto float_opts = means3D.options().dtype(torch::kFloat32);
-	auto byte_opts = means3D.options().dtype(torch::kByte);
 	const int grid_y = (H + 15) / 16;
 	const bool whole = (row_begin == 0 && (row_end < 0 || row_end == grid_y));
 	// compact: the maps hold the slab's pixel rows only ([ch, Hs, W]) and are fully written by the kernels
@@ -171,7 +208,7 @@ FwdResult forward_impl(const torch::Tensor& background, const torch::Tensor& mea
 	torch::Tensor out_color = img(3), out_depth = img(1), out_mdepth = img(1), out_coord = img(3), out_mcoord = img(3), out_alpha = img(1),
 	              out_normal = img(3);
 	torch::Tensor radii = P == 0 ? torch::zeros({P}, int_opts) : new_empty({P}, int_opts);
-	torch::Tensor geomBuffer = torch::empty({0}, byte_opts), binningBuffer = torch::empty({0}, byte_opts), imgBuffer = torch::empty({0}, byte_opts);
+	torch::Tensor geomBuffer = bytes(means3D), binningBuffer = bytes(means3D), imgBuffer = bytes(means3D);
 
 	int rendered = 0;
 	if (P != 0) {
@@ -311,7 +348,7 @@ GradTensors backward_impl(const torch::Tensor& background, const torch::Tensor& 
 		              tan_fovy, kernel_size, dL_dout_color, dL_dout_coord, dL_dout_mcoord, dL_dout_depth, dL_dout_mdepth, dL_dout_alpha,
 		              dL_dout_normal, normalmap, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, alphas, require_coord, require_depth,
 		              debug, 0, -1, sh_rest);
-		torch::Tensor scratch = torch::empty({0}, means3D.options().dtype(torch::kByte));
+		torch::Tensor scratch = bytes(means3D);
 		check(rgs_backward(&c.ch.cam, &c.gh.g, &c.in, &gt.out, resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
 	}
 	return gt;
@@ -367,7 +404,6 @@ IntegrateGaussiansToPointsCUDA(const torch::Tensor& background, const torch::Ten
 	const int PN = points3D.size(0), P = means3D.size(0), H = image_height, W = image_width;
 	auto int_opts = means3D.options().dtype(torch::kInt32);
 	auto float_opts = means3D.options().dtype(torch::kFloat32);
-	auto byte_opts = means3D.options().dtype(torch::kByte);
 	const bool run = P != 0 && PN != 0;  // rasterize_points.cu:341: otherwise the fill values below are returned
 	torch::Tensor out_color = run ? new_empty({9, H, W}, float_opts) : torch::zeros({9, H, W}, float_opts);
 	torch::Tensor radii = run ? new_empty({P}, int_opts) : torch::zeros({P}, int_opts);
@@ -375,8 +411,7 @@ IntegrateGaussiansToPointsCUDA(const torch::Tensor& background, const torch::Ten
 	torch::Tensor out_color_integrated = run ? new_empty({PN, 3}, float_opts) : torch::zeros({PN, 3}, float_opts);
 	torch::Tensor out_coordinate2d = run ? new_empty({PN, 2}, float_opts) : torch::zeros({PN, 2}, float_opts);
 	torch::Tensor out_sdf = run ? new_empty({PN}, float_opts) : torch::full({PN}, -1000.0, float_opts);
-	torch::Tensor geomBuffer = torch::empty({0}, byte_opts), binningBuffer = torch::empty({0}, byte_opts), imgBuffer = torch::empty({0}, byte_opts),
-	              pointBuffer = torch::empty({0}, byte_opts);
+	torch::Tensor geomBuffer = bytes(means3D), binningBuffer = bytes(means3D), imgBuffer = bytes(means3D), pointBuffer = bytes(means3D);
 	int rendered = 0;
 	if (run) {
 		CamHolder ch;
@@ -491,10 +526,8 @@ torch::Tensor ExchangeResult(const int64_t ex, const int P, const int row_floats
 }
 
 void ExchangeRows(const int64_t ex, const torch::Tensor& tiles_touched, const torch::Tensor& radii) {
-	TORCH_CHECK(tiles_touched.is_cuda() && radii.is_cuda() && tiles_touched.scalar_type() == torch::kInt32 && radii.scalar_type() == torch::kInt32,
-	            "tiles_touched / radii must be CUDA int32 tensors");
-	const c10::cuda::CUDAGuard guard(radii.device());
-	torch::Tensor t = tiles_touched.contiguous(), r = radii.contiguous();
+	const torch::Tensor t = arg(tiles_touched, "tiles_touched", torch::kInt32), r = arg(radii, "radii", torch::kInt32);
+	const c10::cuda::CUDAGuard guard(r.device());
 	if (rgs_exchange_rows(reinterpret_cast<rgs_exchange*>(ex), (int)r.numel(), reinterpret_cast<const uint32_t*>(t.data_ptr<int>()), r.data_ptr<int>(),
 	                      at::cuda::getCurrentCUDAStream().stream()) != RGS_OK)
 		throw std::runtime_error(rgs_exchange_last_error());
@@ -540,11 +573,10 @@ BwdResult BackwardPreprocessCUDA(const torch::Tensor& grad_accum, const torch::T
 
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> ActivateForward(const torch::Tensor& raw_scaling, const torch::Tensor& raw_opacity,
                                                                         const torch::Tensor& raw_rotation, const torch::Tensor& filter_3D) {
-	TORCH_CHECK(raw_scaling.is_cuda(), "raw_scaling must be a CUDA tensor: no CPU path");
-	const c10::cuda::CUDAGuard guard(raw_scaling.device());
-	const int P = raw_scaling.size(0);
-	torch::Tensor s = as_input(raw_scaling, raw_scaling, "raw_scaling"), o = as_input(raw_opacity, raw_scaling, "raw_opacity"),
-	              r = as_input(raw_rotation, raw_scaling, "raw_rotation"), f = as_input(filter_3D, raw_scaling, "filter_3D");
+	const torch::Tensor s = arg(raw_scaling, "raw_scaling", torch::kFloat32), o = as_input(raw_opacity, s, "raw_opacity"),
+	                    r = as_input(raw_rotation, s, "raw_rotation"), f = as_input(filter_3D, s, "filter_3D");
+	const c10::cuda::CUDAGuard guard(s.device());
+	const int P = s.size(0);
 	TORCH_CHECK(s.numel() == 3 * (int64_t)P && o.numel() == P && r.numel() == 4 * (int64_t)P && f.numel() == P, "activate: shapes must be [P,3] [P,1] [P,4] [P,1]");
 	torch::Tensor scales = new_empty({P, 3}, s.options()), opacity = new_empty({P, 1}, s.options()), rot = new_empty({P, 4}, s.options());
 	if (P)
@@ -557,12 +589,11 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> ActivateBackward(const t
                                                                          const torch::Tensor& raw_rotation, const torch::Tensor& filter_3D,
                                                                          const torch::Tensor& g_scales, const torch::Tensor& g_opacity,
                                                                          const torch::Tensor& g_rotations) {
-	const c10::cuda::CUDAGuard guard(raw_scaling.device());
-	const int P = raw_scaling.size(0);
-	torch::Tensor s = as_input(raw_scaling, raw_scaling, "raw_scaling"), o = as_input(raw_opacity, raw_scaling, "raw_opacity"),
-	              r = as_input(raw_rotation, raw_scaling, "raw_rotation"), f = as_input(filter_3D, raw_scaling, "filter_3D"),
-	              gs = as_input(g_scales, raw_scaling, "g_scales"), go = as_input(g_opacity, raw_scaling, "g_opacity"),
-	              gr = as_input(g_rotations, raw_scaling, "g_rotations");
+	const torch::Tensor s = arg(raw_scaling, "raw_scaling", torch::kFloat32), o = as_input(raw_opacity, s, "raw_opacity"),
+	                    r = as_input(raw_rotation, s, "raw_rotation"), f = as_input(filter_3D, s, "filter_3D"), gs = as_input(g_scales, s, "g_scales"),
+	                    go = as_input(g_opacity, s, "g_opacity"), gr = as_input(g_rotations, s, "g_rotations");
+	const c10::cuda::CUDAGuard guard(s.device());
+	const int P = s.size(0);
 	TORCH_CHECK(gs.numel() == 3 * (int64_t)P && go.numel() == P && gr.numel() == 4 * (int64_t)P, "activate backward: gradient shapes must be [P,3] [P,1] [P,4]");
 	torch::Tensor ds = new_empty({P, 3}, s.options()), dop = new_empty({P, 1}, s.options()), dr = new_empty({P, 4}, s.options());
 	if (P)
@@ -574,16 +605,21 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> ActivateBackward(const t
 
 void DensificationStats(const torch::Tensor& means2D_grad, const torch::Tensor& radii, torch::Tensor& grad_accum, torch::Tensor& grad_accum_abs,
                         torch::Tensor& grad_accum_abs_max, torch::Tensor& denom, torch::Tensor& max_radii2D) {
-	const c10::cuda::CUDAGuard guard(means2D_grad.device());
-	const int P = means2D_grad.size(0);
+	const torch::Tensor g = arg(means2D_grad, "means2D.grad", torch::kFloat32);
+	const c10::cuda::CUDAGuard guard(g.device());
+	const int P = g.size(0);
 	if (P == 0) return;
-	torch::Tensor g = as_input(means2D_grad, means2D_grad, "means2D.grad");
 	torch::Tensor rad = radii.contiguous();
-	for (const torch::Tensor* t : {&grad_accum, &grad_accum_abs, &grad_accum_abs_max, &denom})
-		TORCH_CHECK(t->is_contiguous() && t->scalar_type() == torch::kFloat32 && t->numel() == P, "densification statistics must be contiguous float32 [P,1] tensors");
+	const std::pair<const char*, const torch::Tensor*> stats[] = {
+	    {"grad_accum", &grad_accum}, {"grad_accum_abs", &grad_accum_abs}, {"grad_accum_abs_max", &grad_accum_abs_max}, {"denom", &denom}};
+	for (const auto& [name, t] : stats) {
+		arg(*t, name, torch::kFloat32, {}, "", &g, REJECT);
+		TORCH_CHECK(t->numel() == P, "densification statistics must be [P,1] tensors");
+	}
 	float* mr = nullptr;
 	if (max_radii2D.numel() != 0) {
-		TORCH_CHECK(max_radii2D.is_contiguous() && max_radii2D.scalar_type() == torch::kFloat32 && max_radii2D.numel() == P, "max_radii2D must be contiguous float32 [P]");
+		arg(max_radii2D, "max_radii2D", torch::kFloat32, {}, "", &g, REJECT);
+		TORCH_CHECK(max_radii2D.numel() == P, "max_radii2D must be [P]");
 		mr = max_radii2D.data_ptr<float>();
 	}
 	check(rgs_densification_stats(P, g.data_ptr<float>(), rad.data_ptr<int>(), grad_accum.data_ptr<float>(), grad_accum_abs.data_ptr<float>(),
@@ -592,10 +628,9 @@ void DensificationStats(const torch::Tensor& means2D_grad, const torch::Tensor& 
 
 // returns (filter_3D [P,1], max_distance [1])
 std::tuple<torch::Tensor, torch::Tensor> Compute3DFilter(const torch::Tensor& xyz, const torch::Tensor& cams, const double focal_length) {
-	TORCH_CHECK(xyz.is_cuda(), "xyz must be a CUDA tensor: no CPU path");
-	const c10::cuda::CUDAGuard guard(xyz.device());
-	torch::Tensor x = as_input(xyz, xyz, "xyz"), c = as_input(cams, xyz, "camera table");
-	const int P = xyz.size(0);
+	const torch::Tensor x = arg(xyz, "xyz", torch::kFloat32), c = as_input(cams, x, "camera table");
+	const c10::cuda::CUDAGuard guard(x.device());
+	const int P = x.size(0);
 	TORCH_CHECK(c.numel() % 16 == 0, "camera table must be [n_cams,16]");
 	const int n = (int)(c.numel() / 16);
 	torch::Tensor out = new_empty({P, 1}, x.options()), mx = torch::zeros({1}, x.options());
@@ -607,19 +642,12 @@ std::tuple<torch::Tensor, torch::Tensor> Compute3DFilter(const torch::Tensor& xy
 
 // ---- fused image-side losses (opt-in, SURVEY.md 8f row 2) -----------------------------------------------------------------
 
-torch::Tensor image_input(const torch::Tensor& t, const torch::Tensor& like, const char* name) {
-	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
-	TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32");
-	TORCH_CHECK(t.device() == like.device(), name, " must be on the same device as the image");
-	return t.contiguous();
-}
-
 // returns (sums [2] float64: sum of the SSIM map, sum |img - gt|; dmaps [3, planes, H, W] or empty)
 std::tuple<torch::Tensor, torch::Tensor> SsimL1Forward(const torch::Tensor& img, const torch::Tensor& gt, const bool need_grad, const int row_lo_in,
                                                         const int row_hi_in) {
 	TORCH_CHECK(img.dim() >= 2 && img.numel() == gt.numel() && img.size(-1) == gt.size(-1) && img.size(-2) == gt.size(-2),
 	            "ssim: images must have the same number of elements and the same [H, W]");
-	torch::Tensor a = image_input(img, img, "img1"), b = image_input(gt, img, "img2");
+	const torch::Tensor a = arg(img, "img1", torch::kFloat32), b = arg(gt, "img2", torch::kFloat32, {}, "", &a);
 	const c10::cuda::CUDAGuard guard(a.device());
 	const int H = a.size(-2), W = a.size(-1);
 	const int planes = (int)(a.numel() / ((int64_t)H * W));
@@ -633,7 +661,8 @@ std::tuple<torch::Tensor, torch::Tensor> SsimL1Forward(const torch::Tensor& img,
 
 torch::Tensor SsimL1Backward(const torch::Tensor& img, const torch::Tensor& gt, const torch::Tensor& dmaps, const double w_ssim, const double w_l1,
                              const torch::Tensor& upstream, const int row_lo_in, const int row_hi_in) {
-	torch::Tensor a = image_input(img, img, "img1"), b = image_input(gt, img, "img2"), d = image_input(dmaps, img, "dmaps");
+	const torch::Tensor a = arg(img, "img1", torch::kFloat32), b = arg(gt, "img2", torch::kFloat32, {}, "", &a),
+	                    d = arg(dmaps, "dmaps", torch::kFloat32, {}, "", &a);
 	const c10::cuda::CUDAGuard guard(a.device());
 	const int H = a.size(-2), W = a.size(-1);
 	const int planes = (int)(a.numel() / ((int64_t)H * W));
@@ -642,7 +671,7 @@ torch::Tensor SsimL1Backward(const torch::Tensor& img, const torch::Tensor& gt, 
 	const float* up_ptr = nullptr;
 	if (upstream.defined() && upstream.numel() != 0) {
 		TORCH_CHECK(upstream.numel() == 1, "ssim backward: upstream gradient must be a scalar");
-		up = image_input(upstream, img, "upstream gradient");
+		up = arg(upstream, "upstream gradient", torch::kFloat32, {}, "", &a);
 		up_ptr = up.data_ptr<float>();
 	}
 	const int row_lo = row_lo_in, row_hi = row_hi_in < 0 ? H : row_hi_in;
@@ -660,10 +689,9 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> NormalCon
                                                                                            const double inv_fx, const double inv_fy, const double cx,
                                                                                            const double cy, const double w_expected,
                                                                                            const double w_median) {
-	torch::Tensor n = image_input(rendered_normal, rendered_normal, "rendered_normal"), e = image_input(map_expected, rendered_normal, "expected map"),
-	              m = image_input(map_median, rendered_normal, "median map");
+	const torch::Tensor n = arg(rendered_normal, "rendered_normal", torch::kFloat32, {3, -1, -1}, "[3,H,W]"),
+	                    e = arg(map_expected, "expected map", torch::kFloat32, {}, "", &n), m = arg(map_median, "median map", torch::kFloat32, {}, "", &n);
 	const c10::cuda::CUDAGuard guard(n.device());
-	TORCH_CHECK(n.dim() == 3 && n.size(0) == 3, "rendered_normal must be [3,H,W]");
 	const int H = n.size(1), W = n.size(2);
 	const int64_t want = (from_depth ? 1 : 3) * (int64_t)H * W;
 	TORCH_CHECK(e.numel() == want && m.numel() == want, from_depth ? "depth maps must be [1,H,W]" : "coordinate maps must be [3,H,W]");
@@ -677,18 +705,11 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> NormalCon
 
 // ---- decoupled-appearance L1 loss (train.py:37-58; rgs_appearance_*) -------------------------------------------------------
 
-void appearance_image(const torch::Tensor& t, const char* name) {
-	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
-	TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32");
-	TORCH_CHECK(t.dim() == 3 && t.size(0) == 3, name, " must be [3, H, W]");
-	TORCH_CHECK(t.size(1) >= 32 && t.size(2) >= 32, "appearance loss: the image must be at least 32 x 32, got ", t.sizes());
-}
-
 // image [3,H0,W0] -> the center crop's bilinear downsample [3, H/32, W/32]
 torch::Tensor AppearanceDownsample(const torch::Tensor& image) {
-	appearance_image(image, "image");
-	const c10::cuda::CUDAGuard guard(image.device());
-	const torch::Tensor a = image.contiguous();
+	const torch::Tensor a = arg(image, "image", torch::kFloat32, {3, -1, -1}, "[3, H, W]");
+	TORCH_CHECK(a.size(1) >= 32 && a.size(2) >= 32, "appearance loss: the image must be at least 32 x 32, got ", a.sizes());
+	const c10::cuda::CUDAGuard guard(a.device());
 	const int H0 = a.size(1), W0 = a.size(2);
 	torch::Tensor down = new_empty({3, H0 / 32, W0 / 32}, a.options());
 	check(rgs_appearance_downsample(H0, W0, a.data_ptr<float>(), down.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
@@ -697,10 +718,10 @@ torch::Tensor AppearanceDownsample(const torch::Tensor& image) {
 
 // d_image += the downsample's transpose applied to d_down (in place)
 void AppearanceDownsampleBackward(const torch::Tensor& d_down, torch::Tensor& d_image) {
-	appearance_image(d_image, "d_image");
-	TORCH_CHECK(d_image.is_contiguous(), "d_image must be contiguous");
+	arg(d_image, "d_image", torch::kFloat32, {3, -1, -1}, "[3, H, W]", nullptr, REJECT);
 	const int H0 = d_image.size(1), W0 = d_image.size(2);
-	torch::Tensor g = image_input(d_down, d_image, "d_down");
+	TORCH_CHECK(H0 >= 32 && W0 >= 32, "appearance loss: the image must be at least 32 x 32, got ", d_image.sizes());
+	const torch::Tensor g = arg(d_down, "d_down", torch::kFloat32, {}, "", &d_image);
 	TORCH_CHECK(g.numel() == 3 * (int64_t)(H0 / 32) * (W0 / 32), "d_down does not belong to this image");
 	const c10::cuda::CUDAGuard guard(d_image.device());
 	check(rgs_appearance_downsample_backward(H0, W0, g.data_ptr<float>(), d_image.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
@@ -713,20 +734,20 @@ struct AppearanceArgs {
 
 AppearanceArgs appearance_args(const torch::Tensor& image, const torch::Tensor& gt, const torch::Tensor& up4, const torch::Tensor& w2, const torch::Tensor& b2,
                                const torch::Tensor& w3, const torch::Tensor& b3) {
-	appearance_image(image, "image");
 	AppearanceArgs a;
-	a.image = image.contiguous();
+	a.image = arg(image, "image", torch::kFloat32, {3, -1, -1}, "[3, H, W]");
 	a.H0 = image.size(1);
 	a.W0 = image.size(2);
+	TORCH_CHECK(a.H0 >= 32 && a.W0 >= 32, "appearance loss: the image must be at least 32 x 32, got ", image.sizes());
 	TORCH_CHECK(gt.sizes() == image.sizes(), "gt must have the image's shape");
-	a.gt = image_input(gt, image, "gt");
+	a.gt = arg(gt, "gt", torch::kFloat32, {}, "", &image);
 	const int64_t H = a.H0 / 32 * 32, W = a.W0 / 32 * 32;
-	a.up4 = image_input(up4, image, "up4 output");
+	a.up4 = arg(up4, "up4 output", torch::kFloat32, {}, "", &image);
 	TORCH_CHECK(a.up4.numel() == 16 * (H / 2) * (W / 2), "up4 output must be [1, 16, ", H / 2, ", ", W / 2, "], got ", up4.sizes());
-	a.w2 = image_input(w2, image, "conv2 weight");
-	a.b2 = image_input(b2, image, "conv2 bias");
-	a.w3 = image_input(w3, image, "conv3 weight");
-	a.b3 = image_input(b3, image, "conv3 bias");
+	a.w2 = arg(w2, "conv2 weight", torch::kFloat32, {}, "", &image);
+	a.b2 = arg(b2, "conv2 bias", torch::kFloat32, {}, "", &image);
+	a.w3 = arg(w3, "conv3 weight", torch::kFloat32, {}, "", &image);
+	a.b3 = arg(b3, "conv3 bias", torch::kFloat32, {}, "", &image);
 	TORCH_CHECK(a.w2.sizes() == torch::IntArrayRef({16, 16, 3, 3}) && a.b2.numel() == 16, "conv2 must be 16 -> 16 with 3x3 kernels");
 	TORCH_CHECK(a.w3.sizes() == torch::IntArrayRef({3, 16, 3, 3}) && a.b3.numel() == 3, "conv3 must be 16 -> 3 with 3x3 kernels");
 	return a;
@@ -758,13 +779,13 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
 	const AppearanceArgs a = appearance_args(image, gt, up4, w2, b2, w3, b3);
 	const c10::cuda::CUDAGuard guard(a.image.device());
 	const int64_t H = a.H0 / 32 * 32, W = a.W0 / 32 * 32;
-	const torch::Tensor ac = image_input(act, image, "activations");
+	const torch::Tensor ac = arg(act, "activations", torch::kFloat32, {}, "", &image);
 	TORCH_CHECK(ac.numel() == 16 * H * W, "activations do not belong to this image");
 	const float* up_ptr = nullptr;
 	torch::Tensor up;
 	if (upstream.defined() && upstream.numel() != 0) {
 		TORCH_CHECK(upstream.numel() == 1, "appearance loss backward: upstream gradient must be a scalar");
-		up = image_input(upstream, image, "upstream gradient");
+		up = arg(upstream, "upstream gradient", torch::kFloat32, {}, "", &image);
 		up_ptr = up.data_ptr<float>();
 	}
 	const auto o = a.image.options();
@@ -782,15 +803,11 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
 // simple_knn's distCUDA2 (reference scene/gaussian_model.py:315-316): points [P,3] float32 on a CUDA device -> [P] float32,
 // the mean squared distance to the 3 nearest other points (rgs_knn_mean_dist2).  Non-contiguous input is accepted.
 torch::Tensor KnnMeanDist2(const torch::Tensor& points) {
-	TORCH_CHECK(points.dim() == 2 && points.size(1) == 3, "distCUDA2: points must have dimensions (num_points, 3), got ", points.sizes());
-	TORCH_CHECK(points.scalar_type() == torch::kFloat32, "distCUDA2: points must be float32, got ", points.scalar_type());
-	TORCH_CHECK(points.is_cuda(), "distCUDA2: points must be a CUDA tensor: no CPU path");
-	TORCH_CHECK(points.size(0) <= INT32_MAX, "distCUDA2: at most 2^31 - 1 points");
-	const c10::cuda::CUDAGuard guard(points.device());
-	const int P = (int)points.size(0);
-	torch::Tensor x = points.contiguous();
-	torch::Tensor out = new_empty({P}, x.options());
-	torch::Tensor scratch = torch::empty({0}, x.options().dtype(torch::kByte));
+	const torch::Tensor x = arg(points, "distCUDA2: points", torch::kFloat32, {-1, 3}, "(num_points, 3)");
+	TORCH_CHECK(x.size(0) <= INT32_MAX, "distCUDA2: at most 2^31 - 1 points");
+	const c10::cuda::CUDAGuard guard(x.device());
+	const int P = (int)x.size(0);
+	torch::Tensor out = new_empty({P}, x.options()), scratch = bytes(x);
 	if (P) check(rgs_knn_mean_dist2(P, x.data_ptr<float>(), out.data_ptr<float>(), resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
 	return out;
 }
@@ -798,9 +815,7 @@ torch::Tensor KnnMeanDist2(const torch::Tensor& points) {
 // ---- TSDF voxel-block grid (rgs_tsdf_*; Python side rade_gs_b200.tsdf.VoxelBlockGrid, which owns every array) ----------------
 
 torch::Tensor grid_array(const py::object& grid, const char* name, torch::ScalarType type) {
-	torch::Tensor t = grid.attr(name).cast<torch::Tensor>();
-	TORCH_CHECK(t.is_cuda() && t.scalar_type() == type && t.is_contiguous(), "VoxelBlockGrid.", name, " must be a contiguous CUDA ", type, " tensor");
-	return t;
+	return arg(grid.attr(name).cast<torch::Tensor>(), name, type, {}, "", nullptr, REJECT);
 }
 
 // the C view of the grid; the Python object keeps the tensors alive
@@ -821,17 +836,6 @@ rgs_tsdf_grid tsdf_grid(const py::object& grid) {
 	g.frame_list = reinterpret_cast<uint64_t*>(grid_array(grid, "frame_list", torch::kInt64).data_ptr<int64_t>());
 	g.counters = grid_array(grid, "counters", torch::kInt32).data_ptr<int32_t>();
 	return g;
-}
-
-// a per-view image on the grid's device: float32, contiguous, [H, W] (depth) or [H, W, 3] (colour)
-torch::Tensor tsdf_image(const torch::Tensor& t, const torch::Tensor& like, const char* name, int channels) {
-	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
-	TORCH_CHECK(t.device() == like.device(), name, " must be on the grid's device");
-	TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32, got ", t.scalar_type());
-	TORCH_CHECK(channels == 1 ? t.dim() == 2 : (t.dim() == 3 && t.size(2) == channels), name, channels == 1 ? " must be [H, W]" : " must be [H, W, 3]",
-	            ", got ", t.sizes());
-	TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
-	return t;
 }
 
 // intrinsic [3,3] and extrinsic [4,4] as CPU float64 tensors -> the fp32 camera of the contract (one conversion, here)
@@ -859,17 +863,15 @@ rgs_tsdf_camera tsdf_camera(const torch::Tensor& depth, const torch::Tensor& int
 	return c;
 }
 
-torch::Tensor tsdf_scratch(const torch::Tensor& like) { return torch::empty({0}, like.options().dtype(torch::kByte)); }
-
 // returns (number of touched blocks, or -1 when the frame-local hash is full; block coordinates int32 [n, 3]; allocated blocks)
 std::tuple<int64_t, torch::Tensor, int64_t> TsdfTouch(const py::object& grid, const torch::Tensor& depth, const torch::Tensor& intrinsic,
                                                       const torch::Tensor& extrinsic, double depth_scale, double depth_max, double trunc_voxel_multiplier) {
 	const torch::Tensor keys = grid_array(grid, "hash_keys", torch::kInt64);
 	const c10::cuda::CUDAGuard guard(keys.device());
-	const torch::Tensor d = tsdf_image(depth, keys, "depth", 1);
+	const torch::Tensor d = arg(depth, "depth", torch::kFloat32, {-1, -1}, "[H, W]", &keys, REJECT);
 	const rgs_tsdf_grid g = tsdf_grid(grid);
 	const rgs_tsdf_camera c = tsdf_camera(d, intrinsic, extrinsic, depth_scale, depth_max, trunc_voxel_multiplier);
-	torch::Tensor out = torch::empty({g.frame_slots / 2, 3}, keys.options().dtype(torch::kInt32)), scratch = tsdf_scratch(keys);
+	torch::Tensor out = torch::empty({g.frame_slots / 2, 3}, keys.options().dtype(torch::kInt32)), scratch = bytes(keys);
 	int64_t allocated = 0;
 	const int64_t n = rgs_tsdf_touch(&g, &c, d.data_ptr<float>(), out.data_ptr<int32_t>(), &allocated, resize_cb, &scratch,
 	                                 at::cuda::getCurrentCUDAStream().stream());
@@ -883,15 +885,13 @@ void TsdfIntegrate(const py::object& grid, const torch::Tensor& block_coords, co
                    int call_id) {
 	const torch::Tensor keys = grid_array(grid, "hash_keys", torch::kInt64);
 	const c10::cuda::CUDAGuard guard(keys.device());
-	TORCH_CHECK(block_coords.is_cuda() && block_coords.device() == keys.device(), "block_coords must be a CUDA tensor on the grid's device");
-	TORCH_CHECK(block_coords.scalar_type() == torch::kInt32 && block_coords.dim() == 2 && block_coords.size(1) == 3,
-	            "block_coords must be int32 [N, 3], got ", block_coords.scalar_type(), " ", block_coords.sizes());
-	TORCH_CHECK(block_coords.is_contiguous(), "block_coords must be contiguous");
-	const torch::Tensor d = tsdf_image(depth, keys, "depth", 1), col = tsdf_image(color, keys, "color", 3);
+	arg(block_coords, "block_coords", torch::kInt32, {-1, 3}, "[N, 3]", &keys, REJECT);
+	const torch::Tensor d = arg(depth, "depth", torch::kFloat32, {-1, -1}, "[H, W]", &keys, REJECT),
+	                    col = arg(color, "color", torch::kFloat32, {-1, -1, 3}, "[H, W, 3]", &keys, REJECT);
 	TORCH_CHECK(col.size(0) == d.size(0) && col.size(1) == d.size(1), "color and depth must have the same [H, W]");
 	const rgs_tsdf_grid g = tsdf_grid(grid);
 	const rgs_tsdf_camera c = tsdf_camera(d, intrinsic, extrinsic, depth_scale, depth_max, trunc_voxel_multiplier);
-	torch::Tensor scratch = tsdf_scratch(keys);
+	torch::Tensor scratch = bytes(keys);
 	check(rgs_tsdf_integrate(&g, &c, block_coords.size(0), block_coords.data_ptr<int32_t>(), d.data_ptr<float>(), col.data_ptr<float>(), call_id, resize_cb,
 	                         &scratch, at::cuda::getCurrentCUDAStream().stream()));
 }
@@ -899,9 +899,9 @@ void TsdfIntegrate(const py::object& grid, const torch::Tensor& block_coords, co
 void TsdfRehash(const py::object& grid, const torch::Tensor& old_keys, const torch::Tensor& old_values) {
 	const torch::Tensor keys = grid_array(grid, "hash_keys", torch::kInt64);
 	const c10::cuda::CUDAGuard guard(keys.device());
-	TORCH_CHECK(old_keys.is_cuda() && old_values.is_cuda() && old_keys.scalar_type() == torch::kInt64 && old_values.scalar_type() == torch::kInt32 &&
-	                old_keys.is_contiguous() && old_values.is_contiguous() && old_keys.numel() == old_values.numel(),
-	            "old hash must be contiguous CUDA int64 keys and int32 values of one length");
+	arg(old_keys, "old hash keys", torch::kInt64, {}, "", &keys, REJECT);
+	arg(old_values, "old hash values", torch::kInt32, {}, "", &keys, REJECT);
+	TORCH_CHECK(old_keys.numel() == old_values.numel(), "old hash keys and values must have one length");
 	const rgs_tsdf_grid g = tsdf_grid(grid);
 	check(rgs_tsdf_rehash(&g, reinterpret_cast<const uint64_t*>(old_keys.data_ptr<int64_t>()), old_values.data_ptr<int32_t>(), old_keys.numel(),
 	                      at::cuda::getCurrentCUDAStream().stream()));
@@ -912,8 +912,7 @@ std::tuple<torch::Tensor, torch::Tensor> TsdfActiveBlocks(const py::object& grid
 	const torch::Tensor hk = grid_array(grid, "hash_keys", torch::kInt64);
 	const c10::cuda::CUDAGuard guard(hk.device());
 	const rgs_tsdf_grid g = tsdf_grid(grid);
-	torch::Tensor keys = torch::empty({g.capacity}, hk.options()), pools = torch::empty({g.capacity}, hk.options().dtype(torch::kInt32)),
-	              scratch = tsdf_scratch(hk);
+	torch::Tensor keys = torch::empty({g.capacity}, hk.options()), pools = torch::empty({g.capacity}, hk.options().dtype(torch::kInt32)), scratch = bytes(hk);
 	const int64_t n = rgs_tsdf_active_blocks(&g, reinterpret_cast<uint64_t*>(keys.data_ptr<int64_t>()), pools.data_ptr<int32_t>(), resize_cb, &scratch,
 	                                         at::cuda::getCurrentCUDAStream().stream());
 	check(n);
@@ -925,26 +924,23 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> TsdfExtract(const py::ob
 	const torch::Tensor hk = grid_array(grid, "hash_keys", torch::kInt64);
 	const c10::cuda::CUDAGuard guard(hk.device());
 	const rgs_tsdf_grid g = tsdf_grid(grid);
-	torch::Tensor v = tsdf_scratch(hk), c = tsdf_scratch(hk), t = tsdf_scratch(hk), scratch = tsdf_scratch(hk);
+	torch::Tensor v = bytes(hk), c = bytes(hk), t = bytes(hk), scratch = bytes(hk);
 	rgs_tsdf_mesh_out out{&v, &c, &t, 0, 0};
 	check(rgs_tsdf_extract(&g, (float)weight_threshold, resize_cb, &out, &scratch, at::cuda::getCurrentCUDAStream().stream()));
-	return std::make_tuple(v.view(torch::kFloat32).view({out.num_vertices, 3}), c.view(torch::kFloat32).view({out.num_vertices, 3}),
-	                       t.view(torch::kInt32).view({out.num_triangles, 3}));
+	return std::make_tuple(rows(v, torch::kFloat32, out.num_vertices, {3}), rows(c, torch::kFloat32, out.num_vertices, {3}),
+	                       rows(t, torch::kInt32, out.num_triangles, {3}));
 }
 
 torch::Tensor TsdfVertexNormals(const torch::Tensor& vertices, const torch::Tensor& triangles) {
-	TORCH_CHECK(vertices.is_cuda() && triangles.is_cuda() && vertices.device() == triangles.device(), "vertices / triangles must be CUDA tensors on one device");
-	TORCH_CHECK(vertices.scalar_type() == torch::kFloat32 && vertices.dim() == 2 && vertices.size(1) == 3 && vertices.is_contiguous(),
-	            "vertices must be contiguous float32 [V, 3]");
-	TORCH_CHECK(triangles.scalar_type() == torch::kInt32 && triangles.dim() == 2 && triangles.size(1) == 3 && triangles.is_contiguous(),
-	            "triangles must be contiguous int32 [F, 3]");
+	arg(vertices, "vertices", torch::kFloat32, {-1, 3}, "[V, 3]", nullptr, REJECT);
+	arg(triangles, "triangles", torch::kInt32, {-1, 3}, "[F, 3]", &vertices, REJECT);
 	const c10::cuda::CUDAGuard guard(vertices.device());
 	const int64_t V = vertices.size(0), F = triangles.size(0);
 	if (F > 0) {
 		const auto mm = torch::aminmax(triangles);
 		TORCH_CHECK(std::get<0>(mm).item<int32_t>() >= 0 && std::get<1>(mm).item<int32_t>() < V, "triangle vertex index out of [0, V)");
 	}
-	torch::Tensor normals = new_empty({V, 3}, vertices.options()), scratch = tsdf_scratch(vertices);
+	torch::Tensor normals = new_empty({V, 3}, vertices.options()), scratch = bytes(vertices);
 	check(rgs_tsdf_vertex_normals(V, vertices.data_ptr<float>(), F, triangles.data_ptr<int32_t>(), normals.data_ptr<float>(), resize_cb, &scratch,
 	                              at::cuda::getCurrentCUDAStream().stream()));
 	return normals;
@@ -952,35 +948,23 @@ torch::Tensor TsdfVertexNormals(const torch::Tensor& vertices, const torch::Tens
 
 // ---- DTU evaluation (rgs_dtu_*; Python side rade_gs_b200.dtu_eval) -------------------------------------------------------
 
-torch::Tensor dtu_points(const torch::Tensor& t, const char* name) {
-	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
-	TORCH_CHECK(t.scalar_type() == torch::kFloat64 && t.dim() == 2 && t.size(1) == 3, name, " must be float64 [N, 3], got ", t.scalar_type(), " ",
-	            t.sizes());
-	return t.contiguous();
-}
-
-torch::Tensor dtu_bytes(const torch::Tensor& like) { return torch::empty({0}, like.options().dtype(torch::kByte)); }
-
 // vertices f64 [V,3], faces int32 [F,3] -> the vertices followed by the surface samples, f64 [V + S, 3]
 torch::Tensor DtuSampleMesh(const torch::Tensor& vertices, const torch::Tensor& faces, double density) {
-	const torch::Tensor v = dtu_points(vertices, "vertices");
-	TORCH_CHECK(faces.is_cuda() && faces.device() == v.device(), "faces must be a CUDA tensor on the vertices' device");
-	TORCH_CHECK(faces.scalar_type() == torch::kInt32 && faces.dim() == 2 && faces.size(1) == 3, "faces must be int32 [F, 3], got ", faces.scalar_type(), " ",
-	            faces.sizes());
+	const torch::Tensor v = arg(vertices, "vertices", torch::kFloat64, {-1, 3}, "[N, 3]");
+	const torch::Tensor f = arg(faces, "faces", torch::kInt32, {-1, 3}, "[F, 3]", &v);
 	const c10::cuda::CUDAGuard guard(v.device());
-	const torch::Tensor f = faces.contiguous();
-	torch::Tensor pts = dtu_bytes(v), scratch = dtu_bytes(v), rows = dtu_bytes(v);
-	rgs_dtu_samples_out out{&pts, &scratch, &rows, 0};
+	torch::Tensor pts = bytes(v), scratch = bytes(v), row_scratch = bytes(v);
+	rgs_dtu_samples_out out{&pts, &scratch, &row_scratch, 0};
 	check(rgs_dtu_sample_mesh(v.size(0), v.data_ptr<double>(), f.size(0), f.data_ptr<int32_t>(), density, resize_cb, &out,
 	                          at::cuda::getCurrentCUDAStream().stream()));
-	return pts.view(torch::kFloat64).view({out.num_points, 3});
+	return rows(pts, torch::kFloat64, out.num_points, {3});
 }
 
 // points f64 [N,3] in processing order -> (kept bool [N], rounds)
 std::tuple<torch::Tensor, int32_t> DtuRadiusDownsample(const torch::Tensor& points, double radius) {
-	const torch::Tensor p = dtu_points(points, "points");
+	const torch::Tensor p = arg(points, "points", torch::kFloat64, {-1, 3}, "[N, 3]");
 	const c10::cuda::CUDAGuard guard(p.device());
-	torch::Tensor kept = new_empty({p.size(0)}, p.options().dtype(torch::kBool)), scratch = dtu_bytes(p);
+	torch::Tensor kept = new_empty({p.size(0)}, p.options().dtype(torch::kBool)), scratch = bytes(p);
 	int32_t rounds = 0;
 	check(rgs_dtu_radius_downsample(p.size(0), p.data_ptr<double>(), radius, reinterpret_cast<uint8_t*>(kept.data_ptr<bool>()), &rounds, resize_cb, &scratch,
 	                                at::cuda::getCurrentCUDAStream().stream()));
@@ -989,10 +973,9 @@ std::tuple<torch::Tensor, int32_t> DtuRadiusDownsample(const torch::Tensor& poin
 
 // reference f64 [M,3], query f64 [N,3] -> (distance f64 [N], index int64 [N])
 std::tuple<torch::Tensor, torch::Tensor> DtuNearest(const torch::Tensor& reference, const torch::Tensor& query) {
-	const torch::Tensor r = dtu_points(reference, "reference"), q = dtu_points(query, "query");
-	TORCH_CHECK(r.device() == q.device(), "reference and query must be on one device");
+	const torch::Tensor r = arg(reference, "reference", torch::kFloat64, {-1, 3}, "[N, 3]"), q = arg(query, "query", torch::kFloat64, {-1, 3}, "[N, 3]", &r);
 	const c10::cuda::CUDAGuard guard(r.device());
-	torch::Tensor dist = new_empty({q.size(0)}, q.options()), index = new_empty({q.size(0)}, q.options().dtype(torch::kInt64)), scratch = dtu_bytes(r);
+	torch::Tensor dist = new_empty({q.size(0)}, q.options()), index = new_empty({q.size(0)}, q.options().dtype(torch::kInt64)), scratch = bytes(r);
 	check(rgs_dtu_nearest(r.size(0), r.data_ptr<double>(), q.size(0), q.data_ptr<double>(), dist.data_ptr<double>(), index.data_ptr<int64_t>(), resize_cb,
 	                      &scratch, at::cuda::getCurrentCUDAStream().stream()));
 	return std::make_tuple(dist, index);
@@ -1000,9 +983,8 @@ std::tuple<torch::Tensor, torch::Tensor> DtuNearest(const torch::Tensor& referen
 
 // masks uint8 [n, H, W] (nonzero = set) -> disk(6) dilation, uint8 [n, H, W]
 torch::Tensor DtuDilateMasks(const torch::Tensor& masks) {
-	TORCH_CHECK(masks.is_cuda() && masks.scalar_type() == torch::kUInt8 && masks.dim() == 3, "masks must be a CUDA uint8 [n, H, W] tensor");
-	const c10::cuda::CUDAGuard guard(masks.device());
-	const torch::Tensor m = masks.contiguous();
+	const torch::Tensor m = arg(masks, "masks", torch::kUInt8, {-1, -1, -1}, "[n, H, W]");
+	const c10::cuda::CUDAGuard guard(m.device());
 	torch::Tensor out = new_empty(m.sizes(), m.options());
 	check(rgs_dtu_dilate_masks((int32_t)m.size(0), (int32_t)m.size(1), (int32_t)m.size(2), m.data_ptr<uint8_t>(), out.data_ptr<uint8_t>(),
 	                           at::cuda::getCurrentCUDAStream().stream()));
@@ -1011,15 +993,10 @@ torch::Tensor DtuDilateMasks(const torch::Tensor& masks) {
 
 // vertices f64 [V,3], proj f64 [n,3,4], dilated uint8 [n,H,W] -> keep bool [V]
 torch::Tensor DtuCullVertices(const torch::Tensor& vertices, const torch::Tensor& proj, const torch::Tensor& dilated) {
-	const torch::Tensor v = dtu_points(vertices, "vertices");
-	TORCH_CHECK(proj.is_cuda() && proj.device() == v.device() && proj.scalar_type() == torch::kFloat64 && proj.dim() == 3 && proj.size(1) == 3 &&
-	                proj.size(2) == 4,
-	            "proj must be a CUDA float64 [n, 3, 4] tensor on the vertices' device");
-	TORCH_CHECK(dilated.is_cuda() && dilated.device() == v.device() && dilated.scalar_type() == torch::kUInt8 && dilated.dim() == 3 &&
-	                dilated.size(0) == proj.size(0),
-	            "dilated must be a CUDA uint8 [n, H, W] tensor with one mask per view");
+	const torch::Tensor v = arg(vertices, "vertices", torch::kFloat64, {-1, 3}, "[N, 3]");
+	const torch::Tensor P = arg(proj, "proj", torch::kFloat64, {-1, 3, 4}, "[n, 3, 4]", &v),
+	                    m = arg(dilated, "dilated", torch::kUInt8, {P.size(0), -1, -1}, "[n, H, W] with one mask per view", &v);
 	const c10::cuda::CUDAGuard guard(v.device());
-	const torch::Tensor P = proj.contiguous(), m = dilated.contiguous();
 	torch::Tensor keep = new_empty({v.size(0)}, v.options().dtype(torch::kBool));
 	check(rgs_dtu_cull_vertices(v.size(0), v.data_ptr<double>(), (int32_t)P.size(0), (int32_t)m.size(1), (int32_t)m.size(2), P.data_ptr<double>(),
 	                            m.data_ptr<uint8_t>(), reinterpret_cast<uint8_t*>(keep.data_ptr<bool>()), at::cuda::getCurrentCUDAStream().stream()));
@@ -1038,19 +1015,16 @@ torch::Tensor tnt_host_transform(const torch::Tensor& T) {
 // points f64 [N,3], transform f64 [4,4] or empty, polygon f64 [K,2] (CUDA) or empty -> (kept bool [N], cropped f64 [n,3])
 std::tuple<torch::Tensor, torch::Tensor> TntCrop(const torch::Tensor& points, const torch::Tensor& transform, int64_t axis, double axis_min, double axis_max,
                                                  const torch::Tensor& polygon) {
-	const torch::Tensor p = dtu_points(points, "points");
+	const torch::Tensor p = arg(points, "points", torch::kFloat64, {-1, 3}, "[N, 3]");
 	const c10::cuda::CUDAGuard guard(p.device());
 	const torch::Tensor T = tnt_host_transform(transform);
 	torch::Tensor poly;
 	rgs_tnt_crop_volume vol{};
 	if (polygon.numel() > 0) {
-		TORCH_CHECK(polygon.is_cuda() && polygon.device() == p.device() && polygon.scalar_type() == torch::kFloat64 && polygon.dim() == 2 &&
-		                polygon.size(1) == 2,
-		            "polygon must be a CUDA float64 [K, 2] tensor on the points' device");
-		poly = polygon.contiguous();
+		poly = arg(polygon, "polygon", torch::kFloat64, {-1, 2}, "[K, 2]", &p);
 		vol = rgs_tnt_crop_volume{(int32_t)axis, (int32_t)poly.size(0), axis_min, axis_max, poly.data_ptr<double>()};
 	}
-	torch::Tensor kept = new_empty({p.size(0)}, p.options().dtype(torch::kBool)), cropped = new_empty({p.size(0), 3}, p.options()), scratch = dtu_bytes(p);
+	torch::Tensor kept = new_empty({p.size(0)}, p.options().dtype(torch::kBool)), cropped = new_empty({p.size(0), 3}, p.options()), scratch = bytes(p);
 	int64_t n = 0;
 	check(rgs_tnt_crop(p.size(0), p.data_ptr<double>(), T.numel() ? T.data_ptr<double>() : nullptr, polygon.numel() ? &vol : nullptr,
 	                   reinterpret_cast<uint8_t*>(kept.data_ptr<bool>()), cropped.data_ptr<double>(), &n, resize_cb, &scratch,
@@ -1060,8 +1034,7 @@ std::tuple<torch::Tensor, torch::Tensor> TntCrop(const torch::Tensor& points, co
 
 // points f64 [N,3] (contiguous CUDA), overwritten with T p
 void TntTransform(torch::Tensor points, const torch::Tensor& transform) {
-	TORCH_CHECK(points.is_cuda() && points.scalar_type() == torch::kFloat64 && points.dim() == 2 && points.size(1) == 3 && points.is_contiguous(),
-	            "points must be a contiguous CUDA float64 [N, 3] tensor");
+	arg(points, "points", torch::kFloat64, {-1, 3}, "[N, 3]", nullptr, REJECT);
 	TORCH_CHECK(transform.numel() == 16, "transform must be [4, 4]");
 	const c10::cuda::CUDAGuard guard(points.device());
 	const torch::Tensor T = tnt_host_transform(transform);
@@ -1070,24 +1043,20 @@ void TntTransform(torch::Tensor points, const torch::Tensor& transform) {
 
 // points f64 [N,3] -> (means f64 [V,3] in ascending voxel key order, counts int64 [V])
 std::tuple<torch::Tensor, torch::Tensor> TntVoxelDownsample(const torch::Tensor& points, double voxel) {
-	const torch::Tensor p = dtu_points(points, "points");
+	const torch::Tensor p = arg(points, "points", torch::kFloat64, {-1, 3}, "[N, 3]");
 	const c10::cuda::CUDAGuard guard(p.device());
-	torch::Tensor means = dtu_bytes(p), counts = dtu_bytes(p), scratch = dtu_bytes(p);
+	torch::Tensor means = bytes(p), counts = bytes(p), scratch = bytes(p);
 	rgs_tnt_voxel_out out{&means, &counts, &scratch, 0};
 	check(rgs_tnt_voxel_downsample(p.size(0), p.data_ptr<double>(), voxel, resize_cb, &out, at::cuda::getCurrentCUDAStream().stream()));
-	return std::make_tuple(means.narrow(0, 0, out.num_voxels * 3 * 8).view(torch::kFloat64).view({out.num_voxels, 3}),
-	                       counts.narrow(0, 0, out.num_voxels * 8).view(torch::kInt64));
+	return std::make_tuple(rows(means, torch::kFloat64, out.num_voxels, {3}), rows(counts, torch::kInt64, out.num_voxels, {}));
 }
 
 // source f64 [N,3], target f64 [M,3], dist f64 [N], index int64 [N] -> the 18 moments (CPU float64)
 torch::Tensor TntIcpMoments(const torch::Tensor& source, const torch::Tensor& target, const torch::Tensor& dist, const torch::Tensor& index, double threshold) {
-	const torch::Tensor s = dtu_points(source, "source"), t = dtu_points(target, "target");
-	TORCH_CHECK(s.device() == t.device() && dist.device() == s.device() && index.device() == s.device(), "all inputs must be on one CUDA device");
-	TORCH_CHECK(dist.scalar_type() == torch::kFloat64 && dist.dim() == 1 && dist.size(0) == s.size(0), "dist must be float64 [N]");
-	TORCH_CHECK(index.scalar_type() == torch::kInt64 && index.dim() == 1 && index.size(0) == s.size(0), "index must be int64 [N]");
+	const torch::Tensor s = arg(source, "source", torch::kFloat64, {-1, 3}, "[N, 3]"), t = arg(target, "target", torch::kFloat64, {-1, 3}, "[M, 3]", &s),
+	                    d = arg(dist, "dist", torch::kFloat64, {s.size(0)}, "[N]", &s), ix = arg(index, "index", torch::kInt64, {s.size(0)}, "[N]", &s);
 	const c10::cuda::CUDAGuard guard(s.device());
-	const torch::Tensor d = dist.contiguous(), ix = index.contiguous();
-	torch::Tensor scratch = dtu_bytes(s), mom = torch::empty({19}, torch::TensorOptions().dtype(torch::kFloat64));
+	torch::Tensor scratch = bytes(s), mom = torch::empty({19}, torch::TensorOptions().dtype(torch::kFloat64));
 	check(rgs_tnt_icp_moments(s.size(0), s.data_ptr<double>(), t.size(0), t.data_ptr<double>(), d.data_ptr<double>(), ix.data_ptr<int64_t>(), threshold,
 	                          mom.data_ptr<double>(), resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
 	return mom.narrow(0, 0, 18);
@@ -1095,23 +1064,10 @@ torch::Tensor TntIcpMoments(const torch::Tensor& source, const torch::Tensor& ta
 
 // ---- tetrahedra mesh extraction (rgs_tetra_*; Python side rade_gs_b200.tetra) ----------------------------------------------
 
-// a CUDA float32 tensor with `inner` elements per row (inner 0: one-dimensional), on `like`'s device when given
-torch::Tensor tetra_f32(const torch::Tensor& t, int64_t inner, const char* name, const torch::Tensor* like = nullptr) {
-	TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor: no CPU path");
-	TORCH_CHECK(!like || t.device() == like->device(), name, " must be on the same device as the other inputs");
-	TORCH_CHECK(t.scalar_type() == torch::kFloat32, name, " must be float32, got ", t.scalar_type());
-	if (inner == 0) {
-		TORCH_CHECK(t.dim() == 1, name, " must be one-dimensional, got ", t.sizes());
-	} else {
-		TORCH_CHECK(t.dim() >= 1 && t.numel() == t.size(0) * inner, name, " must hold ", inner, " values per row, got ", t.sizes());
-	}
-	return t.contiguous();
-}
-
 // xyz, scaling f32 [P,3], rotation f32 [P,4] -> (points f32 [9P,3], scales f32 [9P,1])
 std::tuple<torch::Tensor, torch::Tensor> TetraPoints(const torch::Tensor& xyz, const torch::Tensor& scaling, const torch::Tensor& rotation) {
-	const torch::Tensor x = tetra_f32(xyz, 3, "xyz"), s = tetra_f32(scaling, 3, "scaling", &x), r = tetra_f32(rotation, 4, "rotation", &x);
-	TORCH_CHECK(s.size(0) == x.size(0) && r.size(0) == x.size(0), "xyz, scaling and rotation must have one row per Gaussian");
+	const torch::Tensor x = arg(xyz, "xyz", torch::kFloat32, {-1, 3}, "[P, 3]"), s = arg(scaling, "scaling", torch::kFloat32, {x.size(0), 3}, "[P, 3]", &x),
+	                    r = arg(rotation, "rotation", torch::kFloat32, {x.size(0), 4}, "[P, 4]", &x);
 	const c10::cuda::CUDAGuard guard(x.device());
 	const int64_t P = x.size(0);
 	torch::Tensor pts = new_empty({9 * P, 3}, x.options()), scl = new_empty({9 * P, 1}, x.options());
@@ -1123,21 +1079,14 @@ std::tuple<torch::Tensor, torch::Tensor> TetraPoints(const torch::Tensor& xyz, c
 // accumulates one view into final_alpha f32 [N] and weight int32 [N] (contiguous, in place)
 void TetraCullAdd(const torch::Tensor& alpha, const torch::Tensor& coord, const torch::Tensor& render7, const torch::Tensor& gt_mask, torch::Tensor final_alpha,
                   torch::Tensor weight) {
-	TORCH_CHECK(final_alpha.is_cuda() && final_alpha.scalar_type() == torch::kFloat32 && final_alpha.dim() == 1 && final_alpha.is_contiguous(),
-	            "final_alpha must be a contiguous CUDA float32 [N] tensor");
+	arg(final_alpha, "final_alpha", torch::kFloat32, {-1}, "[N]", nullptr, REJECT);
 	const int64_t N = final_alpha.size(0);
-	TORCH_CHECK(weight.device() == final_alpha.device() && weight.scalar_type() == torch::kInt32 && weight.dim() == 1 && weight.size(0) == N &&
-	                weight.is_contiguous(),
-	            "weight must be a contiguous int32 [N] tensor on final_alpha's device");
-	const torch::Tensor a = tetra_f32(alpha.reshape({-1}), 0, "alpha_integrated", &final_alpha), c = tetra_f32(coord, 2, "point_coordinate", &final_alpha);
-	TORCH_CHECK(a.size(0) == N && c.size(0) == N, "alpha_integrated and point_coordinate must have one row per point (", N, ")");
-	TORCH_CHECK(render7.dim() == 2, "render7 must be [H, W], got ", render7.sizes());
-	const torch::Tensor r7 = tetra_f32(render7, render7.size(1), "render7", &final_alpha);
+	arg(weight, "weight", torch::kInt32, {N}, "[N]", &final_alpha, REJECT);
+	const torch::Tensor a = arg(alpha.reshape({-1}), "alpha_integrated", torch::kFloat32, {N}, "[N]", &final_alpha),
+	                    c = arg(coord, "point_coordinate", torch::kFloat32, {N, 2}, "[N, 2]", &final_alpha),
+	                    r7 = arg(render7, "render7", torch::kFloat32, {-1, -1}, "[H, W]", &final_alpha);
 	torch::Tensor gt;
-	if (gt_mask.numel() > 0) {
-		gt = tetra_f32(gt_mask.reshape({-1}), 0, "gt_mask", &final_alpha);
-		TORCH_CHECK(gt.size(0) == r7.numel(), "gt_mask must have the image's H x W values, got ", gt_mask.sizes());
-	}
+	if (gt_mask.numel() > 0) gt = arg(gt_mask.reshape({-1}), "gt_mask", torch::kFloat32, {r7.numel()}, "the image's H x W values", &final_alpha);
 	const c10::cuda::CUDAGuard guard(final_alpha.device());
 	check(rgs_tetra_cull_add(N, a.data_ptr<float>(), c.data_ptr<float>(), (int32_t)r7.size(0), (int32_t)r7.size(1), r7.data_ptr<float>(),
 	                         gt.defined() ? gt.data_ptr<float>() : nullptr, final_alpha.data_ptr<float>(), weight.data_ptr<int32_t>(),
@@ -1145,11 +1094,8 @@ void TetraCullAdd(const torch::Tensor& alpha, const torch::Tensor& coord, const 
 }
 
 torch::Tensor TetraCullFinish(const torch::Tensor& final_alpha, const torch::Tensor& weight) {
-	const torch::Tensor f = tetra_f32(final_alpha, 0, "final_alpha");
-	TORCH_CHECK(weight.device() == f.device() && weight.scalar_type() == torch::kInt32 && weight.dim() == 1 && weight.size(0) == f.size(0),
-	            "weight must be int32 [N] on final_alpha's device");
+	const torch::Tensor f = arg(final_alpha, "final_alpha", torch::kFloat32, {-1}, "[N]"), w = arg(weight, "weight", torch::kInt32, {f.size(0)}, "[N]", &f);
 	const c10::cuda::CUDAGuard guard(f.device());
-	const torch::Tensor w = weight.contiguous();
 	torch::Tensor sdf = new_empty({f.size(0)}, f.options());
 	check(rgs_tetra_cull_finish(f.size(0), f.data_ptr<float>(), w.data_ptr<int32_t>(), sdf.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
 	return sdf;
@@ -1159,39 +1105,30 @@ torch::Tensor TetraCullFinish(const torch::Tensor& final_alpha, const torch::Ten
 //   -> (ends f32 [M,2,3], end_sdf f32 [M,2,1], end_scales f32 [M,2,1], faces int64 [F,3], interp_v int64 [M,2])
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> TetraMarching(const torch::Tensor& points, const torch::Tensor& sdf,
                                                                                                    const torch::Tensor& scales, const torch::Tensor& tets) {
-	const torch::Tensor p = tetra_f32(points, 3, "vertices"), d = tetra_f32(sdf.reshape({-1}), 0, "sdf", &p), s = tetra_f32(scales.reshape({-1}), 0, "scales", &p);
-	TORCH_CHECK(d.size(0) == p.size(0) && s.size(0) == p.size(0), "sdf and scales must have one value per vertex");
-	TORCH_CHECK(tets.is_cuda() && tets.device() == p.device() && tets.scalar_type() == torch::kInt64 && tets.dim() == 2 && tets.size(1) == 4,
-	            "tets must be a CUDA int64 [T, 4] tensor on the vertices' device, got ", tets.scalar_type(), " ", tets.sizes());
+	const torch::Tensor p = arg(points, "vertices", torch::kFloat32, {-1, 3}, "[N, 3]"),
+	                    d = arg(sdf.reshape({-1}), "sdf", torch::kFloat32, {p.size(0)}, "one value per vertex", &p),
+	                    s = arg(scales.reshape({-1}), "scales", torch::kFloat32, {p.size(0)}, "one value per vertex", &p),
+	                    t = arg(tets, "tets", torch::kInt64, {-1, 4}, "[T, 4]", &p);
 	const c10::cuda::CUDAGuard guard(p.device());
-	const torch::Tensor t = tets.contiguous();
-	torch::Tensor interp = dtu_bytes(p), ends = dtu_bytes(p), esdf = dtu_bytes(p), escl = dtu_bytes(p), faces = dtu_bytes(p), scratch = dtu_bytes(p),
-	              sort = dtu_bytes(p);
+	torch::Tensor interp = bytes(p), ends = bytes(p), esdf = bytes(p), escl = bytes(p), faces = bytes(p), scratch = bytes(p), sort = bytes(p);
 	rgs_tetra_march_out out{&interp, &ends, &esdf, &escl, &faces, &scratch, &sort, 0, 0};
 	check(rgs_tetra_marching(p.size(0), p.data_ptr<float>(), d.data_ptr<float>(), s.data_ptr<float>(), t.size(0), t.data_ptr<int64_t>(), resize_cb, &out,
 	                         at::cuda::getCurrentCUDAStream().stream()));
 	const int64_t M = out.num_vertices, F = out.num_faces;
-	auto view = [](const torch::Tensor& b, int64_t n, torch::ScalarType ty, at::IntArrayRef shape) {
-		return b.narrow(0, 0, n * (ty == torch::kInt64 ? 8 : 4)).view(ty).view(shape);
-	};
-	return std::make_tuple(view(ends, M * 6, torch::kFloat32, {M, 2, 3}), view(esdf, M * 2, torch::kFloat32, {M, 2, 1}),
-	                       view(escl, M * 2, torch::kFloat32, {M, 2, 1}), view(faces, F * 3, torch::kInt64, {F, 3}), view(interp, M * 2, torch::kInt64, {M, 2}));
+	return std::make_tuple(rows(ends, torch::kFloat32, M, {2, 3}), rows(esdf, torch::kFloat32, M, {2, 1}), rows(escl, torch::kFloat32, M, {2, 1}),
+	                       rows(faces, torch::kInt64, F, {3}), rows(interp, torch::kInt64, M, {2}));
 }
 
 // one bisection step in place: left, right f32 [M,3], left_sdf, right_sdf f32 [M] (or [M,1]), mid f32 [M,3]; mid_sdf f32 [M] or empty
 void TetraBisect(const torch::Tensor& mid_sdf, torch::Tensor left, torch::Tensor right, torch::Tensor left_sdf, torch::Tensor right_sdf, torch::Tensor mid) {
+	arg(left, "left", torch::kFloat32, {-1, 3}, "[M, 3]", nullptr, REJECT);
 	const int64_t M = left.size(0);
-	for (const torch::Tensor* t : {&left, &right, &mid})
-		TORCH_CHECK(t->is_cuda() && t->device() == left.device() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == M * 3,
-		            "left, right and mid must be contiguous CUDA float32 [M, 3] tensors on one device");
-	for (const torch::Tensor* t : {&left_sdf, &right_sdf})
-		TORCH_CHECK(t->device() == left.device() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == M,
-		            "left_sdf and right_sdf must be contiguous float32 [M] tensors on the points' device");
+	arg(right, "right", torch::kFloat32, {M, 3}, "[M, 3]", &left, REJECT);
+	arg(mid, "mid", torch::kFloat32, {M, 3}, "[M, 3]", &left, REJECT);
+	arg(left_sdf, "left_sdf", torch::kFloat32, {M}, "[M]", &left, REJECT);
+	arg(right_sdf, "right_sdf", torch::kFloat32, {M}, "[M]", &left, REJECT);
 	torch::Tensor m;
-	if (mid_sdf.numel() > 0) {
-		m = tetra_f32(mid_sdf.reshape({-1}), 0, "mid_sdf", &left);
-		TORCH_CHECK(m.size(0) == M, "mid_sdf must have one value per vertex (", M, "), got ", mid_sdf.sizes());
-	}
+	if (mid_sdf.numel() > 0) m = arg(mid_sdf.reshape({-1}), "mid_sdf", torch::kFloat32, {M}, "one value per vertex", &left);
 	const c10::cuda::CUDAGuard guard(left.device());
 	check(rgs_tetra_bisect(M, m.defined() ? m.data_ptr<float>() : nullptr, left.data_ptr<float>(), right.data_ptr<float>(), left_sdf.data_ptr<float>(),
 	                       right_sdf.data_ptr<float>(), mid.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
@@ -1200,18 +1137,16 @@ void TetraBisect(const torch::Tensor& mid_sdf, torch::Tensor left, torch::Tensor
 // points f32 [M,3], ends f32 [M,2,3], end_scales f32 [M,2(,1)], faces int64 [F,3] -> (vertices f32 [V',3], faces int64 [F',3])
 std::tuple<torch::Tensor, torch::Tensor> TetraFilter(const torch::Tensor& points, const torch::Tensor& ends, const torch::Tensor& end_scales,
                                                      const torch::Tensor& faces) {
-	const torch::Tensor p = tetra_f32(points, 3, "points"), e = tetra_f32(ends, 6, "ends", &p), s = tetra_f32(end_scales, 2, "end_scales", &p);
-	TORCH_CHECK(e.size(0) == p.size(0) && s.size(0) == p.size(0), "ends and end_scales must have one row per vertex");
-	TORCH_CHECK(faces.is_cuda() && faces.device() == p.device() && faces.scalar_type() == torch::kInt64 && faces.dim() == 2 && faces.size(1) == 3,
-	            "faces must be a CUDA int64 [F, 3] tensor on the points' device, got ", faces.scalar_type(), " ", faces.sizes());
+	const torch::Tensor p = arg(points, "points", torch::kFloat32, {-1, 3}, "[M, 3]"),
+	                    e = arg(ends, "ends", torch::kFloat32, {p.size(0), 2, 3}, "[M, 2, 3]", &p),
+	                    s = arg(end_scales.reshape({-1}), "end_scales", torch::kFloat32, {2 * p.size(0)}, "[M, 2]", &p),
+	                    f = arg(faces, "faces", torch::kInt64, {-1, 3}, "[F, 3]", &p);
 	const c10::cuda::CUDAGuard guard(p.device());
-	const torch::Tensor f = faces.contiguous();
-	torch::Tensor verts = dtu_bytes(p), fout = dtu_bytes(p), scratch = dtu_bytes(p);
+	torch::Tensor verts = bytes(p), fout = bytes(p), scratch = bytes(p);
 	rgs_tetra_filter_out out{&verts, &fout, &scratch, 0, 0};
 	check(rgs_tetra_filter(p.size(0), p.data_ptr<float>(), e.data_ptr<float>(), s.data_ptr<float>(), f.size(0), f.data_ptr<int64_t>(), resize_cb, &out,
 	                       at::cuda::getCurrentCUDAStream().stream()));
-	return std::make_tuple(verts.narrow(0, 0, out.num_vertices * 12).view(torch::kFloat32).view({out.num_vertices, 3}),
-	                       fout.narrow(0, 0, out.num_faces * 24).view(torch::kInt64).view({out.num_faces, 3}));
+	return std::make_tuple(rows(verts, torch::kFloat32, out.num_vertices, {3}), rows(fout, torch::kInt64, out.num_faces, {3}));
 }
 
 }  // namespace

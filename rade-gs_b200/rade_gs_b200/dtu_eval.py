@@ -45,7 +45,7 @@ from . import ply_io
 def _device(device) -> torch.device:
     d = torch.device(device)
     if d.type != "cuda":
-        raise RuntimeError("dtu_eval runs on a CUDA device: there is no CPU path")
+        raise RuntimeError("mesh evaluation runs on a CUDA device: there is no CPU path")
     return d
 
 

@@ -44,28 +44,12 @@ import torch
 from diff_gaussian_rasterization import _C
 
 from . import ply_io
+from .dtu_eval import _device, _points, nearest_distances  # noqa: F401  (nearest_distances is part of this module's API)
 
 # eval_tnt/config.py: the scenes' distance threshold tau (metres)
 SCENES_TAU = {"Barn": 0.01, "Caterpillar": 0.005, "Church": 0.025, "Courthouse": 0.025, "Ignatius": 0.003, "Meetingroom": 0.01, "Truck": 0.005}
 MAX_POINT_NUMBER = 4e6   # registration.py: the last stage keeps every k-th point above this many
 PLOT_STRETCH = 5
-
-
-def _device(device) -> torch.device:
-    d = torch.device(device)
-    if d.type != "cuda":
-        raise RuntimeError("tnt_eval runs on a CUDA device: there is no CPU path")
-    return d
-
-
-def _points(x, device, name: str) -> torch.Tensor:
-    t = x.detach() if isinstance(x, torch.Tensor) else torch.as_tensor(np.asarray(x))
-    t = t.to(device=device, dtype=torch.float64)
-    if t.dim() != 2 or t.shape[1] != 3:
-        raise ValueError(f"{name} must be [N, 3], got {tuple(t.shape)}")
-    if t.numel() and not bool(torch.isfinite(t).all()):
-        raise ValueError(f"{name} has NaN or infinite coordinates")
-    return t.contiguous()
 
 
 def _transform(T, name: str = "transform") -> np.ndarray:
@@ -209,15 +193,6 @@ def uniform_for_registration(points) -> torch.Tensor:
     """registration.py's "uniform" branch: every k-th point, k = int(round(n / 4e6)), only above 4e6 points."""
     n = len(points)
     return uniform_down_sample(points, int(round(n / float(MAX_POINT_NUMBER)))) if n > MAX_POINT_NUMBER else points
-
-
-def nearest_distances(reference, query, device="cuda"):
-    """(distance float64 [N], index int64 [N]) of each query point to its nearest reference point (rgs_dtu_nearest)."""
-    dev = _device(device)
-    r, q = _points(reference, dev, "reference"), _points(query, dev, "query")
-    if r.shape[0] == 0:
-        raise ValueError("the reference set is empty")
-    return _C.dtu_nearest(r, q)
 
 
 def icp_moments(source, target, dist, index, threshold: float) -> np.ndarray:
