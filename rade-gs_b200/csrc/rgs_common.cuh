@@ -190,6 +190,11 @@ __device__ constexpr float kSH2[5] = {1.0925484305920792f, -1.0925484305920792f,
 __device__ constexpr float kSH3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f, 0.3731763325901154f,
                                       -0.4570457994644658f, 1.445305721320277f, -0.5900435899266435f};
 
+// 16-byte vector reduction into global memory (sm_90): one REDG lands four consecutive floats.
+__device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
+	asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
 // ---- host-side launch bookkeeping -----------------------------------------------------------------
 void count_launch(int n = 1);
 

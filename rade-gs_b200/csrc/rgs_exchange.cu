@@ -62,10 +62,6 @@ struct rgs_exchange {
 
 namespace rgs {
 
-__device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
-	asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-
 // One thread per Gaussian finds the rows this rank's slab touched (coalesced read of the per-splat tile counts); the rows found by a
 // warp are then handled one after the other by its first RQ lanes (RQ = float4 per row, 4 or 8): read the local row, clear it
 // (self-cleaning accumulator), add the non-zero quarters into the OWNER's `sum` row over NVLink and raise the owner's per-row mark so

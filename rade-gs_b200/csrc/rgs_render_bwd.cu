@@ -4,10 +4,10 @@
 // dispatch :1101-1163).  The per-pixel recurrence (back-to-front re-traversal, T recovered by division,
 // running suffix blends, median terms) is the reference's; the gradient scatter is not:
 //   * the reference issues 10/16/22/25 scalar global atomicAdds per contributing (pixel, splat) pair
-//     (backward.cu:878-1013).  Here the 32 pixels of a warp evaluate the same splat in lock-step, the
-//     16 (or 32) per-splat partial gradients are combined with a recursive-halving shuffle
-//     reduce-scatter (16 resp. 31 SHFL instead of 80 resp. 125 for a butterfly per value), and ONE
-//     coalesced red.global.add of 64 B (128 B) per (warp, splat) lands in a packed accumulator row;
+//     (backward.cu:878-1013).  Here the 32 pixels of a warp evaluate the same splat in lock-step, each lane
+//     writes its 16 (or 25) partial gradients of the hit to shared memory, and after every group of K hits the
+//     warp sums the group through that transpose: lane -> (hit, 4-float slice, 8 of the 32 pixels), a
+//     two-step shuffle tail, and one 16-byte red.global.add.v4.f32 per (hit, slice) into a packed accumulator row;
 //   * constant factors (0.5*W, 0.5*H, 1/focal) are pulled out of the sums and applied once per Gaussian
 //     in backward-preprocess;
 //   * the tile list is cut at the block-wide maximum of last_contributor (nothing behind it can receive
@@ -21,34 +21,40 @@ namespace rgs {
 
 namespace {
 
-// Recursive-halving reduce-scatter over a warp.  On return lane L holds, in v[0], the warp-wide sum of
-// value index (L >> 1) for N == 16 (both lanes of a pair hold it) or index L for N == 32.
-template <int N>
-__device__ __forceinline__ void warp_reduce_scatter(float (&v)[N], int lane) {
-	static_assert(N == 16 || N == 32, "16 or 32 values");
-#pragma unroll
-	for (int h = N / 2, mask = 16; h >= 2; h >>= 1, mask >>= 1) {
-		const bool upper = (lane & mask) != 0;
-#pragma unroll
-		for (int k = 0; k < h; k += 2) {
-			// two values per step, added lane by lane (fadd2)
-			const float s0 = upper ? v[k] : v[k + h], s1 = upper ? v[k + 1] : v[k + h + 1];
-			const float2 keep = make_float2(upper ? v[k + h] : v[k], upper ? v[k + h + 1] : v[k + 1]);
-			const float2 recv = make_float2(__shfl_xor_sync(0xffffffffu, s0, mask), __shfl_xor_sync(0xffffffffu, s1, mask));
-			const float2 sum = fadd2(keep, recv);
-			v[k] = sum.x;
-			v[k + 1] = sum.y;
-		}
-	}
-	{
-		const int mask = (N == 16) ? 2 : 1;
-		const bool upper = (lane & mask) != 0;
-		const float send = upper ? v[0] : v[1];
-		const float keep = upper ? v[1] : v[0];
-		v[0] = keep + __shfl_xor_sync(0xffffffffu, send, mask);
-	}
-	if (N == 16) v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
+// Backward stages 128 records per round, half of forward's BATCH: the smaller ring leaves room for the hit groups below at
+// 4 CTAs per SM (none / depth: 17 + 36 KB) and 3 (coord: 25 + 31.5 KB).  The hit-mask words are indexed by list position, so
+// the round size is backward's own choice.  Measured at C2 on one H100 (depth variant, render_backward stage): 128 records and
+// K = 2 at 4 CTAs/SM 1.25 ms; 256 records and K = 2 at 3 CTAs/SM 1.30 ms; 128 records and K = 4 at 2 CTAs/SM 1.44 ms
+// (H100 80GB HBM3, 700 W power limit).
+constexpr int BWD_BATCH = 128;
+
+// Gradient rows of the hits a warp has queued but not yet summed.  Per warp [K][NQ][S] float4: row (hit, slice) holds
+// that slice of the hit's partial gradients for the 32 pixels (lane-contiguous, so each store of the queueing side is one
+// conflict-free 512-B warp store).  At a flush lane l sums row (l / L) over the pixels (l % L) + L*t, t < PIX, and the L
+// lanes of a row finish with a shuffle butterfly.  The row stride S = 32 + L puts the 8 lanes of a quarter-warp on 8
+// different 16-B bank groups while every lane walks its pixels at constant immediate offsets.
+template <bool COORD>
+struct HitGroup {
+	static constexpr int NC = (COORD ? GRAD_FLOATS_COORD : GRAD_FLOATS_BASE) / 4;  // float4 slices of an accumulator row
+	static constexpr int NQ = COORD ? 7 : 4;  // slices that carry data: floats 25..31 of a coord row are padding
+	static constexpr int K = COORD ? 1 : 2;  // hits per group: K * NC = 8 rows, 4 lanes per row (see BWD_BATCH)
+	static constexpr int CTAS = COORD ? 3 : 4;  // per SM: registers (<= 64 resp. 85) and shared memory both allow it
+	static constexpr int L = 32 / (K * NC);
+	static constexpr int PIX = 32 / L;
+	static constexpr int S = 32 + L;
+	static constexpr int WARP_FLOAT4 = K * NQ * S;
+	static_assert(K * NC <= 32 && 32 % (K * NC) == 0 && PIX >= 8, "lanes must split evenly over (hit, slice) rows");
+};
+
+template <bool COORD>
+constexpr size_t backward_smem_bytes() {
+	constexpr int RFQ = COORD ? 6 : 4;
+	return (size_t)2 * RFQ * BWD_BATCH * sizeof(float4) + (size_t)2 * BWD_BATCH * sizeof(int) +
+	       (size_t)(NTHREADS / 32) * HitGroup<COORD>::WARP_FLOAT4 * sizeof(float4);
 }
+// 228 KB of shared memory per SM, 1 KB of it reserved per resident CTA
+static_assert(HitGroup<false>::CTAS * (backward_smem_bytes<false>() + 1024 + 64) <= 228 * 1024, "none / depth: CTAs per SM");
+static_assert(HitGroup<true>::CTAS * (backward_smem_bytes<true>() + 1024 + 64) <= 228 * 1024, "coord: CTAs per SM");
 
 __device__ __forceinline__ float rcp_approx(float x) {
 	float r;
@@ -69,7 +75,7 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
 }  // namespace
 
 template <bool COORD, bool DEPTH>
-__global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_kernel(
+__global__ void __launch_bounds__(NTHREADS, HitGroup<COORD>::CTAS) render_backward_kernel(
     const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, const float* __restrict__ records,
     int W, int H, int py_off, int Hs, int grid_x, int row_begin, float focal_x, float focal_y, const float* __restrict__ bg_color,
     const float* __restrict__ alphas, const float* __restrict__ normalmap, const uint32_t* __restrict__ n_contrib,
@@ -81,13 +87,16 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 	constexpr bool GEO = COORD || DEPTH;
 	constexpr int RFQ = COORD ? 6 : 4;
 	constexpr int GF = COORD ? GRAD_FLOATS_COORD : GRAD_FLOATS_BASE;
-	extern __shared__ float4 smem[];  // [2][RFQ][BATCH] records, then [2][BATCH] ids
+	constexpr int BATCH = BWD_BATCH;
+	using HG = HitGroup<COORD>;
+	extern __shared__ float4 smem[];  // [2][RFQ][BATCH] records, [2][BATCH] ids, then per warp the HitGroup rows
 	int* s_ids = reinterpret_cast<int*>(smem + 2 * RFQ * BATCH);
 	const uint32_t smem_base = (uint32_t)__cvta_generic_to_shared(smem);
 	__shared__ int s_block_last[NTHREADS / 32];
 
 	const int tid = threadIdx.x;
 	const int warp = tid >> 5, lane = tid & 31;
+	float4* grp = smem + 2 * RFQ * BATCH + 2 * BATCH / 4 + warp * HG::WARP_FLOAT4;
 	const int tile_x = blockIdx.x, tile_y = blockIdx.y + row_begin;
 	const int bx0 = tile_x * TILE_X + (warp & 1) * 8, by0 = tile_y * TILE_Y + (warp >> 1) * 4;
 	const int px = bx0 + (lane & 7), py = by0 + (lane >> 3);
@@ -186,7 +195,9 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 	const float ddelx_dx = 0.5 * W;
 	const float ddely_dy = 0.5 * H;
 
-	// staged index j of round i is list position  n-1 - (i*BATCH + j)
+	// staged index j of round i is list position  n-1 - (i*BATCH + j); threads tid < BATCH stage one record each
+	static_assert(BATCH <= NTHREADS && BATCH % 32 == 0, "one staged record per thread of the first BATCH");
+	const bool stager = tid < BATCH;
 	const size_t rec_stride = (size_t)RFQ * 4;
 	auto issue_gather = [&](int stage, int id) {
 		if (id >= 0) {
@@ -195,12 +206,43 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 #pragma unroll
 			for (int c = 0; c < RFQ; c++) cp_async16(dst + c * BATCH, src + c);
 		}
-		s_ids[stage * BATCH + tid] = id;
+		if (stager) s_ids[stage * BATCH + tid] = id;
 		cp_async_commit();
 	};
-	int id_cur = (tid < n) ? (int)point_list[range.x + n - 1 - tid] : -1;
+	int id_cur = (stager && tid < n) ? (int)point_list[range.x + n - 1 - tid] : -1;
 	issue_gather(0, id_cur);
-	int id_next = (BATCH + tid < n) ? (int)point_list[range.x + n - 1 - BATCH - tid] : -1;
+	int id_next = (stager && BATCH + tid < n) ? (int)point_list[range.x + n - 1 - BATCH - tid] : -1;
+
+	// Queue of hits whose gradient rows wait in `grp` (q of them, warp-uniform); lane h holds the Gaussian id of hit h.  The
+	// queue lives in registers and its own shared memory, not in the record ring, so it carries over batch boundaries and is
+	// summed when it holds K hits and once after the last batch.
+	int q = 0, qid = 0;
+	const int f_row = lane / HG::L, f_sub = lane % HG::L;
+	const int f_hit = f_row / HG::NC, f_slice = f_row % HG::NC;
+	const float4* f_src = grp + (f_hit * HG::NQ + f_slice) * HG::S + f_sub;
+	auto flush = [&](int nq) {
+		__syncwarp();
+		const bool live = f_hit < nq && f_slice < HG::NQ;
+		float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+		if (live) {
+			a = f_src[0];
+#pragma unroll
+			for (int t = 1; t < HG::PIX; t++) {
+				const float4 b = f_src[t * HG::L];
+				a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+			}
+		}
+#pragma unroll
+		for (int o = 1; o < HG::L; o <<= 1) {
+			a.x += __shfl_xor_sync(0xffffffffu, a.x, o);
+			a.y += __shfl_xor_sync(0xffffffffu, a.y, o);
+			a.z += __shfl_xor_sync(0xffffffffu, a.z, o);
+			a.w += __shfl_xor_sync(0xffffffffu, a.w, o);
+		}
+		const int id = __shfl_sync(0xffffffffu, qid, f_hit);
+		if (live && f_sub == 0) red_add_v4(grad_accum + (size_t)id * GF + 4 * f_slice, a);
+		__syncwarp();  // the rows are rewritten by the next hits
+	};
 
 	for (int i = 0; i < rounds; i++) {
 		cp_async_wait_all();
@@ -208,7 +250,7 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 		if (i + 1 < rounds) {
 			issue_gather((i + 1) & 1, id_next);
 			const int nxt = (i + 2) * BATCH + tid;
-			id_next = (nxt < n) ? (int)point_list[range.x + n - 1 - nxt] : -1;
+			id_next = (stager && nxt < n) ? (int)point_list[range.x + n - 1 - nxt] : -1;
 		}
 		const float4* s = smem + (size_t)(i & 1) * RFQ * BATCH;
 		const uint32_t s_addr = smem_base + (uint32_t)((i & 1) * RFQ * BATCH * 16);
@@ -221,7 +263,7 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 		// lane l fetches word (pos0>>5) - l, chunks below pick theirs up with a shuffle
 		const int k_hi = pos0 >> 5;
 		uint32_t wl = 0;
-		if (lane <= 9 && k_hi - lane >= 0) wl = __ldg(my_mask + (size_t)(k_hi - lane) * 8);
+		if (lane <= BATCH / 32 + 1 && k_hi - lane >= 0) wl = __ldg(my_mask + (size_t)(k_hi - lane) * 8);
 
 		for (int c0 = 0; c0 < cnt; c0 += 32) {
 			// staged index j of this chunk <-> list position hi - j
@@ -342,22 +384,24 @@ __global__ void __launch_bounds__(NTHREADS, (COORD ? 3 : 4)) render_backward_ker
 				gv[G_CONY] = cxy.y;
 				gv[G_CONW] = gd.y * dy * hG;
 				gv[G_OPA] = Gm * dL_dopa;
-				warp_reduce_scatter<GF>(gv, lane);
-				float* row = grad_accum + (size_t)lds32(ids_addr + (uint32_t)jj * 4u) * GF;
-				if (GF == 16) {
-					if ((lane & 1) == 0) atomicAdd(row + (lane >> 1), gv[0]);
-				} else {
-					if (lane < 25) atomicAdd(row + lane, gv[0]);
+				float4* slot = grp + q * (HG::NQ * HG::S) + lane;
+#pragma unroll
+				for (int c = 0; c < HG::NQ; c++) slot[c * HG::S] = make_float4(gv[4 * c], gv[4 * c + 1], gv[4 * c + 2], gv[4 * c + 3]);
+				const int hit_id = lds32(ids_addr + (uint32_t)jj * 4u);
+				if (lane == q) qid = hit_id;
+				if (++q == HG::K) {
+					flush(HG::K);
+					q = 0;
 				}
 			}
 		}
 	}
+	if (q > 0) flush(q);
 }
 
 template <bool COORD, bool DEPTH>
 static void launch_variant(const FwdParams& p, GeomView g, BinView b, ImgView img, RenderGradIn gin, float* grad_accum, cudaStream_t s) {
-	constexpr int RFQ = COORD ? 6 : 4;
-	const size_t smem = (size_t)2 * RFQ * BATCH * sizeof(float4) + (size_t)2 * BATCH * sizeof(int);
+	const size_t smem = backward_smem_bytes<COORD>();
 	auto kern = render_backward_kernel<COORD, DEPTH>;
 	static size_t configured[64] = {};
 	ensure_dynamic_smem(kern, smem, configured);
