@@ -642,6 +642,77 @@ typedef struct rgs_tetra_filter_out {
 int32_t rgs_tetra_filter(int64_t M, const float* points, const float* ends, const float* end_scales, int64_t F, const int64_t* faces, rgs_resize_fn resize,
                          rgs_tetra_filter_out* out, void* cuda_stream);
 
+/* ---- densify-and-prune and opacity reset (reference scene/gaussian_model.py:495-513 reset_opacity, :662-741 densify_and_prune) ----
+ * Inputs per Gaussian (fp32, device): grad_accum, grad_accum_abs, denom [P] (the [P,1] statistics), raw scaling [P,3], raw
+ * opacity [P], rotation [P,4], xyz [P,3]; 0 < P < 2^31.
+ *
+ * Floating-point contract.
+ *   - Selections, counts, row order and every copied float are bit-exact against the reference run on CUDA.
+ *   - exp, log and sigmoid = 1 / (1 + exp(-x)) are the accurate libdevice functions (no fast-math), as torch's CUDA kernels
+ *     compute them.  Every other operation is one IEEE fp32 operation rounded on its own, in the order written below.
+ *   - g = accum / denom and g_abs = accum_abs / denom; NaN (0/0, NaN inputs) becomes 0, x/0 for x > 0 stays +inf.
+ *   - |g| for the clone and ratio tests is torch.norm of a one-element row on CUDA: sqrt(g * g) in fp32.
+ *   - ratio = (float)count * (1.0f / (float)P), count = #{|g| >= max_grad}, as ATen's CUDA mean (a sum times the fp32
+ *     reciprocal; torch on the CPU divides instead).  Exact while count <= 2^24.
+ *   - Q = torch.quantile(g_abs, 1 - ratio), linear: q = 1 - ratio, rank = q * (float)(P - 1), lo = (int64)rank,
+ *     hi = ceil(rank), w = rank - lo, a = sorted[lo], b = sorted[hi] (indices clamped to P - 1, which only binds above 2^24
+ *     rows), d = b - a, Q = |w| < 0.5 ? fma(w, d, a) : fma(-d, 1 - w, b) (torch.lerp as built for CUDA).  The order statistics
+ *     come from a full radix sort of g_abs, so Q is exact for any P; there is no 2^24 limit.
+ *   - clone = (|g| >= max_grad or |g_abs| >= Q) and max_k exp(s_k) <= dense; split = (g >= max_grad or g_abs >= Q) and
+ *     max_k exp(s_k) > dense, over the original rows.  A clone carries its parent's raw scaling bit for bit, so the same
+ *     max exp(s) <= dense that made it a clone keeps it from being split.
+ *   - New rows: q = r / sqrt(((r0 r0 + r1 r1) + r2 r2) + r3 r3); R as build_rotation (utils/general_utils.py:80-101), each
+ *     product, sum and difference rounded (2 * t and 1 - t as written); xyz_new_i = ((R_i0 s0 + R_i1 s1) + R_i2 s2) + xyz_i,
+ *     every product and sum rounded, left to right.  This is the order of torch.bmm on the CPU; cuBLAS's torch.bmm on CUDA
+ *     may order or fuse the three products differently, which moves xyz_new_i by at most
+ *     2^-21 * (|R_i0 s0| + |R_i1 s1| + |R_i2 s2| + |xyz_i|).  The same bound covers torch on the CPU, whose vectorised sqrt
+ *     (the quaternion norm) is not correctly rounded; CUDA's sqrtf, used here, is.
+ *   - Split children: scaling log(exp(s) * (1.0f / 1.6f)) (torch on CUDA multiplies by the fp32 reciprocal of a Python
+ *     scalar divisor; on the CPU it divides: the two differ by at most one rounding of the quotient).
+ *   - Prune: sigmoid(o) < min_opacity, or, when prune_large: 0 > max_screen_size (max_radii2D is all zeros by then) or
+ *     max_k exp(s_k) > world.  Python thresholds are rounded to fp32 first (max_grad, dense = percent_dense * extent,
+ *     min_opacity, max_screen_size, world = 0.1 * extent), as torch compares a float32 tensor with a Python scalar.
+ *   - reset_opacity: coef = sqrt(((sq0 sq1) sq2) / ((a0 a1) a2)), sq_k = exp(s_k)^2, a_k = sq_k + f^2; o = sigmoid(x) * coef;
+ *     x' = min(o, 0.01f) / coef; result log(x' / (1 - x')).
+ *
+ * Output rows, in order: the original rows not split, the clones, the first child of every split row, the second child of
+ * every split row, each in index order and each without the rows the final prune drops.
+ *
+ * rgs_densify_select: flags [P] (one byte per Gaussian), block_offsets [5 * rgs_densify_blocks(P) + 5] (per-CTA offsets, then
+ *   the totals), ratio_q [2] (device:
+ *   ratio, Q) and counts_host [5] (host: C clones, S split rows, surviving originals K0, surviving clones K1, surviving
+ *   children per copy K2; the result has K0 + K1 + 2 K2 rows).  Scratch through the resize callback (about 8 bytes per
+ *   Gaussian plus the sort's workspace).  One stream synchronisation (the counts).
+ * rgs_densify_plan: src, draw [K0 + K1 + 2 K2] (source row and draw index of every output row, draw -1 on original rows,
+ *   draw < C a clone's row of the clone draws, draw >= C row draw - C of the split draws) and the exp(scaling) rows packed
+ *   as the std of the draws: std_clone [C,3], std_split [2S,3] (stds.repeat(2, 1)).
+ * rgs_densify_gather: xyz_out and scaling_out [N,3] of every output row from the caller's draws sample_clone [C,3] and
+ *   sample_split [2S,3]; every other column through cols: out[j] = in[src[j]] (width floats per row), zeros on new rows
+ *   when zero_new_rows.
+ * rgs_reset_opacity: out [P] as above. */
+#define RGS_DENSIFY_MAX_COLUMNS 18
+typedef struct rgs_densify_thresholds {
+	float max_grad, dense, min_opacity, max_screen_size, world;
+	float inv_split;       /* 1.0f / (float)(0.8 * N), N = 2 */
+	int32_t prune_large;   /* max_screen_size is truthy */
+} rgs_densify_thresholds;
+typedef struct rgs_densify_column {
+	const float* in;       /* [P, width] */
+	float* out;            /* [N, width] */
+	int64_t width;
+	int32_t zero_new_rows;
+} rgs_densify_column;
+int32_t rgs_densify_blocks(int32_t P);
+int32_t rgs_densify_select(int32_t P, const float* grad_accum, const float* grad_accum_abs, const float* denom, const float* scaling, const float* opacity,
+                           const rgs_densify_thresholds* thresholds, uint8_t* flags, int32_t* block_offsets, float* ratio_q, int32_t* counts_host,
+                           rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+int32_t rgs_densify_plan(int32_t P, const uint8_t* flags, const int32_t* block_offsets, const int32_t* counts_host, const float* scaling, int32_t* src,
+                         int32_t* draw, float* std_clone, float* std_split, void* cuda_stream);
+int32_t rgs_densify_gather(int32_t N, const int32_t* src, const int32_t* draw, int32_t C, const float* xyz, const float* rotation, const float* scaling,
+                           const float* sample_clone, const float* sample_split, float inv_split, float* xyz_out, float* scaling_out, int32_t n_cols,
+                           const rgs_densify_column* cols, void* cuda_stream);
+int32_t rgs_reset_opacity(int32_t P, const float* scaling, const float* opacity, const float* filter_3D, float* out, void* cuda_stream);
+
 /* Introspection for parity tests: views into the private buffers written by rgs_forward
  * (the reference keeps the same data at BinningState::point_list / ImageState::ranges,
  * rasterizer_impl.cu:237-250,224-235).  Pointers are device addresses inside the given buffers. */

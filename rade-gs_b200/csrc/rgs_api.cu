@@ -1011,6 +1011,57 @@ int32_t rgs_appearance_l1_backward(int32_t H0, int32_t W0, const float* image, c
 	                   "appearance l1 backward");
 }
 
+int32_t rgs_densify_blocks(int32_t P) { return P > 0 ? densify_blocks(P) : 0; }
+
+int32_t rgs_densify_select(int32_t P, const float* grad_accum, const float* grad_accum_abs, const float* denom, const float* scaling, const float* opacity,
+                           const rgs_densify_thresholds* thresholds, uint8_t* flags, int32_t* block_offsets, float* ratio_q, int32_t* counts_host,
+                           rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (P <= 0) return fail(RGS_E_INVALID, "densify: the model has no Gaussians");
+	if (!grad_accum || !grad_accum_abs || !denom || !scaling || !opacity || !thresholds || !flags || !block_offsets || !ratio_q || !counts_host || !scratch)
+		return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	char* buf = nullptr;
+	if (const int rc = grow(scratch, scratch_user, densify_select_scratch_bytes(P), buf, "densify scratch")) return rc;
+	// the five totals follow the per-CTA offsets in the scratch's tail: one copy brings them to the host
+	int32_t* totals = block_offsets + 5 * (size_t)densify_blocks(P);
+	cudaError_t e = launch_densify_select(P, grad_accum, grad_accum_abs, denom, scaling, opacity, *thresholds, flags, block_offsets, ratio_q, totals, buf, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(counts_host, totals, 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+	return cuda_status(e, "densify select");
+}
+
+int32_t rgs_densify_plan(int32_t P, const uint8_t* flags, const int32_t* block_offsets, const int32_t* counts_host, const float* scaling, int32_t* src,
+                         int32_t* draw, float* std_clone, float* std_split, void* cuda_stream) {
+	if (P <= 0) return fail(RGS_E_INVALID, "densify: the model has no Gaussians");
+	if (!flags || !block_offsets || !counts_host || !scaling) return fail(RGS_E_INVALID, "null pointer");
+	const int32_t* c = counts_host;
+	for (int k = 0; k < 5; k++)
+		if (c[k] < 0 || c[k] > P) return fail(RGS_E_INVALID, "densify plan: counts out of range");
+	if ((c[0] && !std_clone) || (c[1] && !std_split) || ((c[2] || c[3] || c[4]) && (!src || !draw))) return fail(RGS_E_INVALID, "null pointer");
+	return cuda_status(launch_densify_plan(P, flags, block_offsets, counts_host, scaling, src, draw, std_clone, std_split, (cudaStream_t)cuda_stream),
+	                   "densify plan");
+}
+
+int32_t rgs_densify_gather(int32_t N, const int32_t* src, const int32_t* draw, int32_t C, const float* xyz, const float* rotation, const float* scaling,
+                           const float* sample_clone, const float* sample_split, float inv_split, float* xyz_out, float* scaling_out, int32_t n_cols,
+                           const rgs_densify_column* cols, void* cuda_stream) {
+	if (N < 0 || C < 0 || n_cols < 0 || n_cols > RGS_DENSIFY_MAX_COLUMNS) return fail(RGS_E_INVALID, "densify gather: bad sizes");
+	if (N == 0) return RGS_OK;
+	if (!src || !draw || !xyz || !rotation || !scaling || !xyz_out || !scaling_out || (n_cols && !cols)) return fail(RGS_E_INVALID, "null pointer");
+	for (int k = 0; k < n_cols; k++)
+		if (!cols[k].in || !cols[k].out || cols[k].width <= 0) return fail(RGS_E_INVALID, "densify gather: bad column");
+	return cuda_status(launch_densify_gather(N, src, draw, C, xyz, rotation, scaling, sample_clone, sample_split, inv_split, xyz_out, scaling_out, n_cols,
+	                                         cols, (cudaStream_t)cuda_stream),
+	                   "densify gather");
+}
+
+int32_t rgs_reset_opacity(int32_t P, const float* scaling, const float* opacity, const float* filter_3D, float* out, void* cuda_stream) {
+	if (P < 0) return fail(RGS_E_INVALID, "negative Gaussian count");
+	if (P == 0) return RGS_OK;
+	if (!scaling || !opacity || !filter_3D || !out) return fail(RGS_E_INVALID, "null pointer");
+	return cuda_status(launch_reset_opacity(P, scaling, opacity, filter_3D, out, (cudaStream_t)cuda_stream), "reset opacity");
+}
+
 int32_t rgs_debug_get_views(const rgs_camera* cam, int32_t P, int64_t num_rendered, const char* geom_buffer, const char* binning_buffer,
                             const char* image_buffer, rgs_debug_views* views) {
 	if (!cam || !views) return fail(RGS_E_INVALID, "null pointer");

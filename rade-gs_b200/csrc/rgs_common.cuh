@@ -380,4 +380,17 @@ cudaError_t launch_appearance_l1_backward(int H0, int W0, const float* img, cons
                                           const float* b3, const float* upstream, float* d_img, float* d_up4, float* d_w2, float* d_b2, float* d_w3,
                                           float* d_b3, double* partials, float* d_x, cudaStream_t s);
 
+// densify-and-prune and opacity reset (rgs_densify.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
+int densify_blocks(int P);
+size_t densify_select_scratch_bytes(int P);
+cudaError_t launch_densify_select(int P, const float* accum, const float* accum_abs, const float* denom, const float* scaling, const float* opacity,
+                                  const rgs_densify_thresholds& th, uint8_t* flags, int* block_offsets, float* ratio_q, int* totals, char* scratch,
+                                  cudaStream_t s);
+cudaError_t launch_densify_plan(int P, const uint8_t* flags, const int* block_offsets, const int32_t* counts, const float* scaling, int* src, int* draw,
+                                float* std_clone, float* std_split, cudaStream_t s);
+cudaError_t launch_densify_gather(int N, const int* src, const int* draw, int C, const float* xyz, const float* rotation, const float* scaling,
+                                  const float* sample_clone, const float* sample_split, float inv_split, float* xyz_out, float* scaling_out, int n_cols,
+                                  const rgs_densify_column* cols, cudaStream_t s);
+cudaError_t launch_reset_opacity(int P, const float* scaling, const float* opacity, const float* filter_3D, float* out, cudaStream_t s);
+
 }  // namespace rgs

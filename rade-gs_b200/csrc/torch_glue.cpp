@@ -800,6 +800,127 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
 	return std::make_tuple(d_img, d_up4, d_w2, d_b2, d_w3, d_b3);
 }
 
+// ---- densify-and-prune and opacity reset (scene/gaussian_model.py:495-513, :662-741; rgs_densify_*, rgs_reset_opacity) ----------
+
+// a per-Gaussian input: float32 on `like`'s device with `width` floats per row over P rows
+torch::Tensor per_gaussian(const torch::Tensor& t, const char* name, int64_t P, int64_t width, const torch::Tensor* like) {
+	const torch::Tensor a = arg(t, name, torch::kFloat32, {}, "", like);
+	TORCH_CHECK(a.dim() >= 1 && a.size(0) == P && a.numel() == P * width, "densify: ", name, " must have ", width, " float(s) per row over ", P,
+	            " rows, got ", t.sizes());
+	return a;
+}
+
+// returns (flags [P] uint8, block_offsets int32, ratio_q [2] float32 = (ratio, Q), counts (C, S, K0, K1, K2))
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, std::vector<int64_t>> DensifySelect(
+    const torch::Tensor& grad_accum, const torch::Tensor& grad_accum_abs, const torch::Tensor& denom, const torch::Tensor& scaling,
+    const torch::Tensor& opacity, const double max_grad, const double dense, const double min_opacity, const bool prune_large,
+    const double max_screen_size, const double world) {
+	const torch::Tensor acc = arg(grad_accum, "xyz_gradient_accum", torch::kFloat32);
+	TORCH_CHECK(acc.dim() >= 1 && acc.size(0) > 0, "densify: the model has no Gaussians");
+	TORCH_CHECK(acc.size(0) <= INT32_MAX, "densify: at most 2^31 - 1 Gaussians");
+	const int64_t P = acc.size(0);
+	per_gaussian(acc, "xyz_gradient_accum", P, 1, nullptr);
+	const torch::Tensor ab = per_gaussian(grad_accum_abs, "xyz_gradient_accum_abs", P, 1, &acc), dn = per_gaussian(denom, "denom", P, 1, &acc),
+	                    sc = per_gaussian(scaling, "_scaling", P, 3, &acc), op = per_gaussian(opacity, "_opacity", P, 1, &acc);
+	const c10::cuda::CUDAGuard guard(acc.device());
+	const auto o = acc.options();
+	torch::Tensor flags = new_empty({P}, o.dtype(torch::kUInt8));
+	torch::Tensor offsets = new_empty({5 * (int64_t)rgs_densify_blocks((int)P) + 5}, o.dtype(torch::kInt32));
+	torch::Tensor ratio_q = new_empty({2}, o), scratch = bytes(acc);
+	rgs_densify_thresholds th;
+	th.max_grad = (float)max_grad;
+	th.dense = (float)dense;
+	th.min_opacity = (float)min_opacity;
+	th.max_screen_size = (float)max_screen_size;
+	th.world = (float)world;
+	th.inv_split = 1.0f / (float)(0.8 * 2);
+	th.prune_large = prune_large ? 1 : 0;
+	int32_t counts[5];
+	check(rgs_densify_select((int)P, acc.data_ptr<float>(), ab.data_ptr<float>(), dn.data_ptr<float>(), sc.data_ptr<float>(), op.data_ptr<float>(), &th,
+	                         flags.data_ptr<uint8_t>(), offsets.data_ptr<int32_t>(), ratio_q.data_ptr<float>(), counts, resize_cb, &scratch,
+	                         at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(flags, offsets, ratio_q, std::vector<int64_t>(counts, counts + 5));
+}
+
+// returns (src [N] int32, draw [N] int32, std_clone [C,3], std_split [2S,3]), N = K0 + K1 + 2 K2
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> DensifyPlan(const torch::Tensor& flags, const torch::Tensor& block_offsets,
+                                                                                   const std::vector<int64_t>& counts, const torch::Tensor& scaling) {
+	const torch::Tensor f = arg(flags, "flags", torch::kUInt8, {-1}, "[P]");
+	const int64_t P = f.size(0);
+	TORCH_CHECK(P > 0 && P <= INT32_MAX, "densify: the model has no Gaussians");
+	const torch::Tensor bo = arg(block_offsets, "block_offsets", torch::kInt32, {5 * (int64_t)rgs_densify_blocks((int)P) + 5}, "[5 * blocks + 5]", &f);
+	const torch::Tensor sc = per_gaussian(scaling, "_scaling", P, 3, &f);
+	TORCH_CHECK(counts.size() == 5, "densify plan: five counts");
+	int32_t c[5];
+	for (int k = 0; k < 5; k++) {
+		TORCH_CHECK(counts[k] >= 0 && counts[k] <= P, "densify plan: counts out of range");
+		c[k] = (int32_t)counts[k];
+	}
+	const c10::cuda::CUDAGuard guard(f.device());
+	const auto o = sc.options();
+	const int64_t N = (int64_t)c[2] + c[3] + 2 * (int64_t)c[4];
+	torch::Tensor src = new_empty({N}, o.dtype(torch::kInt32)), draw = new_empty({N}, o.dtype(torch::kInt32));
+	torch::Tensor std_clone = new_empty({c[0], 3}, o), std_split = new_empty({2 * (int64_t)c[1], 3}, o);
+	check(rgs_densify_plan((int)P, f.data_ptr<uint8_t>(), bo.data_ptr<int32_t>(), c, sc.data_ptr<float>(), N ? src.data_ptr<int32_t>() : nullptr,
+	                       N ? draw.data_ptr<int32_t>() : nullptr, c[0] ? std_clone.data_ptr<float>() : nullptr,
+	                       c[1] ? std_split.data_ptr<float>() : nullptr, at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(src, draw, std_clone, std_split);
+}
+
+// returns (xyz [N,3], scaling [N,3], one tensor [N, *column.shape[1:]] per column); columns: (tensor [P, ...], zero on new rows)
+std::tuple<torch::Tensor, torch::Tensor, std::vector<torch::Tensor>> DensifyGather(const torch::Tensor& src, const torch::Tensor& draw, const int64_t C,
+                                                                                    const torch::Tensor& xyz, const torch::Tensor& rotation,
+                                                                                    const torch::Tensor& scaling, const torch::Tensor& sample_clone,
+                                                                                    const torch::Tensor& sample_split,
+                                                                                    const std::vector<std::tuple<torch::Tensor, bool>>& columns) {
+	const torch::Tensor x = arg(xyz, "_xyz", torch::kFloat32);
+	const int64_t P = x.size(0);
+	per_gaussian(x, "_xyz", P, 3, nullptr);
+	const torch::Tensor r = per_gaussian(rotation, "_rotation", P, 4, &x), sc = per_gaussian(scaling, "_scaling", P, 3, &x);
+	const torch::Tensor s = arg(src, "src", torch::kInt32, {-1}, "[N]", &x), d = arg(draw, "draw", torch::kInt32, {-1}, "[N]", &x);
+	const int64_t N = s.size(0);
+	TORCH_CHECK(d.size(0) == N, "densify gather: src and draw differ in length");
+	TORCH_CHECK(C >= 0 && C <= P, "densify gather: clone count out of range");
+	const torch::Tensor smc = arg(sample_clone, "clone draws", torch::kFloat32, {C, 3}, "[C, 3]", &x);
+	const torch::Tensor sms = arg(sample_split, "split draws", torch::kFloat32, {-1, 3}, "[2S, 3]", &x);
+	TORCH_CHECK((int64_t)columns.size() <= RGS_DENSIFY_MAX_COLUMNS, "densify gather: at most ", RGS_DENSIFY_MAX_COLUMNS, " columns");
+	const c10::cuda::CUDAGuard guard(x.device());
+	const auto o = x.options();
+	std::vector<torch::Tensor> ins, outs;
+	std::vector<rgs_densify_column> cols;
+	for (const auto& [t, zero_new] : columns) {
+		const torch::Tensor in = arg(t, "column", torch::kFloat32, {}, "", &x);
+		TORCH_CHECK(in.dim() >= 1 && in.size(0) == P, "densify gather: every column must have the model's ", P, " rows, got ", t.sizes());
+		std::vector<int64_t> shape(in.sizes().begin(), in.sizes().end());
+		shape[0] = N;
+		torch::Tensor out = new_empty(shape, o);
+		const int64_t width = P ? in.numel() / P : 0;
+		if (width > 0 && N > 0) cols.push_back(rgs_densify_column{in.data_ptr<float>(), out.data_ptr<float>(), width, zero_new ? 1 : 0});
+		ins.push_back(in);
+		outs.push_back(out);
+	}
+	torch::Tensor xyz_out = new_empty({N, 3}, o), scaling_out = new_empty({N, 3}, o);
+	check(rgs_densify_gather((int)N, s.data_ptr<int32_t>(), d.data_ptr<int32_t>(), (int)C, x.data_ptr<float>(), r.data_ptr<float>(), sc.data_ptr<float>(),
+	                         C ? smc.data_ptr<float>() : nullptr, sms.size(0) ? sms.data_ptr<float>() : nullptr, 1.0f / (float)(0.8 * 2),
+	                         xyz_out.data_ptr<float>(), scaling_out.data_ptr<float>(), (int)cols.size(), cols.data(),
+	                         at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(xyz_out, scaling_out, outs);
+}
+
+// GaussianModel.reset_opacity's new raw opacity [P,1]
+torch::Tensor ResetOpacity(const torch::Tensor& scaling, const torch::Tensor& opacity, const torch::Tensor& filter_3D) {
+	const torch::Tensor op = arg(opacity, "_opacity", torch::kFloat32);
+	const int64_t P = op.size(0);
+	TORCH_CHECK(P > 0 && P <= INT32_MAX, "reset_opacity: the model has no Gaussians");
+	per_gaussian(op, "_opacity", P, 1, nullptr);
+	const torch::Tensor sc = per_gaussian(scaling, "_scaling", P, 3, &op), f = per_gaussian(filter_3D, "filter_3D", P, 1, &op);
+	const c10::cuda::CUDAGuard guard(op.device());
+	torch::Tensor out = new_empty({P, 1}, op.options());
+	check(rgs_reset_opacity((int)P, sc.data_ptr<float>(), op.data_ptr<float>(), f.data_ptr<float>(), out.data_ptr<float>(),
+	                        at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
 // simple_knn's distCUDA2 (reference scene/gaussian_model.py:315-316): points [P,3] float32 on a CUDA device -> [P] float32,
 // the mean squared distance to the 3 nearest other points (rgs_knn_mean_dist2).  Non-contiguous input is accepted.
 torch::Tensor KnnMeanDist2(const torch::Tensor& points) {
@@ -1225,6 +1346,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("activate_forward", &ActivateForward);
 	m.def("activate_backward", &ActivateBackward);
 	m.def("densification_stats", &DensificationStats);
+	// densify-and-prune: one private submodule, called by rade_gs_b200.densify (the stages are not a public API of their own)
+	py::module_ d = m.def_submodule("_densify", "densify-and-prune stages behind rade_gs_b200.densify");
+	d.def("select", &DensifySelect, py::arg("grad_accum"), py::arg("grad_accum_abs"), py::arg("denom"), py::arg("scaling"), py::arg("opacity"),
+	      py::arg("max_grad"), py::arg("dense"), py::arg("min_opacity"), py::arg("prune_large"), py::arg("max_screen_size"), py::arg("world"));
+	d.def("plan", &DensifyPlan, py::arg("flags"), py::arg("block_offsets"), py::arg("counts"), py::arg("scaling"));
+	d.def("gather", &DensifyGather, py::arg("src"), py::arg("draw"), py::arg("C"), py::arg("xyz"), py::arg("rotation"), py::arg("scaling"),
+	      py::arg("sample_clone"), py::arg("sample_split"), py::arg("columns"));
+	d.def("reset_opacity", &ResetOpacity, py::arg("scaling"), py::arg("opacity"), py::arg("filter_3D"));
 	m.def("knn_mean_dist2", &KnnMeanDist2, py::arg("points"));
 	m.def("tsdf_touch", &TsdfTouch);
 	m.def("tsdf_integrate", &TsdfIntegrate);
