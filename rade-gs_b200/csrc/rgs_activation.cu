@@ -59,20 +59,18 @@ __global__ void __launch_bounds__(256) activate_backward_kernel(int P, const flo
 	const float go = g_opacity[i];
 	// opacity_out = o * coef
 	d_raw_opacity[i] = go * coef * o * (1.0f - o);
-	const float d_coef = go * o;
-	// coef = sqrt(q), q = det1 / det2   (autograd: sqrt -> g / (2 result); div -> g / b, -g a / b^2)
-	const float d_q = d_coef / (2.0f * coef);
-	const float d_det1 = d_q / det2;
-	const float d_det2 = -d_q * det1 / (det2 * det2);
+	// coef = sqrt(prod_j sq_j / after_j) with after_j = sq_j + f^2 and sq_j = exp(2 raw_j), so
+	//   d coef / d raw_k = coef * (1 - sq_k / after_k) = coef * f^2 / after_k.
+	// Autograd's chain through det1 and det2 subtracts two terms of size d_coef * coef that nearly cancel, and its
+	// -d_q * det1 / det2^2 underflows: det2 >= f^6 reaches 1e-24 at f = 1e-4, and det2 * det2 leaves the fp32 range.
+	// This form has no quotient by det2^2 and no cancellation: every factor is a product of positive terms.
+	const float d_coef_f2 = go * o * coef * f2;
 #pragma unroll
 	for (int k = 0; k < 3; k++) {
 		const float scale_out = sqrtf(after[k]);
-		// after_k feeds det2 (product of the three) and scales_out_k = sqrt(after_k)
-		const float d_after = d_det2 * (after[(k + 1) % 3] * after[(k + 2) % 3]) + g_scales[3 * i + k] / (2.0f * scale_out);
-		// sq_k feeds det1 and after_k
-		const float d_sq = d_det1 * (sq[(k + 1) % 3] * sq[(k + 2) % 3]) + d_after;
-		// sq = s^2, s = exp(raw)
-		d_raw_scaling[3 * i + k] = d_sq * 2.0f * s[k] * s[k];
+		// scales_out_k = sqrt(after_k): d / d raw_k = g / (2 scale_out) * 2 s^2
+		const float d_scale = g_scales[3 * i + k] / (2.0f * scale_out) * 2.0f * s[k] * s[k];
+		d_raw_scaling[3 * i + k] = d_coef_f2 / after[k] + d_scale;
 	}
 	const float4 r = *reinterpret_cast<const float4*>(raw_rotation + 4 * i);
 	const float4 g = *reinterpret_cast<const float4*>(g_rotations + 4 * i);
