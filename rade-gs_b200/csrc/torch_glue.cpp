@@ -992,7 +992,7 @@ std::tuple<int64_t, torch::Tensor, int64_t> TsdfTouch(const py::object& grid, co
 	const torch::Tensor d = arg(depth, "depth", torch::kFloat32, {-1, -1}, "[H, W]", &keys, REJECT);
 	const rgs_tsdf_grid g = tsdf_grid(grid);
 	const rgs_tsdf_camera c = tsdf_camera(d, intrinsic, extrinsic, depth_scale, depth_max, trunc_voxel_multiplier);
-	torch::Tensor out = torch::empty({g.frame_slots / 2, 3}, keys.options().dtype(torch::kInt32)), scratch = bytes(keys);
+	torch::Tensor out = new_empty({g.frame_slots / 2, 3}, keys.options().dtype(torch::kInt32)), scratch = bytes(keys);
 	int64_t allocated = 0;
 	const int64_t n = rgs_tsdf_touch(&g, &c, d.data_ptr<float>(), out.data_ptr<int32_t>(), &allocated, resize_cb, &scratch,
 	                                 at::cuda::getCurrentCUDAStream().stream());
@@ -1033,7 +1033,7 @@ std::tuple<torch::Tensor, torch::Tensor> TsdfActiveBlocks(const py::object& grid
 	const torch::Tensor hk = grid_array(grid, "hash_keys", torch::kInt64);
 	const c10::cuda::CUDAGuard guard(hk.device());
 	const rgs_tsdf_grid g = tsdf_grid(grid);
-	torch::Tensor keys = torch::empty({g.capacity}, hk.options()), pools = torch::empty({g.capacity}, hk.options().dtype(torch::kInt32)), scratch = bytes(hk);
+	torch::Tensor keys = new_empty({g.capacity}, hk.options()), pools = new_empty({g.capacity}, hk.options().dtype(torch::kInt32)), scratch = bytes(hk);
 	const int64_t n = rgs_tsdf_active_blocks(&g, reinterpret_cast<uint64_t*>(keys.data_ptr<int64_t>()), pools.data_ptr<int32_t>(), resize_cb, &scratch,
 	                                         at::cuda::getCurrentCUDAStream().stream());
 	check(n);
