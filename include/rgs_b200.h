@@ -642,6 +642,63 @@ typedef struct rgs_tetra_filter_out {
 int32_t rgs_tetra_filter(int64_t M, const float* points, const float* ends, const float* end_scales, int64_t F, const int64_t* faces, rgs_resize_fn resize,
                          rgs_tetra_filter_out* out, void* cuda_stream);
 
+/* ---- Delaunay tetrahedralization of the tetra points (mesh_extract_tetrahedra.py:63, cpp.triangulate) ----
+ *
+ * rgs_delaunay: points fp32 [N, 3] on the device -> int32 cells [T, 4] through resize(out->cells_user), the Delaunay
+ * tetrahedralization of the distinct points.
+ *
+ * Predicates (exact on the fp64 values of the fp32 inputs).
+ *   orient3d(a, b, c, d) = sign det[b - a, c - a, d - a]; a cell is positive when it is > 0.
+ *   insphere(a, b, c, d, e) = -sign D5, D5 = det of the rows (x, y, z, x^2 + y^2 + z^2, 1) of a, b, c, d, e: for a
+ *   positive a, b, c, d it is > 0 exactly when e lies strictly inside their circumsphere ("in conflict").
+ *   Both run Shewchuk's stage-A floating-point filter first (bound (7 + 56 eps) eps, resp. (16 + 224 eps) eps, times the
+ *   permanent, plus 2^-600 for underflowed products; eps = 2^-53; the file is compiled without FMA contraction).  When the
+ *   filter cannot decide, the determinant is summed exactly over its monomials as a fixed-point integer: any finite fp32
+ *   coordinates are in range there, and the filter neither overflows nor underflows beyond its slack for coordinates up
+ *   to 2^128.  rgs_delaunay's own limit is |coordinate| <= 2^90, so that the ghosts below stay finite fp32 values.
+ *   Perturbed insphere (Devillers & Teillaud 2011, the scheme of CGAL's Delaunay_triangulation_3): when insphere is 0, the
+ *   five points are ranked by lexicographic (x, y, z) order and, from the largest down, the first non-zero
+ *   -(-1)^i orient3d(the four points other than point i, in order) is the sign (i = 0..4 the position in (a, b, c, d, e)).
+ *   The ranking depends on the coordinates only, so the cells depend on the point set, not on the input order.
+ * Duplicates.  Numerically equal points (-0.0 == 0.0) count as one, represented by their smallest index; the other copies
+ *   appear in no cell.
+ * Ghosts.  With lo, hi the bounding box of the input, c = (lo + hi) / 2, R the smallest power of two >= max(hi - lo)
+ *   (at least 2^-100) and S = D R, D = 2^30, four ghost vertices g = fl32(c + S s) for s = (1,1,1), (1,-1,-1), (-1,1,-1),
+ *   (-1,-1,1) bound the points and take part in the perturbation like any point (they rank by their coordinates).  The
+ *   output is every cell of Del(P u G) without a ghost vertex; each is a Delaunay cell of P.  The one difference from
+ *   Del(P): a hull cell of P whose circumsphere contains a ghost is missing (only near-flat hull slivers have such spheres).
+ * Output.  Every cell is positive; each row is rotated by an even permutation so that its smallest index comes first and
+ *   the smallest of the other three second; rows are sorted lexicographically.  The bits do not depend on scheduling.
+ *   Fewer than 4 distinct points, or coplanar points, give T = 0 (scipy raises instead).
+ * Limits.  0 <= N <= RGS_DELAUNAY_MAX_POINTS; more than 2^29 cells (a face is referenced as cell << 2 | face in an int32)
+ *   return RGS_E_CAPACITY.  A coordinate that is not finite or exceeds 2^90 in magnitude returns RGS_E_INVALID.  A new cell
+ *   that is not positive, or a point that finds no cell, is a predicate bug: RGS_E_CUDA with a message, never a cell.
+ * Memory (through resize, one user pointer each): points_user about 64 bytes per point plus the sorts' workspace;
+ *   mesh_user[0] and [1] (the mesh, 56 bytes per cell, starting at 8 N + 64 cells and doubling into the other buffer when
+ *   full); slab_user about 2.8 KB per nominee slot, K = min(N, 2^19) slots of 64 cells and 128 faces.  The cavities that
+ *   overflow a round's slot are inserted right after it through the same claims in max(1, K / 16) slots 16 times as
+ *   large; one larger still is inserted alone with the whole slab area, doubled until it fits.  sort_user about 40 bytes
+ *   per cell.  Host reads: 3, plus one per round, one per large-slot pass and two per lone cavity.  Statistics: rounds;
+ *   the largest cavity inserted through a slot; overflowed = the round slots that overflowed, summed over rounds (a point
+ *   counts once per round it overflows in); alone = the cavities inserted alone; the mesh growths.  Building a star
+ *   links its cells in O(b^2) steps of one thread for b boundary faces. */
+#define RGS_DELAUNAY_MAX_POINTS (1 << 26)
+typedef struct rgs_delaunay_out {
+	void* cells_user;
+	void* points_user;
+	void* mesh_user[2];
+	void* slab_user;
+	void* sort_user;
+	int64_t num_cells;
+	int32_t rounds, max_cavity, overflowed, alone, mesh_growths;
+} rgs_delaunay_out;
+int32_t rgs_delaunay(int64_t N, const float* points, rgs_resize_fn resize, rgs_delaunay_out* out, void* cuda_stream);
+/* The predicates above, by the same device code, on M index tuples [M, 5] (a, b, c, d, e) into points fp32 [N, 3]:
+ * signs int8 [M, 3] = (orient3d(a, b, c, d), insphere(a, b, c, d, e), perturbed insphere).  An index outside [0, N) or a
+ * coordinate that is not finite returns RGS_E_INVALID.  4 bytes of scratch through resize; one host read. */
+int32_t rgs_delaunay_predicates(int64_t N, const float* points, int64_t M, const int32_t* tuples, int8_t* signs, rgs_resize_fn resize,
+                                void* scratch_user, void* cuda_stream);
+
 /* ---- densify-and-prune and opacity reset (reference scene/gaussian_model.py:495-513 reset_opacity, :662-741 densify_and_prune) ----
  * Inputs per Gaussian (fp32, device): grad_accum, grad_accum_abs, denom [P] (the [P,1] statistics), raw scaling [P,3], raw
  * opacity [P], rotation [P,4], xyz [P,3]; 0 < P < 2^31.

@@ -935,6 +935,144 @@ int32_t rgs_tetra_filter(int64_t M, const float* points, const float* ends, cons
 	return RGS_OK;
 }
 
+// ---- Delaunay tetrahedralization (rgs_delaunay.cu) ----
+
+int32_t rgs_delaunay(int64_t N, const float* points, rgs_resize_fn resize, rgs_delaunay_out* out, void* cuda_stream) {
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	out->num_cells = 0;
+	out->rounds = out->max_cavity = out->overflowed = out->alone = out->mesh_growths = 0;
+	if (N < 0 || N > RGS_DELAUNAY_MAX_POINTS) return fail(RGS_E_INVALID, "delaunay: point count out of range (at most 2^26)");
+	if (N > 0 && !points) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	constexpr int64_t MAX_CELLS = (int64_t)1 << 29;
+	int rc;
+	char* cells_out = nullptr;
+	if (N == 0) return grow(resize, out->cells_user, 0, cells_out, "delaunay");
+
+	size_t bytes = 0;
+	char* pbuf = nullptr;
+	carve_dt_points(nullptr, (int)N, &bytes);
+	if ((rc = grow(resize, out->points_user, bytes, pbuf, "delaunay scratch")) != RGS_OK) return rc;
+	const DtPointsView v = carve_dt_points(pbuf, (int)N, nullptr);
+	DtCounters h;
+	if ((rc = cuda_status(launch_dt_prepare((int)N, points, v, &h, s), "delaunay")) != RGS_OK) return rc;
+	if (h.bad) return fail(RGS_E_INVALID, "delaunay: a coordinate is not finite or exceeds 2^90 in magnitude");
+	const int n = (int)h.unique;
+	if (n < 4) return grow(resize, out->cells_user, 0, cells_out, "delaunay");
+
+	int cur = 0;
+	int64_t cap = std::min<int64_t>(8 * (int64_t)n + 64, MAX_CELLS);
+	char* mbuf = nullptr;
+	carve_dt_mesh(nullptr, cap, &bytes);
+	if ((rc = grow(resize, out->mesh_user[0], bytes, mbuf, "delaunay mesh")) != RGS_OK) return rc;
+	DtMesh m = carve_dt_mesh(mbuf, cap, nullptr);
+	if ((rc = cuda_status(launch_dt_init((int)N, points, n, v, h, m, cap, s), "delaunay")) != RGS_OK) return rc;
+
+	const int K = std::min(DT_MAX_SLOTS, n);
+	int64_t cc_total = (int64_t)K * DT_SLOT_CELLS, cb_total = (int64_t)K * DT_SLOT_FACES;
+	DtSlots sl;
+	auto slabs = [&]() -> int {
+		char* buf = nullptr;
+		carve_dt_slots(nullptr, K, cc_total, cb_total, &bytes);
+		const int r = grow(resize, out->slab_user, bytes, buf, "delaunay slabs");
+		sl = carve_dt_slots(buf, K, cc_total, cb_total, nullptr);
+		return r;
+	};
+	// the mesh moves into the other buffer at (at least) twice the size; dead rows fill the new tail
+	auto grow_mesh = [&](int64_t want) -> int {
+		const int64_t nc = std::min(std::max(2 * cap, want), MAX_CELLS);
+		if (nc < want || nc <= cap) return fail(RGS_E_CAPACITY, "delaunay: the mesh needs more than 2^29 cells");
+		char* buf = nullptr;
+		carve_dt_mesh(nullptr, nc, &bytes);
+		if (const int r = grow(resize, out->mesh_user[1 - cur], bytes, buf, "delaunay mesh")) return r;
+		const DtMesh nm = carve_dt_mesh(buf, nc, nullptr);
+		if (const int r = cuda_status(launch_dt_grow_mesh(m, cap, nm, nc, s), "delaunay")) return r;
+		m = nm;
+		cap = nc;
+		cur = 1 - cur;
+		out->mesh_growths++;
+		return RGS_OK;
+	};
+	auto checked = [&](const DtCounters& c) -> int {
+		return c.violation ? fail(RGS_E_CUDA, "delaunay: a new cell is not positively oriented or a point found no cell (predicate bug)") : RGS_OK;
+	};
+	if ((rc = slabs()) != RGS_OK) return rc;
+
+	// Every pass can leave the device's cell counter above the capacity (a winner that found no room has added its cells
+	// already); the mesh then grows to at least twice that count, so `cells`, the extent the next pass initialises and
+	// scans, is the device's count.
+	int epoch = 0, cells = 1;
+	auto after_pass = [&]() -> int {
+		if (const int r = checked(h)) return r;
+		if (h.full)
+			if (const int r = grow_mesh(2 * (int64_t)h.cells)) return r;
+		cells = (int)std::min<int64_t>(h.cells, cap);
+		return RGS_OK;
+	};
+	// the cavities too large for a round's slot go in right after it, several at once, in slots 16 times as large
+	const int KL = std::max(1, K / 16);
+	while ((int)h.inserted < n) {
+		out->rounds++;
+		if ((rc = cuda_status(launch_dt_round(n, v, m, sl, K, DT_SLOT_CELLS, DT_SLOT_FACES, ++epoch, cap, cells, s), "delaunay")) != RGS_OK ||
+		    (rc = cuda_status(launch_dt_read(v, &h, s), "delaunay")) != RGS_OK || (rc = after_pass()) != RGS_OK)
+			return rc;
+		if (h.overflowed == 0) continue;
+		out->overflowed += h.overflowed;
+		if ((rc = cuda_status(launch_dt_large(n, v, m, sl, KL, (int)(cc_total / KL), (int)(cb_total / KL), ++epoch, cap, cells, s), "delaunay")) != RGS_OK ||
+		    (rc = cuda_status(launch_dt_read(v, &h, s), "delaunay")) != RGS_OK || (rc = after_pass()) != RGS_OK)
+			return rc;
+		// one still larger: the smallest such point goes in alone, with the whole slab area (grown as needed)
+		while (h.overflowed > 0) {
+			if ((rc = cuda_status(launch_dt_single_cavity(v, m, sl, cc_total, cb_total, cells, s), "delaunay")) != RGS_OK ||
+			    (rc = cuda_status(launch_dt_read(v, &h, s), "delaunay")) != RGS_OK)
+				return rc;
+			if (h.overflowed) {
+				cc_total *= 2;
+				cb_total *= 2;
+				if (cc_total > MAX_CELLS) return fail(RGS_E_CAPACITY, "delaunay: a cavity exceeds 2^29 cells");
+				if ((rc = slabs()) != RGS_OK) return rc;
+				continue;
+			}
+			if ((rc = cuda_status(launch_dt_single_star(n, v, m, sl, cc_total, cb_total, ++epoch, cap, s), "delaunay")) != RGS_OK ||
+			    (rc = cuda_status(launch_dt_read(v, &h, s), "delaunay")) != RGS_OK || (rc = after_pass()) != RGS_OK)
+				return rc;
+			if (!h.full) {
+				out->alone++;
+				break;
+			}
+			h.overflowed = 1;
+		}
+	}
+	out->max_cavity = h.max_cavity;
+
+	char* sbuf = nullptr;
+	int T = 0;
+	if ((rc = grow(resize, out->sort_user, dt_sort_bytes(cells), sbuf, "delaunay sort")) != RGS_OK ||
+	    (rc = cuda_status(launch_dt_emit(n, v, m, sbuf, cells, &T, s), "delaunay")) != RGS_OK ||
+	    (rc = grow(resize, out->cells_user, (size_t)T * 4 * sizeof(int32_t), cells_out, "delaunay")) != RGS_OK ||
+	    (rc = cuda_status(launch_dt_sort(sbuf, cells, T, reinterpret_cast<int4*>(cells_out), s), "delaunay")) != RGS_OK)
+		return rc;
+	out->num_cells = T;
+	return RGS_OK;
+}
+
+int32_t rgs_delaunay_predicates(int64_t N, const float* points, int64_t M, const int32_t* tuples, int8_t* signs, rgs_resize_fn resize,
+                                void* scratch_user, void* cuda_stream) {
+	if (N < 0 || N > INT32_MAX || M < 0 || M > INT32_MAX) return fail(RGS_E_INVALID, "delaunay predicates: count out of range");
+	if (M == 0) return RGS_OK;
+	if (!resize || !points || !tuples || !signs) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = nullptr;
+	int bad = 0;
+	int rc;
+	if ((rc = grow(resize, scratch_user, sizeof(int), buf, "delaunay predicates scratch")) != RGS_OK ||
+	    (rc = cuda_status(launch_dt_predicates((int)N, points, (int)M, tuples, signs, reinterpret_cast<int*>(buf), &bad, (cudaStream_t)cuda_stream),
+	                      "delaunay predicates")) != RGS_OK)
+		return rc;
+	if (bad == 1) return fail(RGS_E_INVALID, "delaunay predicates: an index lies outside [0, N)");
+	if (bad) return fail(RGS_E_INVALID, "delaunay predicates: a coordinate is not finite");
+	return RGS_OK;
+}
+
 int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt, float* dmaps,
                                  double* sums, void* cuda_stream) {
 	if (planes < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");

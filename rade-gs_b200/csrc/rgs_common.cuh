@@ -362,6 +362,71 @@ size_t tetra_filter_scratch_bytes(int M, int64_t F);
 cudaError_t launch_tetra_filter(int M, const float* points, const float* ends, const float* end_scl, int64_t F, const int64_t* faces, char* scratch,
                                 float* out_vertices, int64_t* out_faces, int64_t* num_vertices, int64_t* num_faces, int32_t* bad, cudaStream_t s);
 
+// Delaunay tetrahedralization (rgs_delaunay.cu; contract in include/rgs_b200.h).  rgs_api.cu drives the rounds and owns
+// every allocation; argument checks are its job.
+constexpr float DT_MAX_COORD = 0x1p90f;     // |coordinate| bound of rgs_delaunay's input
+constexpr double DT_GHOST_SCALE = 0x1p30;   // D: ghost distance in units of the box's power-of-two extent
+constexpr int DT_SLOT_CELLS = 64;           // per-nominee cavity capacity of a round ...
+constexpr int DT_SLOT_FACES = 128;          // ... and its boundary-face capacity
+constexpr int DT_MAX_SLOTS = 1 << 19;       // nominees per round
+
+struct DtCounters {
+	int bad;                 // points out of range or not finite
+	uint32_t box[6];         // ordered-int bounding box (lo xyz, hi xyz)
+	int cells;               // cells in use (dead ones included)
+	int slots;               // nominees this round
+	int full;                // a winner found no room to append: grow the mesh
+	int overflowed;          // cavities larger than their slot in this pass
+	int overflow_point;      // the smallest of their points
+	int violation;           // a new cell was not positive, or a point found no cell: a predicate bug
+	int inserted;            // points inserted so far
+	int max_cavity;          // largest cavity inserted through a slot
+	int out_cells;           // cells emitted
+	uint32_t unique, spare;  // host side only: distinct points
+};
+struct DtPointsView {
+	DtCounters* cnt;
+	float4* verts;           // [n + 4] representatives in Morton order, then the ghosts
+	uint32_t* rep;           // [n] original index of each vertex
+	int32_t* loc;            // [n] located cell, -1 once inserted
+	uint64_t* key64[2];
+	uint32_t *key32[2], *ids[2], *first, *rank;   // first: after preparation, the round's overflowed points
+	char* temp;
+	size_t temp_bytes;
+};
+struct DtMesh {
+	int4* tet;               // [cap] vertices, positive; -1 rows are dead
+	int4* adj;               // [cap] neighbour across the face opposite vertex k: cell << 2 | face, -1 for none
+	uint64_t* claim;         // [cap] (priority << 32 | slot) of the round
+	uint64_t* nom;           // [cap] nominee of the round: (hash << 32 | point)
+	int2* died;              // [cap] (pass, slot) that removed the cell
+	int32_t* loc;            // the points' located cells (set by the launchers)
+};
+struct DtSlots {
+	int *point, *cell, *k, *b, *base, *won;   // [K]
+	int* cav;                // [K * DT_SLOT_CELLS] cavity cells
+	int4* bnd;               // [K * DT_SLOT_FACES] the new cell of each boundary face
+	int* bout;               // [K * DT_SLOT_FACES] the outside neighbour of each boundary face
+};
+DtPointsView carve_dt_points(char* base, int N, size_t* total);
+DtMesh carve_dt_mesh(char* base, int64_t cap, size_t* total);
+DtSlots carve_dt_slots(char* base, int K, int64_t cc_total, int64_t cb_total, size_t* total);
+size_t dt_sort_bytes(int64_t cells);
+cudaError_t launch_dt_prepare(int N, const float* pts, const DtPointsView& v, DtCounters* host, cudaStream_t s);
+cudaError_t launch_dt_init(int N, const float* pts, int n, const DtPointsView& v, const DtCounters& host, const DtMesh& m, int64_t cap, cudaStream_t s);
+cudaError_t launch_dt_round(int n, const DtPointsView& v, const DtMesh& m, const DtSlots& sl, int K, int cc, int cb, int epoch, int64_t cap, int cells,
+                            cudaStream_t s);
+cudaError_t launch_dt_large(int n, const DtPointsView& v, const DtMesh& m, const DtSlots& sl, int K, int cc, int cb, int epoch, int64_t cap, int cells,
+                            cudaStream_t s);
+cudaError_t launch_dt_single_cavity(const DtPointsView& v, const DtMesh& m, const DtSlots& sl, int64_t cc_total, int64_t cb_total, int cells, cudaStream_t s);
+cudaError_t launch_dt_single_star(int n, const DtPointsView& v, const DtMesh& m, const DtSlots& sl, int64_t cc_total, int64_t cb_total, int epoch, int64_t cap,
+                                  cudaStream_t s);
+cudaError_t launch_dt_read(const DtPointsView& v, DtCounters* host, cudaStream_t s);
+cudaError_t launch_dt_grow_mesh(const DtMesh& from, int64_t from_cap, const DtMesh& to, int64_t to_cap, cudaStream_t s);
+cudaError_t launch_dt_emit(int n, const DtPointsView& v, const DtMesh& m, char* sort, int64_t cells, int* T, cudaStream_t s);
+cudaError_t launch_dt_sort(char* sort, int64_t cells, int T, int4* out, cudaStream_t s);
+cudaError_t launch_dt_predicates(int N, const float* pts, int M, const int32_t* tuples, int8_t* signs, int* bad_dev, int* bad_host, cudaStream_t s);
+
 // fused image-side losses (rgs_image_loss.cu; SURVEY.md 8f row 2)
 void launch_ssim_l1_forward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, float* dmaps, double* sums,
                             cudaStream_t s);

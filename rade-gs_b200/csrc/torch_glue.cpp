@@ -1270,6 +1270,32 @@ std::tuple<torch::Tensor, torch::Tensor> TetraFilter(const torch::Tensor& points
 	return std::make_tuple(rows(verts, torch::kFloat32, out.num_vertices, {3}), rows(fout, torch::kInt64, out.num_faces, {3}));
 }
 
+// points f32 [N,3] -> (cells int32 [T,4], statistics {rounds, max_cavity, overflowed, alone, mesh_growths})
+std::tuple<torch::Tensor, py::dict> DelaunayTriangulate(const torch::Tensor& points) {
+	const torch::Tensor p = arg(points, "points", torch::kFloat32, {-1, 3}, "[N, 3]");
+	const c10::cuda::CUDAGuard guard(p.device());
+	torch::Tensor cells = bytes(p), pts = bytes(p), mesh0 = bytes(p), mesh1 = bytes(p), slab = bytes(p), sort = bytes(p);
+	rgs_delaunay_out out{&cells, &pts, {&mesh0, &mesh1}, &slab, &sort, 0, 0, 0, 0, 0, 0};
+	check(rgs_delaunay(p.size(0), p.data_ptr<float>(), resize_cb, &out, at::cuda::getCurrentCUDAStream().stream()));
+	py::dict st;
+	st["rounds"] = out.rounds;
+	st["max_cavity"] = out.max_cavity;
+	st["overflowed"] = out.overflowed;
+	st["alone"] = out.alone;
+	st["mesh_growths"] = out.mesh_growths;
+	return std::make_tuple(rows(cells, torch::kInt32, out.num_cells, {4}), st);
+}
+
+// points f32 [N,3], tuples int32 [M,5] -> int8 [M,3] (orient3d, insphere, perturbed insphere)
+torch::Tensor DelaunayPredicates(const torch::Tensor& points, const torch::Tensor& tuples) {
+	const torch::Tensor p = arg(points, "points", torch::kFloat32, {-1, 3}, "[N, 3]"), t = arg(tuples, "tuples", torch::kInt32, {-1, 5}, "[M, 5]", &p);
+	const c10::cuda::CUDAGuard guard(p.device());
+	torch::Tensor signs = new_empty({t.size(0), 3}, p.options().dtype(torch::kInt8)), scratch = bytes(p);
+	check(rgs_delaunay_predicates(p.size(0), p.data_ptr<float>(), t.size(0), t.data_ptr<int32_t>(), signs.data_ptr<int8_t>(), resize_cb, &scratch,
+	                              at::cuda::getCurrentCUDAStream().stream()));
+	return signs;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1376,6 +1402,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("tetra_marching", &TetraMarching, py::arg("vertices"), py::arg("sdf"), py::arg("scales"), py::arg("tets"));
 	m.def("tetra_bisect", &TetraBisect, py::arg("mid_sdf"), py::arg("left"), py::arg("right"), py::arg("left_sdf"), py::arg("right_sdf"), py::arg("mid"));
 	m.def("tetra_filter", &TetraFilter, py::arg("points"), py::arg("ends"), py::arg("end_scales"), py::arg("faces"));
+	// exact Delaunay of the tetra points: a private submodule behind rade_gs_b200.tetra.delaunay
+	py::module_ dt = m.def_submodule("_delaunay", "exact Delaunay tetrahedralization behind rade_gs_b200.tetra.delaunay");
+	dt.def("triangulate", &DelaunayTriangulate, py::arg("points"));
+	dt.def("predicates", &DelaunayPredicates, py::arg("points"), py::arg("tuples"));
 	m.def("grad_stride",[](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });

@@ -4,7 +4,7 @@
 The pieces keep the reference's names and shapes::
 
     points, scales = tetra_points(gaussians.get_xyz, gaussians.get_scaling_with_3D_filter, gaussians._rotation)
-    cells = triangulate(points)                                   # host Delaunay
+    cells = delaunay(points)                                      # exact Delaunay on the GPU
     def evaluate_sdf(pts):                                        # evaluage_cull_alpha: the caller's loop over views
         cull = CullSDF(pts.shape[0], pts.device)
         for view in views:
@@ -19,8 +19,12 @@ The arithmetic of the cull SDF, marching tetrahedra, the bisection and the filte
 
 Deliberate differences from the reference:
 
-* ``triangulate`` falls back to ``scipy.spatial.Delaunay`` when the reference's CGAL binding (tetranerf) is not installed;
-  where points are cospherical the two may return different cells.
+* ``delaunay`` replaces the reference's ``cpp.triangulate`` on the GPU: exact predicates with the symbolic perturbation
+  CGAL uses, so the cells are unique and positively oriented (bit-equality with CGAL is not claimed).  It differs from
+  Del(points) only by the rare near-flat hull cells whose circumsphere reaches its bounding ghost vertices, and it
+  returns no cells for fewer than 4 distinct or coplanar points (scipy raises).
+* ``triangulate`` (host points) falls back to ``scipy.spatial.Delaunay`` when the reference's CGAL binding (tetranerf) is
+  not installed; where points are cospherical the two may return different cells, and scipy mixes orientations.
 * ``marching_tetrahedra`` runs on the GPU in one pass at any size (the reference moves it to the CPU and, above 2^25 tets,
   loops over chunks); the vertices and the face order are the reference's, chunked order included.
 * ``extract_mesh`` returns at once, without evaluating the SDF again, when the surface is empty.
@@ -48,6 +52,15 @@ def tetra_points(xyz: torch.Tensor, scaling_with_3D_filter: torch.Tensor, rotati
     ``trimesh.creation.box()`` order), then the P centres: ``points`` f32 [9P, 3]; ``scales`` f32 [9P, 1] = max(3s).
     ``rotation`` is the raw quaternion (``GaussianModel._rotation``); it is normalised here."""
     return _C.tetra_points(_f32(xyz, "xyz"), _f32(scaling_with_3D_filter, "scaling_with_3D_filter"), _f32(rotation, "rotation"))
+
+
+def delaunay(points: torch.Tensor, return_stats: bool = False):
+    """Exact Delaunay tetrahedralisation of ``points`` f32 [N, 3] on their CUDA device: int32 [T, 4] cells, every one
+    positively oriented, rows canonical and sorted (contract at ``rgs_delaunay`` in include/rgs_b200.h).  Equal points
+    count once (the smallest index represents them); fewer than 4 distinct or coplanar points give no cells.  With
+    ``return_stats``, also a dict of the rounds, the largest cavity, the overflowed cavities and the mesh growths."""
+    cells, stats = _C._delaunay.triangulate(_f32(points, "points"))
+    return (cells, stats) if return_stats else cells
 
 
 def triangulate(points) -> torch.Tensor:
