@@ -699,6 +699,40 @@ int32_t rgs_delaunay(int64_t N, const float* points, rgs_resize_fn resize, rgs_d
 int32_t rgs_delaunay_predicates(int64_t N, const float* points, int64_t M, const int32_t* tuples, int8_t* signs, rgs_resize_fn resize,
                                 void* scratch_user, void* cuda_stream);
 
+/* ---- LPIPS v0.1 with the VGG16 trunk (metric.py:74, lpipsPyTorch's LPIPS('vgg')) ----
+ *
+ * The two images of one pair go through together: every activation is fp32 NHWC [2, H, W, C], image x first.  The
+ * stages, in the order a caller runs them: input conv, then per block its 3x3 convs, the distance of the block's last
+ * ReLU (relu1_2, relu2_2, relu3_3, relu4_3, relu5_3) and, except after block 5, the max-pool.
+ *
+ * rgs_lpips_input_conv (conv1_1, fp32 SIMT): x, y fp32 CHW [3, H, W], H >= 16 and W >= 16 (the reference fails below 16
+ *   inside its fourth pool), H * W <= 2^28.  z = (v - mean_c) / std_c in fp32 with mean = (-.030, -.088, -.188) and
+ *   std = (.458, .448, .450) as fp32 constants, applied to the [0, 1] values as given (lpipsPyTorch does not rescale to
+ *   [-1, 1]); zero padding of z; weight fp32 [64][3][3][3] (torch's layout), bias [64]; per output
+ *   acc = fma chain over (c, ky, kx) in that order from 0, then relu(acc + bias) rounded to TF32 -> out [2, H, W, 64].
+ * rgs_lpips_conv3x3 (TF32 tensor cores): in [2, H, W, C_in], weight [C_out][3][3][C_in] (torch's [C_out][C_in][3][3]
+ *   repacked), bias [C_out], C_in % 32 == 0, C_out % 64 == 0, both <= 512 -> out [2, H, W, C_out] = relu(conv + bias)
+ *   rounded to TF32 with cvt.rna (nearest, ties away from zero).  The products run on wgmma.mma_async .tf32, which reads
+ *   the top 19 bits of each operand and ignores the low 13: operands that are not TF32 values are truncated.  Every
+ *   activation this file writes is a TF32 value, and rade_gs_b200.metrics rounds the weights with cvt.rna's rule when it
+ *   loads them, so in the full trunk no operand bit is dropped; the error is the fp32 accumulation of K = 9 C_in
+ *   products in the tensor cores' order, the bias addition and the output rounding (2^-11 relative).
+ * rgs_lpips_maxpool: 2x2, stride 2, floor: in [2, H, W, C] -> out [2, H / 2, W / 2, C], C % 4 == 0; torch.max_pool2d's
+ *   rule (window scanned row by row, a value replaces the maximum when greater or NaN), so results are bit-equal to it.
+ * rgs_lpips_distance: feats [2, H, W, C], C in {64, 128, 256, 512}, lin fp32 [C] (the layer's 1x1 head).  Per pixel,
+ *   fp32: n = sqrt(sum_c f^2) + 1e-10 for each image, map = sum_c lin_c (fx / nx - fy / ny)^2 -> map [H, W].  mean (one
+ *   fp64 on the device) = (sum of map) / (H W), summed in fp64 in a fixed order: 16 pixels per warp in pixel order, 8 warps
+ *   per CTA in warp order, the CTA sums in a fixed 512-thread tree.  Scratch through resize: 8 bytes per 128 pixels.
+ *   The LPIPS value is the sum of the five layer means.
+ * Every stage is deterministic: the same inputs give the same bits on every run and on every H100.  No stage reads
+ * memory it did not write except its inputs.  An output must not overlap an input. */
+int32_t rgs_lpips_input_conv(int32_t H, int32_t W, const float* x, const float* y, const float* weight, const float* bias, float* out, void* cuda_stream);
+int32_t rgs_lpips_conv3x3(int32_t H, int32_t W, int32_t C_in, int32_t C_out, const float* in, const float* weight, const float* bias, float* out,
+                          void* cuda_stream);
+int32_t rgs_lpips_maxpool(int32_t H, int32_t W, int32_t C, const float* in, float* out, void* cuda_stream);
+int32_t rgs_lpips_distance(int32_t H, int32_t W, int32_t C, const float* feats, const float* lin, float* map, double* mean, rgs_resize_fn resize,
+                           void* scratch_user, void* cuda_stream);
+
 /* ---- densify-and-prune and opacity reset (reference scene/gaussian_model.py:495-513 reset_opacity, :662-741 densify_and_prune) ----
  * Inputs per Gaussian (fp32, device): grad_accum, grad_accum_abs, denom [P] (the [P,1] statistics), raw scaling [P,3], raw
  * opacity [P], rotation [P,4], xyz [P,3]; 0 < P < 2^31.

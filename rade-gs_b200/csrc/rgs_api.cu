@@ -1073,6 +1073,48 @@ int32_t rgs_delaunay_predicates(int64_t N, const float* points, int64_t M, const
 	return RGS_OK;
 }
 
+// the activation sizes every LPIPS stage accepts: [2, H, W, C] with 2 H W C < 2^31 elements
+static int lpips_size(int32_t H, int32_t W, int64_t C, int32_t min_side, const char* what) {
+	if (H < min_side || W < min_side)
+		return fail(RGS_E_INVALID, std::string(what) + ": the image must be at least " + std::to_string(min_side) + " x " + std::to_string(min_side) +
+		                               " pixels, got " + std::to_string(H) + " x " + std::to_string(W));
+	if ((int64_t)H * W * C * 2 > INT32_MAX) return fail(RGS_E_INVALID, std::string(what) + ": the activations exceed 2^31 elements");
+	return RGS_OK;
+}
+
+int32_t rgs_lpips_input_conv(int32_t H, int32_t W, const float* x, const float* y, const float* weight, const float* bias, float* out, void* cuda_stream) {
+	if (const int rc = lpips_size(H, W, 64, 16, "lpips input conv")) return rc;
+	if (!x || !y || !weight || !bias || !out) return fail(RGS_E_INVALID, "null pointer");
+	return cuda_status(launch_lpips_input_conv(H, W, x, y, weight, bias, out, (cudaStream_t)cuda_stream), "lpips input conv");
+}
+
+int32_t rgs_lpips_conv3x3(int32_t H, int32_t W, int32_t C_in, int32_t C_out, const float* in, const float* weight, const float* bias, float* out,
+                          void* cuda_stream) {
+	if (C_in <= 0 || C_in % 32 || C_in > 512 || C_out <= 0 || C_out % 64 || C_out > 512)
+		return fail(RGS_E_INVALID, "lpips conv3x3: C_in must be a multiple of 32 and C_out of 64, both at most 512");
+	if (const int rc = lpips_size(H, W, std::max(C_in, C_out), 1, "lpips conv3x3")) return rc;
+	if (!in || !weight || !bias || !out) return fail(RGS_E_INVALID, "null pointer");
+	return cuda_status(launch_lpips_conv3x3(H, W, C_in, C_out, in, weight, bias, out, (cudaStream_t)cuda_stream), "lpips conv3x3");
+}
+
+int32_t rgs_lpips_maxpool(int32_t H, int32_t W, int32_t C, const float* in, float* out, void* cuda_stream) {
+	if (C <= 0 || C % 4) return fail(RGS_E_INVALID, "lpips maxpool: C must be a positive multiple of 4");
+	if (const int rc = lpips_size(H, W, C, 2, "lpips maxpool")) return rc;
+	if (!in || !out) return fail(RGS_E_INVALID, "null pointer");
+	return cuda_status(launch_lpips_maxpool(H, W, C, in, out, (cudaStream_t)cuda_stream), "lpips maxpool");
+}
+
+int32_t rgs_lpips_distance(int32_t H, int32_t W, int32_t C, const float* feats, const float* lin, float* map, double* mean, rgs_resize_fn resize,
+                           void* scratch_user, void* cuda_stream) {
+	if (C != 64 && C != 128 && C != 256 && C != 512) return fail(RGS_E_INVALID, "lpips distance: C must be 64, 128, 256 or 512");
+	if (const int rc = lpips_size(H, W, C, 1, "lpips distance")) return rc;
+	if (!feats || !lin || !map || !mean || !resize) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = nullptr;
+	if (const int rc = grow(resize, scratch_user, sizeof(double) * lpips_distance_blocks(H * W), buf, "lpips distance scratch")) return rc;
+	return cuda_status(launch_lpips_distance(H * W, C, feats, lin, map, reinterpret_cast<double*>(buf), mean, (cudaStream_t)cuda_stream),
+	                   "lpips distance");
+}
+
 int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt, float* dmaps,
                                  double* sums, void* cuda_stream) {
 	if (planes < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");

@@ -458,4 +458,11 @@ cudaError_t launch_densify_gather(int N, const int* src, const int* draw, int C,
                                   const rgs_densify_column* cols, cudaStream_t s);
 cudaError_t launch_reset_opacity(int P, const float* scaling, const float* opacity, const float* filter_3D, float* out, cudaStream_t s);
 
+// LPIPS-VGG trunk and distance (rgs_lpips.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
+int lpips_distance_blocks(int HW);   // fp64 partial sums the distance of one layer writes
+cudaError_t launch_lpips_input_conv(int H, int W, const float* x, const float* y, const float* weight, const float* bias, float* out, cudaStream_t s);
+cudaError_t launch_lpips_conv3x3(int H, int W, int Cin, int Cout, const float* in, const float* weight, const float* bias, float* out, cudaStream_t s);
+cudaError_t launch_lpips_maxpool(int H, int W, int C, const float* in, float* out, cudaStream_t s);
+cudaError_t launch_lpips_distance(int HW, int C, const float* feats, const float* lin, float* map, double* partial, double* mean, cudaStream_t s);
+
 }  // namespace rgs

@@ -1296,6 +1296,64 @@ torch::Tensor DelaunayPredicates(const torch::Tensor& points, const torch::Tenso
 	return signs;
 }
 
+// ---- LPIPS-VGG stages (rgs_lpips_*; Python side rade_gs_b200.metrics) ------------------------------------------------------
+// Each stage writes its [2, H, W, C] activations into `buffer` (a byte tensor grown through resize_cb, a fresh one when
+// None): rade_gs_b200.metrics alternates two of them, so only two activation maps of the trunk are alive at a time.
+
+torch::Tensor activation_out(const c10::optional<torch::Tensor>& buffer, const torch::Tensor& like, const torch::Tensor& input, int64_t H, int64_t W,
+                             int64_t C) {
+	torch::Tensor b = buffer.has_value() ? *buffer : bytes(like);
+	TORCH_CHECK(b.scalar_type() == torch::kUInt8 && b.dim() == 1 && b.is_contiguous(), "buffer must be a contiguous 1-D uint8 tensor");
+	TORCH_CHECK(b.device() == like.device(), "buffer must be on the same device as the other inputs");
+	TORCH_CHECK(!b.is_alias_of(input), "buffer must not hold the input");
+	resize_cb(&b, (size_t)(2 * H * W * C) * sizeof(float));
+	return rows(b, torch::kFloat32, 2, {H, W, C});
+}
+
+// x, y f32 [3,H,W], weight f32 [64,3,3,3], bias f32 [64] -> f32 [2,H,W,64]
+torch::Tensor LpipsInputConv(const torch::Tensor& x, const torch::Tensor& y, const torch::Tensor& weight, const torch::Tensor& bias,
+                             const c10::optional<torch::Tensor>& buffer) {
+	const torch::Tensor a = arg(x, "x", torch::kFloat32, {3, -1, -1}, "[3, H, W]"), b = arg(y, "y", torch::kFloat32, {3, a.size(1), a.size(2)}, "[3, H, W] like x", &a),
+	                    w = arg(weight, "weight", torch::kFloat32, {64, 3, 3, 3}, "[64, 3, 3, 3]", &a), bs = arg(bias, "bias", torch::kFloat32, {64}, "[64]", &a);
+	const c10::cuda::CUDAGuard guard(a.device());
+	torch::Tensor out = activation_out(buffer, a, a, a.size(1), a.size(2), 64);
+	check(rgs_lpips_input_conv(a.size(1), a.size(2), a.data_ptr<float>(), b.data_ptr<float>(), w.data_ptr<float>(), bs.data_ptr<float>(), out.data_ptr<float>(),
+	                           at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
+// input f32 [2,H,W,C_in], weight f32 [C_out,3,3,C_in] (TF32 values), bias f32 [C_out] -> f32 [2,H,W,C_out]
+torch::Tensor LpipsConv3x3(const torch::Tensor& input, const torch::Tensor& weight, const torch::Tensor& bias, const c10::optional<torch::Tensor>& buffer) {
+	const torch::Tensor in = arg(input, "input", torch::kFloat32, {2, -1, -1, -1}, "[2, H, W, C_in]"),
+	                    w = arg(weight, "weight", torch::kFloat32, {-1, 3, 3, in.size(3)}, "[C_out, 3, 3, C_in]", &in),
+	                    bs = arg(bias, "bias", torch::kFloat32, {w.size(0)}, "[C_out]", &in);
+	const c10::cuda::CUDAGuard guard(in.device());
+	torch::Tensor out = activation_out(buffer, in, input, in.size(1), in.size(2), w.size(0));
+	check(rgs_lpips_conv3x3(in.size(1), in.size(2), in.size(3), w.size(0), in.data_ptr<float>(), w.data_ptr<float>(), bs.data_ptr<float>(), out.data_ptr<float>(),
+	                        at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
+// input f32 [2,H,W,C] -> f32 [2,H/2,W/2,C]
+torch::Tensor LpipsMaxpool(const torch::Tensor& input, const c10::optional<torch::Tensor>& buffer) {
+	const torch::Tensor in = arg(input, "input", torch::kFloat32, {2, -1, -1, -1}, "[2, H, W, C]");
+	const c10::cuda::CUDAGuard guard(in.device());
+	torch::Tensor out = activation_out(buffer, in, input, in.size(1) / 2, in.size(2) / 2, in.size(3));
+	check(rgs_lpips_maxpool(in.size(1), in.size(2), in.size(3), in.data_ptr<float>(), out.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
+// feats f32 [2,H,W,C], lin f32 [C] -> (map f32 [H,W], mean f64 [1])
+std::tuple<torch::Tensor, torch::Tensor> LpipsDistance(const torch::Tensor& feats, const torch::Tensor& lin) {
+	const torch::Tensor f = arg(feats, "feats", torch::kFloat32, {2, -1, -1, -1}, "[2, H, W, C]"),
+	                    l = arg(lin.reshape({-1}), "lin", torch::kFloat32, {f.size(3)}, "C values", &f);
+	const c10::cuda::CUDAGuard guard(f.device());
+	torch::Tensor map = new_empty({f.size(1), f.size(2)}, f.options()), mean = new_empty({1}, f.options().dtype(torch::kFloat64)), scratch = bytes(f);
+	check(rgs_lpips_distance(f.size(1), f.size(2), f.size(3), f.data_ptr<float>(), l.data_ptr<float>(), map.data_ptr<float>(), mean.data_ptr<double>(), resize_cb,
+	                         &scratch, at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(map, mean);
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1406,6 +1464,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	py::module_ dt = m.def_submodule("_delaunay", "exact Delaunay tetrahedralization behind rade_gs_b200.tetra.delaunay");
 	dt.def("triangulate", &DelaunayTriangulate, py::arg("points"));
 	dt.def("predicates", &DelaunayPredicates, py::arg("points"), py::arg("tuples"));
+	// LPIPS-VGG trunk and distance: a private submodule behind rade_gs_b200.metrics.lpips
+	py::module_ lp = m.def_submodule("_lpips", "LPIPS-VGG stages behind rade_gs_b200.metrics.lpips");
+	lp.def("input_conv", &LpipsInputConv, py::arg("x"), py::arg("y"), py::arg("weight"), py::arg("bias"), py::arg("buffer") = py::none());
+	lp.def("conv3x3", &LpipsConv3x3, py::arg("input"), py::arg("weight"), py::arg("bias"), py::arg("buffer") = py::none());
+	lp.def("maxpool", &LpipsMaxpool, py::arg("input"), py::arg("buffer") = py::none());
+	lp.def("distance", &LpipsDistance, py::arg("feats"), py::arg("lin"));
 	m.def("grad_stride",[](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });
