@@ -9,6 +9,8 @@
 //       -- five masked-index torch passes over [P] tensors -- with one pass.
 // Operation order follows the torch expressions; products and sums that torch rounds separately are kept from
 // contracting into FMAs (__fmul_rn / __fadd_rn) so the results match the eager reference to the last bit or two.
+//
+// This file also holds the C-ABI entry points rgs_activate_*, rgs_densification_stats and rgs_compute_3d_filter (include/rgs_b200.h).
 #include "rgs_common.cuh"
 
 namespace rgs {
@@ -166,34 +168,62 @@ __global__ void __launch_bounds__(256) filter3d_finish_kernel(int P, const unsig
 	filter_3D[i] = __fmul_rn(__fmul_rn(d, inv_focal), scale);
 }
 
-void launch_compute_3d_filter(int P, const float* xyz, int n_cams, const float* cams, float focal_length, float* filter_3D, float* max_distance,
-                              cudaStream_t s) {
+}  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+int32_t rgs_activate_forward(int32_t P, const float* raw_scaling, const float* raw_opacity, const float* raw_rotation, const float* filter_3D,
+                             float* scales, float* opacity, float* rotations, void* cuda_stream) {
+	if (P < 0) return fail(RGS_E_INVALID, "negative Gaussian count");
+	if (P == 0) return RGS_OK;
+	if (!raw_scaling || !raw_opacity || !raw_rotation || !filter_3D || !scales || !opacity || !rotations) return fail(RGS_E_INVALID, "null pointer");
+	activate_forward_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)cuda_stream>>>(P, raw_scaling, raw_opacity, raw_rotation, filter_3D, scales, opacity,
+	                                                                                rotations);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "activate forward");
+}
+
+int32_t rgs_activate_backward(int32_t P, const float* raw_scaling, const float* raw_opacity, const float* raw_rotation, const float* filter_3D,
+                              const float* g_scales, const float* g_opacity, const float* g_rotations, float* d_raw_scaling, float* d_raw_opacity,
+                              float* d_raw_rotation, void* cuda_stream) {
+	if (P < 0) return fail(RGS_E_INVALID, "negative Gaussian count");
+	if (P == 0) return RGS_OK;
+	if (!raw_scaling || !raw_opacity || !raw_rotation || !filter_3D || !g_scales || !g_opacity || !g_rotations || !d_raw_scaling || !d_raw_opacity ||
+	    !d_raw_rotation)
+		return fail(RGS_E_INVALID, "null pointer");
+	activate_backward_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)cuda_stream>>>(P, raw_scaling, raw_opacity, raw_rotation, filter_3D, g_scales, g_opacity,
+	                                                                                 g_rotations, d_raw_scaling, d_raw_opacity, d_raw_rotation);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "activate backward");
+}
+
+int32_t rgs_densification_stats(int32_t P, const float* means2D_grad, const int32_t* radii, float* grad_accum, float* grad_accum_abs,
+                                float* grad_accum_abs_max, float* denom, float* max_radii2D, void* cuda_stream) {
+	if (P < 0) return fail(RGS_E_INVALID, "negative Gaussian count");
+	if (P == 0) return RGS_OK;
+	if (!means2D_grad || !radii || !grad_accum || !grad_accum_abs || !grad_accum_abs_max || !denom) return fail(RGS_E_INVALID, "null pointer");
+	densification_stats_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)cuda_stream>>>(P, means2D_grad, radii, grad_accum, grad_accum_abs,
+	                                                                                    grad_accum_abs_max, denom, max_radii2D);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "densification stats");
+}
+
+int32_t rgs_compute_3d_filter(int32_t P, const float* xyz, int32_t n_cams, const float* cams, float focal_length, float* filter_3D,
+                              float* max_distance, void* cuda_stream) {
+	if (P < 0 || n_cams < 0) return fail(RGS_E_INVALID, "negative count");
+	if (P == 0) return RGS_OK;
+	if (!xyz || !filter_3D || !max_distance || (n_cams > 0 && !cams)) return fail(RGS_E_INVALID, "null pointer");
+	if (!(focal_length > 0.0f)) return fail(RGS_E_INVALID, "focal_length must be positive");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
 	unsigned int* max_bits = reinterpret_cast<unsigned int*>(max_distance);
 	cudaMemsetAsync(max_bits, 0, sizeof(unsigned int), s);
 	filter3d_distance_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, xyz, n_cams, cams, filter_3D, max_bits);
 	count_launch();
 	filter3d_finish_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, max_bits, 1.0f / focal_length, (float)0.4472135954999579 /* 0.2 ** 0.5 */, filter_3D);
 	count_launch();
+	return cuda_status(cudaGetLastError(), "compute 3d filter");
 }
 
-void launch_activate_forward(int P, const float* raw_scaling, const float* raw_opacity, const float* raw_rotation, const float* filter_3D, float* scales,
-                             float* opacity, float* rotations, cudaStream_t s) {
-	activate_forward_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, raw_scaling, raw_opacity, raw_rotation, filter_3D, scales, opacity, rotations);
-	count_launch();
-}
-
-void launch_activate_backward(int P, const float* raw_scaling, const float* raw_opacity, const float* raw_rotation, const float* filter_3D,
-                              const float* g_scales, const float* g_opacity, const float* g_rotations, float* d_raw_scaling, float* d_raw_opacity,
-                              float* d_raw_rotation, cudaStream_t s) {
-	activate_backward_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, raw_scaling, raw_opacity, raw_rotation, filter_3D, g_scales, g_opacity, g_rotations,
-	                                                          d_raw_scaling, d_raw_opacity, d_raw_rotation);
-	count_launch();
-}
-
-void launch_densification_stats(int P, const float* means2D_grad, const int* radii, float* grad_accum, float* grad_accum_abs, float* grad_accum_abs_max,
-                                float* denom, float* max_radii2D, cudaStream_t s) {
-	densification_stats_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, means2D_grad, radii, grad_accum, grad_accum_abs, grad_accum_abs_max, denom, max_radii2D);
-	count_launch();
-}
-
-}  // namespace rgs
+}  // extern "C"

@@ -16,6 +16,8 @@
 //
 // Zero padding of conv2 and conv3 is at the borders of the crop-sized maps.  Backward reads the activations instead of
 // recomputing them: a recompute would need conv2 on a 3-pixel halo around each tile (about 1.7x forward's conv2 FMAs).
+//
+// This file also holds the C-ABI entry points rgs_appearance_* (include/rgs_b200.h).
 #include "rgs_common.cuh"
 
 namespace rgs {
@@ -467,48 +469,70 @@ float down_scale(int in, int out) { return out > 1 ? (float)(in - 1) / (float)(o
 
 size_t g_fwd_smem[64], g_bwd_smem[64];
 
+int32_t appearance_size(int32_t H0, int32_t W0) {
+	if (H0 < 32 || W0 < 32) return fail(RGS_E_INVALID, "appearance loss: the image must be at least 32 x 32");
+	if ((int64_t)H0 * W0 > (int64_t)1 << 28) return fail(RGS_E_INVALID, "appearance loss: image too large");
+	return RGS_OK;
+}
+
 }  // namespace
+}  // namespace rgs
 
-cudaError_t launch_appearance_downsample(int H0, int W0, const float* img, float* down, cudaStream_t s) {
+using namespace rgs;
+
+extern "C" {
+
+int32_t rgs_appearance_downsample(int32_t H0, int32_t W0, const float* image, float* down, void* cuda_stream) {
+	if (const int32_t rc = appearance_size(H0, W0)) return rc;
+	if (!image || !down) return fail(RGS_E_INVALID, "null pointer");
 	const Crop k = make_crop(H0, W0);
 	const int n = 3 * k.h * k.w;
-	downsample_kernel<<<(n + 255) / 256, 256, 0, s>>>(k, down_scale(k.H, k.h), down_scale(k.W, k.w), img, down);
+	downsample_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)cuda_stream>>>(k, down_scale(k.H, k.h), down_scale(k.W, k.w), image, down);
 	count_launch();
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "appearance downsample");
 }
 
-cudaError_t launch_appearance_downsample_backward(int H0, int W0, const float* d_down, float* d_img, cudaStream_t s) {
+int32_t rgs_appearance_downsample_backward(int32_t H0, int32_t W0, const float* d_down, float* d_image, void* cuda_stream) {
+	if (const int32_t rc = appearance_size(H0, W0)) return rc;
+	if (!d_down || !d_image) return fail(RGS_E_INVALID, "null pointer");
 	const Crop k = make_crop(H0, W0);
 	const int n = 3 * k.h * k.w;
-	downsample_backward_kernel<<<(n + 255) / 256, 256, 0, s>>>(k, down_scale(k.H, k.h), down_scale(k.W, k.w), d_down, d_img);
+	downsample_backward_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)cuda_stream>>>(k, down_scale(k.H, k.h), down_scale(k.W, k.w), d_down, d_image);
 	count_launch();
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "appearance downsample backward");
 }
 
-cudaError_t launch_appearance_l1_forward(int H0, int W0, const float* img, const float* gt, const float* up4, const float* w2, const float* b2, const float* w3,
-                                         const float* b3, float* act, float* out, double* partials, float* loss, cudaStream_t s) {
+int32_t rgs_appearance_l1_forward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* w2, const float* b2,
+                                  const float* w3, const float* b3, float* act, float* transformed, double* partials, float* loss, void* cuda_stream) {
+	if (const int32_t rc = appearance_size(H0, W0)) return rc;
+	if (!image || !gt || !up4 || !w2 || !b2 || !w3 || !b3 || !partials || !loss) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
 	const Crop k = make_crop(H0, W0);
 	const size_t bytes = F_SMEM * sizeof(float);
 	ensure_dynamic_smem(tail_forward_kernel, bytes, g_fwd_smem);
-	tail_forward_kernel<<<NCTA, NT, bytes, s>>>(k, img, gt, up4, w2, b2, w3, b3, act, out, partials);
+	tail_forward_kernel<<<NCTA, NT, bytes, s>>>(k, image, gt, up4, w2, b2, w3, b3, act, transformed, partials);
 	loss_finish_kernel<<<1, 1, 0, s>>>(partials, NCTA, 3.0 * k.H * k.W, loss);
 	count_launch(2);
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "appearance l1 forward");
 }
 
-cudaError_t launch_appearance_l1_backward(int H0, int W0, const float* img, const float* gt, const float* up4, const float* act, const float* w2, const float* w3,
-                                          const float* b3, const float* upstream, float* d_img, float* d_up4, float* d_w2, float* d_b2, float* d_w3,
-                                          float* d_b3, double* partials, float* d_x, cudaStream_t s) {
+int32_t rgs_appearance_l1_backward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* act, const float* w2,
+                                   const float* w3, const float* b3, const float* upstream, float* d_image, float* d_up4, float* d_w2, float* d_b2,
+                                   float* d_w3, float* d_b3, double* partials, float* d_x, void* cuda_stream) {
+	if (const int32_t rc = appearance_size(H0, W0)) return rc;
+	if (!image || !gt || !up4 || !act || !w2 || !w3 || !b3 || !d_image || !d_up4 || !d_w2 || !d_b2 || !d_w3 || !d_b3 || !partials || !d_x)
+		return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
 	const Crop k = make_crop(H0, W0);
 	const size_t bytes = B_SMEM * sizeof(float);
 	ensure_dynamic_smem(tail_backward_kernel, bytes, g_bwd_smem);
-	cudaMemsetAsync(d_img, 0, (size_t)3 * H0 * W0 * sizeof(float), s);  // outside the crop (slice_backward's zero fill)
-	tail_backward_kernel<<<NCTA, NT, bytes, s>>>(k, img, gt, up4, act, w2, w3, b3, upstream, d_img, d_x, partials);
+	cudaMemsetAsync(d_image, 0, (size_t)3 * H0 * W0 * sizeof(float), s);  // outside the crop (slice_backward's zero fill)
+	tail_backward_kernel<<<NCTA, NT, bytes, s>>>(k, image, gt, up4, act, w2, w3, b3, upstream, d_image, d_x, partials);
 	grad_finish_kernel<<<(GRAD_FLOATS + 255) / 256, 256, 0, s>>>(partials, NCTA, d_w2, d_b2, d_w3, d_b3);
 	const int n = 16 * k.Hu * k.Wu;
 	upsample_transpose_kernel<<<(n + 255) / 256, 256, 0, s>>>(k, d_x, d_up4);
 	count_launch(3);
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "appearance l1 backward");
 }
 
-}  // namespace rgs
+}  // extern "C"

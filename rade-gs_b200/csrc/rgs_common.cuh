@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <string>
+
 #include "../../include/rgs_b200.h"
 
 namespace rgs {
@@ -198,6 +200,26 @@ __device__ __forceinline__ void red_add_v4(float* addr, float4 v) {
 // ---- host-side launch bookkeeping -----------------------------------------------------------------
 void count_launch(int n = 1);
 
+// ---- C-ABI status (rgs_api.cu): every entry point reports through these; rgs_last_error() reads the message ----
+// `msg` into the calling thread's error buffer; returns `code`.
+int fail(int code, const std::string& msg);
+
+#define RGS_CUDA_TRY(expr)                                                                                   \
+	do {                                                                                                     \
+		cudaError_t _e = (expr);                                                                             \
+		if (_e != cudaSuccess) return fail(RGS_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
+	} while (0)
+
+// A launcher's result as a status of entry `what`.  The DTU and TNT launchers report a non-finite input point as
+// cudaErrorInvalidValue; they pass `invalid`, the message that turns it into RGS_E_INVALID.
+int cuda_status(cudaError_t e, const char* what, const char* invalid = nullptr);
+
+extern const char* const kNonFinitePoint;
+
+// `bytes` from the caller's resize callback into `buf`.  NULL is a failure only when bytes were asked for: an empty
+// output may come back as NULL.
+int grow(rgs_resize_fn fn, void* user, size_t bytes, char*& buf, const char* what);
+
 // Opt a kernel in to `bytes` of dynamic shared memory on the CURRENT device (the attribute is per device and per
 // function; remembered per device so the driver call happens once, also when one process drives several GPUs).
 template <typename Kernel>
@@ -262,18 +284,6 @@ void launch_preprocess_backward(const FwdParams& p, GeomView g, const int* radii
                                 bool prefilled = false);
 void launch_backward_zero_fill(const FwdParams& p, ParamGradOut out, cudaStream_t s);
 
-// fused activations / densification statistics (rgs_activation.cu; SURVEY.md 8f row 1)
-void launch_activate_forward(int P, const float* raw_scaling, const float* raw_opacity, const float* raw_rotation, const float* filter_3D, float* scales,
-                             float* opacity, float* rotations, cudaStream_t s);
-void launch_activate_backward(int P, const float* raw_scaling, const float* raw_opacity, const float* raw_rotation, const float* filter_3D,
-                              const float* g_scales, const float* g_opacity, const float* g_rotations, float* d_raw_scaling, float* d_raw_opacity,
-                              float* d_raw_rotation, cudaStream_t s);
-void launch_densification_stats(int P, const float* means2D_grad, const int* radii, float* grad_accum, float* grad_accum_abs, float* grad_accum_abs_max,
-                                float* denom, float* max_radii2D, cudaStream_t s);
-
-void launch_compute_3d_filter(int P, const float* xyz, int n_cams, const float* cams, float focal_length, float* filter_3D, float* max_distance,
-                              cudaStream_t s);
-
 // opacity integration at query points (rgs_integrate.cu; SURVEY.md 8f row 3)
 struct IntegrateView {
 	int PN;
@@ -294,175 +304,5 @@ struct IntegrateOut {
 size_t integrate_sort_temp_bytes(int PN);
 size_t integrate_mask_words(int64_t R, int tiles);
 void launch_integrate(const FwdParams& p, GeomView g, BinView b, ImgView img, const int* radii, IntegrateView v, IntegrateOut out, cudaStream_t s);
-
-// mean squared distance to the 3 nearest other points (rgs_knn.cu; simple_knn's distCUDA2).  One stream synchronisation
-// inside (the finite-point count sizes the tree); returns the first CUDA error.
-size_t knn_scratch_bytes(int P);
-cudaError_t launch_knn_mean_dist2(int P, const float* points, float* out, char* scratch, cudaStream_t s);
-
-// TSDF fusion and marching cubes (rgs_tsdf.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
-size_t tsdf_touch_scratch_bytes(int64_t n);
-cudaError_t launch_tsdf_touch(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c, const float* depth, int32_t* counters_host, cudaStream_t s);
-cudaError_t launch_tsdf_touch_sort(const rgs_tsdf_grid& g, int64_t n, int32_t* out, char* scratch, cudaStream_t s);
-cudaError_t launch_tsdf_integrate(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c, int64_t n, const int32_t* bc, const float* depth, const float* color,
-                                  int32_t call_id, int32_t* slot, cudaStream_t s);
-cudaError_t launch_tsdf_rehash(const rgs_tsdf_grid& g, const uint64_t* old_keys, const int32_t* old_vals, int64_t old_slots, cudaStream_t s);
-size_t tsdf_active_scratch_bytes(int N);
-cudaError_t launch_tsdf_active(const rgs_tsdf_grid& g, int N, uint64_t* keys, int32_t* pools, char* scratch, cudaStream_t s);
-size_t tsdf_extract_scratch_bytes(const rgs_tsdf_grid& g, int N);
-cudaError_t launch_tsdf_extract_count(const rgs_tsdf_grid& g, int N, float thr, char* scratch, int64_t* totals_host, cudaStream_t s);
-cudaError_t launch_tsdf_extract_emit(const rgs_tsdf_grid& g, int N, char* scratch, float* verts, float* colors, int32_t* tris, cudaStream_t s);
-size_t tsdf_normals_scratch_bytes(int64_t V, int64_t F);
-cudaError_t launch_tsdf_normals(int64_t V, const float* verts, int64_t F, const int32_t* tris, float* normals, char* scratch, cudaStream_t s);
-
-// DTU evaluation (rgs_dtu_eval.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
-size_t dtu_sample_scratch_bytes(int64_t F);
-cudaError_t launch_dtu_sample_count(int64_t V, const double* verts, int64_t F, const int32_t* faces, double density, char* scratch, int64_t* totals_host,
-                                    cudaStream_t s);
-size_t dtu_sample_rows_bytes(int64_t R);
-cudaError_t launch_dtu_sample_emit(int64_t V, const double* verts, int64_t F, const int32_t* faces, double density, char* scratch, int64_t S, int64_t R,
-                                   char* rows_scratch, double* out, cudaStream_t s);
-size_t dtu_downsample_scratch_bytes(int N);
-cudaError_t launch_dtu_downsample(int N, const double* pts, double radius, uint8_t* kept, char* scratch, int32_t* rounds, cudaStream_t s);
-size_t dtu_nearest_scratch_bytes(int M, int N);
-cudaError_t launch_dtu_nearest(int M, const double* ref, int N, const double* query, double* dist, int64_t* index, char* scratch, cudaStream_t s);
-cudaError_t launch_dtu_dilate(int n_views, int H, int W, const uint8_t* masks, uint8_t* out, cudaStream_t s);
-cudaError_t launch_dtu_cull(int64_t V, const double* verts, int n_views, int H, int W, const double* proj, const uint8_t* masks, uint8_t* keep,
-                            cudaStream_t s);
-
-// TNT evaluation (rgs_tnt_eval.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
-size_t tnt_crop_scratch_bytes(int N);
-cudaError_t launch_tnt_crop(int N, const double* pts, const double* xform, int axis, double axis_min, double axis_max, int K, const double* polygon,
-                            uint8_t* kept, double* cropped, int64_t* num_kept, char* scratch, cudaStream_t s);
-cudaError_t launch_tnt_transform(int64_t N, double* pts, const double* xform, cudaStream_t s);
-size_t tnt_bounds_scratch_bytes();
-size_t tnt_voxel_scratch_bytes(int N);
-cudaError_t launch_tnt_bounds(int N, const double* pts, char* scratch, double* lo, double* hi, int64_t* nonfinite, cudaStream_t s);
-cudaError_t launch_tnt_voxel_sort(int N, const double* pts, const double* origin, double voxel, char* scratch, int32_t* num_voxels, cudaStream_t s);
-cudaError_t launch_tnt_voxel_mean(int N, const double* pts, int V, char* scratch, double* means, int64_t* counts, cudaStream_t s);
-size_t tnt_moments_scratch_bytes(int64_t N);
-cudaError_t launch_tnt_moments(int64_t N, const double* src, int64_t M, const double* tgt, const double* dist, const int64_t* index, double thr,
-                               char* scratch, double* moments_host, cudaStream_t s);
-
-// Tetrahedra mesh extraction (rgs_tetra.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
-cudaError_t launch_tetra_points(int P, const float* xyz, const float* scaling, const float* rotation, float* points, float* scales, cudaStream_t s);
-cudaError_t launch_tetra_cull_add(int64_t N, const float* alpha, const float* coord, int H, int W, const float* render7, const float* gt_mask, float* fin,
-                                  int32_t* weight, cudaStream_t s);
-cudaError_t launch_tetra_cull_finish(int64_t N, const float* fin, const int32_t* weight, float* sdf, cudaStream_t s);
-size_t tetra_march_scratch1_bytes(int64_t T);
-size_t tetra_march_scratch2_bytes(int V);
-cudaError_t launch_tetra_march_valid(int64_t T, int64_t N, const int64_t* tets, const float* sdf, char* scratch1, int32_t* bad, int32_t* num_valid,
-                                     cudaStream_t s);
-cudaError_t launch_tetra_march_sort(int64_t T, int64_t N, const int64_t* tets, const float* sdf, int V, const char* scratch1, char* scratch2,
-                                    int32_t* num_vertices, int32_t* num_faces, cudaStream_t s);
-cudaError_t launch_tetra_march_emit(int64_t T, const float* points, const float* sdf, const float* scales, int V, const char* scratch1, char* scratch2,
-                                    int64_t N, int64_t* interp, float* ends, float* end_sdf, float* end_scl, int64_t* faces, cudaStream_t s);
-cudaError_t launch_tetra_bisect(int64_t M, const float* mid_sdf, float* left, float* right, float* left_sdf, float* right_sdf, float* mid, cudaStream_t s);
-size_t tetra_filter_scratch_bytes(int M, int64_t F);
-cudaError_t launch_tetra_filter(int M, const float* points, const float* ends, const float* end_scl, int64_t F, const int64_t* faces, char* scratch,
-                                float* out_vertices, int64_t* out_faces, int64_t* num_vertices, int64_t* num_faces, int32_t* bad, cudaStream_t s);
-
-// Delaunay tetrahedralization (rgs_delaunay.cu; contract in include/rgs_b200.h).  rgs_api.cu drives the rounds and owns
-// every allocation; argument checks are its job.
-constexpr float DT_MAX_COORD = 0x1p90f;     // |coordinate| bound of rgs_delaunay's input
-constexpr double DT_GHOST_SCALE = 0x1p30;   // D: ghost distance in units of the box's power-of-two extent
-constexpr int DT_SLOT_CELLS = 64;           // per-nominee cavity capacity of a round ...
-constexpr int DT_SLOT_FACES = 128;          // ... and its boundary-face capacity
-constexpr int DT_MAX_SLOTS = 1 << 19;       // nominees per round
-
-struct DtCounters {
-	int bad;                 // points out of range or not finite
-	uint32_t box[6];         // ordered-int bounding box (lo xyz, hi xyz)
-	int cells;               // cells in use (dead ones included)
-	int slots;               // nominees this round
-	int full;                // a winner found no room to append: grow the mesh
-	int overflowed;          // cavities larger than their slot in this pass
-	int overflow_point;      // the smallest of their points
-	int violation;           // a new cell was not positive, or a point found no cell: a predicate bug
-	int inserted;            // points inserted so far
-	int max_cavity;          // largest cavity inserted through a slot
-	int out_cells;           // cells emitted
-	uint32_t unique, spare;  // host side only: distinct points
-};
-struct DtPointsView {
-	DtCounters* cnt;
-	float4* verts;           // [n + 4] representatives in Morton order, then the ghosts
-	uint32_t* rep;           // [n] original index of each vertex
-	int32_t* loc;            // [n] located cell, -1 once inserted
-	uint64_t* key64[2];
-	uint32_t *key32[2], *ids[2], *first, *rank;   // first: after preparation, the round's overflowed points
-	char* temp;
-	size_t temp_bytes;
-};
-struct DtMesh {
-	int4* tet;               // [cap] vertices, positive; -1 rows are dead
-	int4* adj;               // [cap] neighbour across the face opposite vertex k: cell << 2 | face, -1 for none
-	uint64_t* claim;         // [cap] (priority << 32 | slot) of the round
-	uint64_t* nom;           // [cap] nominee of the round: (hash << 32 | point)
-	int2* died;              // [cap] (pass, slot) that removed the cell
-	int32_t* loc;            // the points' located cells (set by the launchers)
-};
-struct DtSlots {
-	int *point, *cell, *k, *b, *base, *won;   // [K]
-	int* cav;                // [K * DT_SLOT_CELLS] cavity cells
-	int4* bnd;               // [K * DT_SLOT_FACES] the new cell of each boundary face
-	int* bout;               // [K * DT_SLOT_FACES] the outside neighbour of each boundary face
-};
-DtPointsView carve_dt_points(char* base, int N, size_t* total);
-DtMesh carve_dt_mesh(char* base, int64_t cap, size_t* total);
-DtSlots carve_dt_slots(char* base, int K, int64_t cc_total, int64_t cb_total, size_t* total);
-size_t dt_sort_bytes(int64_t cells);
-cudaError_t launch_dt_prepare(int N, const float* pts, const DtPointsView& v, DtCounters* host, cudaStream_t s);
-cudaError_t launch_dt_init(int N, const float* pts, int n, const DtPointsView& v, const DtCounters& host, const DtMesh& m, int64_t cap, cudaStream_t s);
-cudaError_t launch_dt_round(int n, const DtPointsView& v, const DtMesh& m, const DtSlots& sl, int K, int cc, int cb, int epoch, int64_t cap, int cells,
-                            cudaStream_t s);
-cudaError_t launch_dt_large(int n, const DtPointsView& v, const DtMesh& m, const DtSlots& sl, int K, int cc, int cb, int epoch, int64_t cap, int cells,
-                            cudaStream_t s);
-cudaError_t launch_dt_single_cavity(const DtPointsView& v, const DtMesh& m, const DtSlots& sl, int64_t cc_total, int64_t cb_total, int cells, cudaStream_t s);
-cudaError_t launch_dt_single_star(int n, const DtPointsView& v, const DtMesh& m, const DtSlots& sl, int64_t cc_total, int64_t cb_total, int epoch, int64_t cap,
-                                  cudaStream_t s);
-cudaError_t launch_dt_read(const DtPointsView& v, DtCounters* host, cudaStream_t s);
-cudaError_t launch_dt_grow_mesh(const DtMesh& from, int64_t from_cap, const DtMesh& to, int64_t to_cap, cudaStream_t s);
-cudaError_t launch_dt_emit(int n, const DtPointsView& v, const DtMesh& m, char* sort, int64_t cells, int* T, cudaStream_t s);
-cudaError_t launch_dt_sort(char* sort, int64_t cells, int T, int4* out, cudaStream_t s);
-cudaError_t launch_dt_predicates(int N, const float* pts, int M, const int32_t* tuples, int8_t* signs, int* bad_dev, int* bad_host, cudaStream_t s);
-
-// fused image-side losses (rgs_image_loss.cu; SURVEY.md 8f row 2)
-void launch_ssim_l1_forward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, float* dmaps, double* sums,
-                            cudaStream_t s);
-void launch_ssim_l1_backward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, const float* dmaps, float w_ssim,
-                             float w_l1, const float* upstream, float* d_img, cudaStream_t s);
-void launch_normal_consistency(int H, int W, bool from_depth, float inv_fx, float inv_fy, float cx, float cy, const float* rendered_normal,
-                               const float* map_e, const float* map_m, float w_e, float w_m, double* loss_sum, float* d_normal, float* d_e, float* d_m,
-                               cudaStream_t s);
-
-// decoupled-appearance L1 loss (rgs_appearance.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
-cudaError_t launch_appearance_downsample(int H0, int W0, const float* img, float* down, cudaStream_t s);
-cudaError_t launch_appearance_downsample_backward(int H0, int W0, const float* d_down, float* d_img, cudaStream_t s);
-cudaError_t launch_appearance_l1_forward(int H0, int W0, const float* img, const float* gt, const float* up4, const float* w2, const float* b2, const float* w3,
-                                         const float* b3, float* act, float* out, double* partials, float* loss, cudaStream_t s);
-cudaError_t launch_appearance_l1_backward(int H0, int W0, const float* img, const float* gt, const float* up4, const float* act, const float* w2, const float* w3,
-                                          const float* b3, const float* upstream, float* d_img, float* d_up4, float* d_w2, float* d_b2, float* d_w3,
-                                          float* d_b3, double* partials, float* d_x, cudaStream_t s);
-
-// densify-and-prune and opacity reset (rgs_densify.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
-int densify_blocks(int P);
-size_t densify_select_scratch_bytes(int P);
-cudaError_t launch_densify_select(int P, const float* accum, const float* accum_abs, const float* denom, const float* scaling, const float* opacity,
-                                  const rgs_densify_thresholds& th, uint8_t* flags, int* block_offsets, float* ratio_q, int* totals, char* scratch,
-                                  cudaStream_t s);
-cudaError_t launch_densify_plan(int P, const uint8_t* flags, const int* block_offsets, const int32_t* counts, const float* scaling, int* src, int* draw,
-                                float* std_clone, float* std_split, cudaStream_t s);
-cudaError_t launch_densify_gather(int N, const int* src, const int* draw, int C, const float* xyz, const float* rotation, const float* scaling,
-                                  const float* sample_clone, const float* sample_split, float inv_split, float* xyz_out, float* scaling_out, int n_cols,
-                                  const rgs_densify_column* cols, cudaStream_t s);
-cudaError_t launch_reset_opacity(int P, const float* scaling, const float* opacity, const float* filter_3D, float* out, cudaStream_t s);
-
-// LPIPS-VGG trunk and distance (rgs_lpips.cu; contract in include/rgs_b200.h).  Argument checks are the caller's.
-int lpips_distance_blocks(int HW);   // fp64 partial sums the distance of one layer writes
-cudaError_t launch_lpips_input_conv(int H, int W, const float* x, const float* y, const float* weight, const float* bias, float* out, cudaStream_t s);
-cudaError_t launch_lpips_conv3x3(int H, int W, int Cin, int Cout, const float* in, const float* weight, const float* bias, float* out, cudaStream_t s);
-cudaError_t launch_lpips_maxpool(int H, int W, int C, const float* in, float* out, cudaStream_t s);
-cudaError_t launch_lpips_distance(int HW, int C, const float* feats, const float* lin, float* map, double* partial, double* mean, cudaStream_t s);
 
 }  // namespace rgs

@@ -19,6 +19,8 @@
 // apart, so each winner rewrites its neighbours' back-pointers alone.  The cavities larger than a round's slot go through
 // the same claim protocol right after the round, in 16x larger slots; one still larger is inserted on its own, with the
 // whole slab area as its capacity.
+//
+// This file also holds the C-ABI entry points rgs_delaunay and rgs_delaunay_predicates (include/rgs_b200.h).
 #include <algorithm>
 #include <cstring>
 #include <cub/cub.cuh>
@@ -31,6 +33,51 @@ namespace {
 constexpr int DT_BLOCK = 256;
 constexpr uint64_t NO_NOMINEE = ~0ull;
 constexpr uint64_t VISITED = ~1ull;   // a mark in nom[] for the single-cavity pass; point ids stay below 2^29
+
+constexpr float DT_MAX_COORD = 0x1p90f;     // |coordinate| bound of rgs_delaunay's input
+constexpr double DT_GHOST_SCALE = 0x1p30;   // D: ghost distance in units of the box's power-of-two extent
+constexpr int DT_SLOT_CELLS = 64;           // per-nominee cavity capacity of a round ...
+constexpr int DT_SLOT_FACES = 128;          // ... and its boundary-face capacity
+constexpr int DT_MAX_SLOTS = 1 << 19;       // nominees per round
+
+struct DtCounters {
+	int bad;                 // points out of range or not finite
+	uint32_t box[6];         // ordered-int bounding box (lo xyz, hi xyz)
+	int cells;               // cells in use (dead ones included)
+	int slots;               // nominees this round
+	int full;                // a winner found no room to append: grow the mesh
+	int overflowed;          // cavities larger than their slot in this pass
+	int overflow_point;      // the smallest of their points
+	int violation;           // a new cell was not positive, or a point found no cell: a predicate bug
+	int inserted;            // points inserted so far
+	int max_cavity;          // largest cavity inserted through a slot
+	int out_cells;           // cells emitted
+	uint32_t unique, spare;  // host side only: distinct points
+};
+struct DtPointsView {
+	DtCounters* cnt;
+	float4* verts;           // [n + 4] representatives in Morton order, then the ghosts
+	uint32_t* rep;           // [n] original index of each vertex
+	int32_t* loc;            // [n] located cell, -1 once inserted
+	uint64_t* key64[2];
+	uint32_t *key32[2], *ids[2], *first, *rank;   // first: after preparation, the round's overflowed points
+	char* temp;
+	size_t temp_bytes;
+};
+struct DtMesh {
+	int4* tet;               // [cap] vertices, positive; -1 rows are dead
+	int4* adj;               // [cap] neighbour across the face opposite vertex k: cell << 2 | face, -1 for none
+	uint64_t* claim;         // [cap] (priority << 32 | slot) of the round
+	uint64_t* nom;           // [cap] nominee of the round: (hash << 32 | point)
+	int2* died;              // [cap] (pass, slot) that removed the cell
+	int32_t* loc;            // the points' located cells (set by the launchers)
+};
+struct DtSlots {
+	int *point, *cell, *k, *b, *base, *won;   // [K]
+	int* cav;                // [K * DT_SLOT_CELLS] cavity cells
+	int4* bnd;               // [K * DT_SLOT_FACES] the new cell of each boundary face
+	int* bout;               // [K * DT_SLOT_FACES] the outside neighbour of each boundary face
+};
 
 // ---------------------------------------------------------------------------------------------------------------------
 // exact predicates
@@ -641,8 +688,6 @@ __global__ void __launch_bounds__(DT_BLOCK) dt_predicates_kernel(int M, int N, c
 
 inline unsigned blocks(int64_t n) { return (unsigned)((n + DT_BLOCK - 1) / DT_BLOCK); }
 
-}  // namespace
-
 // ---------------------------------------------------------------------------------------------------------------------
 // host side
 
@@ -887,4 +932,147 @@ cudaError_t launch_dt_predicates(int N, const float* pts, int M, const int32_t* 
 	return cudaGetLastError();
 }
 
+}  // namespace
 }  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+int32_t rgs_delaunay(int64_t N, const float* points, rgs_resize_fn resize, rgs_delaunay_out* out, void* cuda_stream) {
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	out->num_cells = 0;
+	out->rounds = out->max_cavity = out->overflowed = out->alone = out->mesh_growths = 0;
+	if (N < 0 || N > RGS_DELAUNAY_MAX_POINTS) return fail(RGS_E_INVALID, "delaunay: point count out of range (at most 2^26)");
+	if (N > 0 && !points) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	constexpr int64_t MAX_CELLS = (int64_t)1 << 29;
+	int rc;
+	char* cells_out = nullptr;
+	if (N == 0) return grow(resize, out->cells_user, 0, cells_out, "delaunay");
+
+	size_t bytes = 0;
+	char* pbuf = nullptr;
+	carve_dt_points(nullptr, (int)N, &bytes);
+	if ((rc = grow(resize, out->points_user, bytes, pbuf, "delaunay scratch")) != RGS_OK) return rc;
+	const DtPointsView v = carve_dt_points(pbuf, (int)N, nullptr);
+	DtCounters h;
+	if ((rc = cuda_status(launch_dt_prepare((int)N, points, v, &h, s), "delaunay")) != RGS_OK) return rc;
+	if (h.bad) return fail(RGS_E_INVALID, "delaunay: a coordinate is not finite or exceeds 2^90 in magnitude");
+	const int n = (int)h.unique;
+	if (n < 4) return grow(resize, out->cells_user, 0, cells_out, "delaunay");
+
+	int cur = 0;
+	int64_t cap = std::min<int64_t>(8 * (int64_t)n + 64, MAX_CELLS);
+	char* mbuf = nullptr;
+	carve_dt_mesh(nullptr, cap, &bytes);
+	if ((rc = grow(resize, out->mesh_user[0], bytes, mbuf, "delaunay mesh")) != RGS_OK) return rc;
+	DtMesh m = carve_dt_mesh(mbuf, cap, nullptr);
+	if ((rc = cuda_status(launch_dt_init((int)N, points, n, v, h, m, cap, s), "delaunay")) != RGS_OK) return rc;
+
+	const int K = std::min(DT_MAX_SLOTS, n);
+	int64_t cc_total = (int64_t)K * DT_SLOT_CELLS, cb_total = (int64_t)K * DT_SLOT_FACES;
+	DtSlots sl;
+	auto slabs = [&]() -> int {
+		char* buf = nullptr;
+		carve_dt_slots(nullptr, K, cc_total, cb_total, &bytes);
+		const int r = grow(resize, out->slab_user, bytes, buf, "delaunay slabs");
+		sl = carve_dt_slots(buf, K, cc_total, cb_total, nullptr);
+		return r;
+	};
+	// the mesh moves into the other buffer at (at least) twice the size; dead rows fill the new tail
+	auto grow_mesh = [&](int64_t want) -> int {
+		const int64_t nc = std::min(std::max(2 * cap, want), MAX_CELLS);
+		if (nc < want || nc <= cap) return fail(RGS_E_CAPACITY, "delaunay: the mesh needs more than 2^29 cells");
+		char* buf = nullptr;
+		carve_dt_mesh(nullptr, nc, &bytes);
+		if (const int r = grow(resize, out->mesh_user[1 - cur], bytes, buf, "delaunay mesh")) return r;
+		const DtMesh nm = carve_dt_mesh(buf, nc, nullptr);
+		if (const int r = cuda_status(launch_dt_grow_mesh(m, cap, nm, nc, s), "delaunay")) return r;
+		m = nm;
+		cap = nc;
+		cur = 1 - cur;
+		out->mesh_growths++;
+		return RGS_OK;
+	};
+	auto checked = [&](const DtCounters& c) -> int {
+		return c.violation ? fail(RGS_E_CUDA, "delaunay: a new cell is not positively oriented or a point found no cell (predicate bug)") : RGS_OK;
+	};
+	if ((rc = slabs()) != RGS_OK) return rc;
+
+	// Every pass can leave the device's cell counter above the capacity (a winner that found no room has added its cells
+	// already); the mesh then grows to at least twice that count, so `cells`, the extent the next pass initialises and
+	// scans, is the device's count.
+	int epoch = 0, cells = 1;
+	auto after_pass = [&]() -> int {
+		if (const int r = checked(h)) return r;
+		if (h.full)
+			if (const int r = grow_mesh(2 * (int64_t)h.cells)) return r;
+		cells = (int)std::min<int64_t>(h.cells, cap);
+		return RGS_OK;
+	};
+	// the cavities too large for a round's slot go in right after it, several at once, in slots 16 times as large
+	const int KL = std::max(1, K / 16);
+	while ((int)h.inserted < n) {
+		out->rounds++;
+		if ((rc = cuda_status(launch_dt_round(n, v, m, sl, K, DT_SLOT_CELLS, DT_SLOT_FACES, ++epoch, cap, cells, s), "delaunay")) != RGS_OK ||
+		    (rc = cuda_status(launch_dt_read(v, &h, s), "delaunay")) != RGS_OK || (rc = after_pass()) != RGS_OK)
+			return rc;
+		if (h.overflowed == 0) continue;
+		out->overflowed += h.overflowed;
+		if ((rc = cuda_status(launch_dt_large(n, v, m, sl, KL, (int)(cc_total / KL), (int)(cb_total / KL), ++epoch, cap, cells, s), "delaunay")) != RGS_OK ||
+		    (rc = cuda_status(launch_dt_read(v, &h, s), "delaunay")) != RGS_OK || (rc = after_pass()) != RGS_OK)
+			return rc;
+		// one still larger: the smallest such point goes in alone, with the whole slab area (grown as needed)
+		while (h.overflowed > 0) {
+			if ((rc = cuda_status(launch_dt_single_cavity(v, m, sl, cc_total, cb_total, cells, s), "delaunay")) != RGS_OK ||
+			    (rc = cuda_status(launch_dt_read(v, &h, s), "delaunay")) != RGS_OK)
+				return rc;
+			if (h.overflowed) {
+				cc_total *= 2;
+				cb_total *= 2;
+				if (cc_total > MAX_CELLS) return fail(RGS_E_CAPACITY, "delaunay: a cavity exceeds 2^29 cells");
+				if ((rc = slabs()) != RGS_OK) return rc;
+				continue;
+			}
+			if ((rc = cuda_status(launch_dt_single_star(n, v, m, sl, cc_total, cb_total, ++epoch, cap, s), "delaunay")) != RGS_OK ||
+			    (rc = cuda_status(launch_dt_read(v, &h, s), "delaunay")) != RGS_OK || (rc = after_pass()) != RGS_OK)
+				return rc;
+			if (!h.full) {
+				out->alone++;
+				break;
+			}
+			h.overflowed = 1;
+		}
+	}
+	out->max_cavity = h.max_cavity;
+
+	char* sbuf = nullptr;
+	int T = 0;
+	if ((rc = grow(resize, out->sort_user, dt_sort_bytes(cells), sbuf, "delaunay sort")) != RGS_OK ||
+	    (rc = cuda_status(launch_dt_emit(n, v, m, sbuf, cells, &T, s), "delaunay")) != RGS_OK ||
+	    (rc = grow(resize, out->cells_user, (size_t)T * 4 * sizeof(int32_t), cells_out, "delaunay")) != RGS_OK ||
+	    (rc = cuda_status(launch_dt_sort(sbuf, cells, T, reinterpret_cast<int4*>(cells_out), s), "delaunay")) != RGS_OK)
+		return rc;
+	out->num_cells = T;
+	return RGS_OK;
+}
+
+int32_t rgs_delaunay_predicates(int64_t N, const float* points, int64_t M, const int32_t* tuples, int8_t* signs, rgs_resize_fn resize,
+                                void* scratch_user, void* cuda_stream) {
+	if (N < 0 || N > INT32_MAX || M < 0 || M > INT32_MAX) return fail(RGS_E_INVALID, "delaunay predicates: count out of range");
+	if (M == 0) return RGS_OK;
+	if (!resize || !points || !tuples || !signs) return fail(RGS_E_INVALID, "null pointer");
+	char* buf = nullptr;
+	int bad = 0;
+	int rc;
+	if ((rc = grow(resize, scratch_user, sizeof(int), buf, "delaunay predicates scratch")) != RGS_OK ||
+	    (rc = cuda_status(launch_dt_predicates((int)N, points, (int)M, tuples, signs, reinterpret_cast<int*>(buf), &bad, (cudaStream_t)cuda_stream),
+	                      "delaunay predicates")) != RGS_OK)
+		return rc;
+	if (bad == 1) return fail(RGS_E_INVALID, "delaunay predicates: an index lies outside [0, N)");
+	if (bad) return fail(RGS_E_INVALID, "delaunay predicates: a coordinate is not finite");
+	return RGS_OK;
+}
+
+}  // extern "C"

@@ -10,6 +10,8 @@
 //   gather   every output row written once from its source: the sampled offset R * sample + xyz and the split scaling
 //            log(exp(s) / 1.6) on new rows, every other column copied, zeros for the moments of new rows.
 // The floating-point contract (bit-exactness, operation order) is stated in include/rgs_b200.h.
+//
+// This file also holds the C-ABI entry points rgs_densify_* and rgs_reset_opacity (include/rgs_b200.h).
 #include <cub/cub.cuh>
 
 #include "rgs_common.cuh"
@@ -261,9 +263,9 @@ __global__ void __launch_bounds__(DENSIFY_CTA) reset_opacity_kernel(int P, const
 	out[i] = logf(__fdiv_rn(x, __fsub_rn(1.0f, x)));
 }
 
-int densify_blocks(int P) { return (P + DENSIFY_CTA - 1) / DENSIFY_CTA; }
+static int densify_blocks(int P) { return (P + DENSIFY_CTA - 1) / DENSIFY_CTA; }
 
-size_t densify_select_scratch_bytes(int P) {
+static size_t densify_select_scratch_bytes(int P) {
 	size_t sort_bytes = 0;
 	cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, (const float*)nullptr, (float*)nullptr, P);
 	Carver c(nullptr);
@@ -274,9 +276,9 @@ size_t densify_select_scratch_bytes(int P) {
 	return c.size();
 }
 
-cudaError_t launch_densify_select(int P, const float* accum, const float* accum_abs, const float* denom, const float* scaling, const float* opacity,
-                                  const rgs_densify_thresholds& th, uint8_t* flags, int* block_offsets, float* ratio_q, int* totals, char* scratch,
-                                  cudaStream_t s) {
+static cudaError_t launch_densify_select(int P, const float* accum, const float* accum_abs, const float* denom, const float* scaling,
+                                         const float* opacity, const rgs_densify_thresholds& th, uint8_t* flags, int* block_offsets, float* ratio_q,
+                                         int* totals, char* scratch, cudaStream_t s) {
 	size_t sort_bytes = 0;
 	RGS_TRY(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, (const float*)nullptr, (float*)nullptr, P));
 	Carver c(scratch);
@@ -296,17 +298,54 @@ cudaError_t launch_densify_select(int P, const float* accum, const float* accum_
 	return cudaGetLastError();
 }
 
-cudaError_t launch_densify_plan(int P, const uint8_t* flags, const int* block_offsets, const int32_t* counts, const float* scaling, int* src, int* draw,
-                                float* std_clone, float* std_split, cudaStream_t s) {
-	const PlanTotals t{counts[0], counts[1], counts[2], counts[3], counts[4]};
-	densify_plan_kernel<<<densify_blocks(P), DENSIFY_CTA, 0, s>>>(P, flags, block_offsets, t, scaling, src, draw, std_clone, std_split);
-	count_launch();
-	return cudaGetLastError();
+}  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+int32_t rgs_densify_blocks(int32_t P) { return P > 0 ? densify_blocks(P) : 0; }
+
+int32_t rgs_densify_select(int32_t P, const float* grad_accum, const float* grad_accum_abs, const float* denom, const float* scaling, const float* opacity,
+                           const rgs_densify_thresholds* thresholds, uint8_t* flags, int32_t* block_offsets, float* ratio_q, int32_t* counts_host,
+                           rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (P <= 0) return fail(RGS_E_INVALID, "densify: the model has no Gaussians");
+	if (!grad_accum || !grad_accum_abs || !denom || !scaling || !opacity || !thresholds || !flags || !block_offsets || !ratio_q || !counts_host || !scratch)
+		return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	char* buf = nullptr;
+	if (const int rc = grow(scratch, scratch_user, densify_select_scratch_bytes(P), buf, "densify scratch")) return rc;
+	// the five totals follow the per-CTA offsets in the scratch's tail: one copy brings them to the host
+	int32_t* totals = block_offsets + 5 * (size_t)densify_blocks(P);
+	cudaError_t e = launch_densify_select(P, grad_accum, grad_accum_abs, denom, scaling, opacity, *thresholds, flags, block_offsets, ratio_q, totals, buf, s);
+	if (e == cudaSuccess) e = cudaMemcpyAsync(counts_host, totals, 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+	return cuda_status(e, "densify select");
 }
 
-cudaError_t launch_densify_gather(int N, const int* src, const int* draw, int C, const float* xyz, const float* rotation, const float* scaling,
-                                  const float* sample_clone, const float* sample_split, float inv_split, float* xyz_out, float* scaling_out, int n_cols,
-                                  const rgs_densify_column* cols, cudaStream_t s) {
+int32_t rgs_densify_plan(int32_t P, const uint8_t* flags, const int32_t* block_offsets, const int32_t* counts_host, const float* scaling, int32_t* src,
+                         int32_t* draw, float* std_clone, float* std_split, void* cuda_stream) {
+	if (P <= 0) return fail(RGS_E_INVALID, "densify: the model has no Gaussians");
+	if (!flags || !block_offsets || !counts_host || !scaling) return fail(RGS_E_INVALID, "null pointer");
+	const int32_t* c = counts_host;
+	for (int k = 0; k < 5; k++)
+		if (c[k] < 0 || c[k] > P) return fail(RGS_E_INVALID, "densify plan: counts out of range");
+	if ((c[0] && !std_clone) || (c[1] && !std_split) || ((c[2] || c[3] || c[4]) && (!src || !draw))) return fail(RGS_E_INVALID, "null pointer");
+	const PlanTotals t{c[0], c[1], c[2], c[3], c[4]};
+	densify_plan_kernel<<<densify_blocks(P), DENSIFY_CTA, 0, (cudaStream_t)cuda_stream>>>(P, flags, block_offsets, t, scaling, src, draw, std_clone, std_split);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "densify plan");
+}
+
+int32_t rgs_densify_gather(int32_t N, const int32_t* src, const int32_t* draw, int32_t C, const float* xyz, const float* rotation, const float* scaling,
+                           const float* sample_clone, const float* sample_split, float inv_split, float* xyz_out, float* scaling_out, int32_t n_cols,
+                           const rgs_densify_column* cols, void* cuda_stream) {
+	if (N < 0 || C < 0 || n_cols < 0 || n_cols > RGS_DENSIFY_MAX_COLUMNS) return fail(RGS_E_INVALID, "densify gather: bad sizes");
+	if (N == 0) return RGS_OK;
+	if (!src || !draw || !xyz || !rotation || !scaling || !xyz_out || !scaling_out || (n_cols && !cols)) return fail(RGS_E_INVALID, "null pointer");
+	for (int k = 0; k < n_cols; k++)
+		if (!cols[k].in || !cols[k].out || cols[k].width <= 0) return fail(RGS_E_INVALID, "densify gather: bad column");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
 	densify_rows_kernel<<<densify_blocks(N), DENSIFY_CTA, 0, s>>>(N, src, draw, C, xyz, rotation, scaling, sample_clone, sample_split, inv_split, xyz_out,
 	                                                              scaling_out);
 	count_launch();
@@ -320,13 +359,16 @@ cudaError_t launch_densify_gather(int N, const int* src, const int* draw, int C,
 		densify_gather_kernel<<<dim3(grid_x, n_cols), DENSIFY_CTA, 0, s>>>(N, src, draw, g);
 		count_launch();
 	}
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "densify gather");
 }
 
-cudaError_t launch_reset_opacity(int P, const float* scaling, const float* opacity, const float* filter_3D, float* out, cudaStream_t s) {
-	reset_opacity_kernel<<<densify_blocks(P), DENSIFY_CTA, 0, s>>>(P, scaling, opacity, filter_3D, out);
+int32_t rgs_reset_opacity(int32_t P, const float* scaling, const float* opacity, const float* filter_3D, float* out, void* cuda_stream) {
+	if (P < 0) return fail(RGS_E_INVALID, "negative Gaussian count");
+	if (P == 0) return RGS_OK;
+	if (!scaling || !opacity || !filter_3D || !out) return fail(RGS_E_INVALID, "null pointer");
+	reset_opacity_kernel<<<densify_blocks(P), DENSIFY_CTA, 0, (cudaStream_t)cuda_stream>>>(P, scaling, opacity, filter_3D, out);
 	count_launch();
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "reset opacity");
 }
 
-}  // namespace rgs
+}  // extern "C"

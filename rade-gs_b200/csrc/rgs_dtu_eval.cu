@@ -13,6 +13,8 @@
 //   nearest    an fp64 copy of rgs_knn.cu's design: Morton-sorted 32-point leaves of the reference set under an implicit
 //              box tree, one warp per 32 Morton-sorted queries, nearer child first, stack one entry per lane.
 //   cull       disk(6) dilation of each view's mask, then one thread per vertex over all views.
+//
+// This file also holds the C-ABI entry points rgs_dtu_* (include/rgs_b200.h).
 #include <cub/cub.cuh>
 
 #include "rgs_common.cuh"
@@ -568,8 +570,6 @@ __global__ void __launch_bounds__(256) cull_kernel(int64_t V, const double* __re
 	keep[i] = ok;
 }
 
-}  // namespace
-
 // ---- sampling ----
 
 struct SampleScratch {
@@ -804,21 +804,79 @@ cudaError_t launch_dtu_nearest(int M, const double* ref, int N, const double* qu
 	return cudaGetLastError();
 }
 
-// ---- cull ----
-
-cudaError_t launch_dtu_dilate(int n_views, int H, int W, const uint8_t* masks, uint8_t* out, cudaStream_t s) {
-	const int64_t n = (int64_t)n_views * H * W;
-	if (n == 0) return cudaSuccess;
-	dilate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(n_views, H, W, masks, out);
-	count_launch();
-	return cudaGetLastError();
-}
-
-cudaError_t launch_dtu_cull(int64_t V, const double* verts, int n_views, int H, int W, const double* proj, const uint8_t* masks, uint8_t* keep, cudaStream_t s) {
-	if (V == 0) return cudaSuccess;
-	cull_kernel<<<(unsigned)((V + 255) / 256), 256, 0, s>>>(V, verts, n_views, H, W, proj, masks, keep);
-	count_launch();
-	return cudaGetLastError();
-}
-
+}  // namespace
 }  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+int32_t rgs_dtu_sample_mesh(int64_t V, const double* vertices, int64_t F, const int32_t* faces, double density, rgs_resize_fn resize,
+                            rgs_dtu_samples_out* out, void* cuda_stream) {
+	if (V < 0 || F < 0 || V > INT32_MAX || F > INT32_MAX - 1) return fail(RGS_E_INVALID, "dtu sample: vertex / face count out of range");
+	if (!resize || !out || (V > 0 && !vertices) || (F > 0 && !faces)) return fail(RGS_E_INVALID, "null pointer");
+	if (!(std::isfinite(density) && density > 0.0)) return fail(RGS_E_INVALID, "dtu sample: density must be positive and finite");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int rc;
+	int64_t totals[2] = {0, 0};   // samples, rows
+	char* buf = nullptr;
+	if (F > 0) {
+		if (V == 0) return fail(RGS_E_INVALID, "dtu sample: faces without vertices");
+		if ((rc = grow(resize, out->scratch_user, dtu_sample_scratch_bytes(F), buf, "dtu sample scratch")) != RGS_OK ||
+		    (rc = cuda_status(launch_dtu_sample_count(V, vertices, F, faces, density, buf, totals, s), "dtu sample")) != RGS_OK)
+			return rc;
+		if (V + totals[0] > INT32_MAX)
+			return fail(RGS_E_INVALID, "dtu sample: more than 2^31 - 1 points (or a face index outside [0, V), or a triangle whose sample count is not finite)");
+	}
+	out->num_points = V + totals[0];
+	char *rows = nullptr, *pts;
+	if ((totals[0] > 0 && (rc = grow(resize, out->rows_user, dtu_sample_rows_bytes(totals[1]), rows, "dtu sample")) != RGS_OK) ||
+	    (rc = grow(resize, out->points_user, (size_t)out->num_points * 3 * sizeof(double), pts, "dtu sample")) != RGS_OK)
+		return rc;
+	if (out->num_points == 0) return RGS_OK;
+	return cuda_status(launch_dtu_sample_emit(V, vertices, F, faces, density, buf, totals[0], totals[1], rows, reinterpret_cast<double*>(pts), s), "dtu sample", kNonFinitePoint);
+}
+
+int32_t rgs_dtu_radius_downsample(int64_t N, const double* points, double radius, uint8_t* kept, int32_t* rounds, rgs_resize_fn scratch,
+                                  void* scratch_user, void* cuda_stream) {
+	if (rounds) *rounds = 0;
+	if (N < 0 || N > INT32_MAX) return fail(RGS_E_INVALID, "dtu downsample: point count out of range");
+	if (!(std::isfinite(radius) && radius > 0.0)) return fail(RGS_E_INVALID, "dtu downsample: radius must be positive and finite");
+	if (N == 0) return RGS_OK;
+	if (!points || !kept || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, dtu_downsample_scratch_bytes((int)N), buf, "dtu downsample scratch")) return rc;
+	return cuda_status(launch_dtu_downsample((int)N, points, radius, kept, buf, rounds, (cudaStream_t)cuda_stream), "dtu downsample", kNonFinitePoint);
+}
+
+int32_t rgs_dtu_nearest(int64_t M, const double* reference, int64_t N, const double* query, double* dist, int64_t* index, rgs_resize_fn scratch,
+                        void* scratch_user, void* cuda_stream) {
+	if (M < 0 || N < 0 || M > INT32_MAX || N > INT32_MAX) return fail(RGS_E_INVALID, "dtu nearest: point count out of range");
+	if (M == 0) return fail(RGS_E_INVALID, "dtu nearest: the reference set is empty");
+	if (!reference || !scratch || (N > 0 && (!query || !dist || !index))) return fail(RGS_E_INVALID, "null pointer");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, dtu_nearest_scratch_bytes((int)M, (int)N), buf, "dtu nearest scratch")) return rc;
+	return cuda_status(launch_dtu_nearest((int)M, reference, (int)N, query, dist, index, buf, (cudaStream_t)cuda_stream), "dtu nearest", kNonFinitePoint);
+}
+
+int32_t rgs_dtu_dilate_masks(int32_t n_views, int32_t H, int32_t W, const uint8_t* masks, uint8_t* dilated, void* cuda_stream) {
+	if (n_views < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "dtu dilate: image size must be positive");
+	if (n_views > 0 && (!masks || !dilated)) return fail(RGS_E_INVALID, "null pointer");
+	const int64_t n = (int64_t)n_views * H * W;
+	if (n == 0) return RGS_OK;
+	dilate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(n_views, H, W, masks, dilated);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "dtu dilate", kNonFinitePoint);
+}
+
+int32_t rgs_dtu_cull_vertices(int64_t V, const double* vertices, int32_t n_views, int32_t H, int32_t W, const double* proj, const uint8_t* dilated,
+                              uint8_t* keep, void* cuda_stream) {
+	if (V < 0 || n_views < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "dtu cull: negative count or empty image");
+	if (V > 0 && (!vertices || !keep || (n_views > 0 && (!proj || !dilated)))) return fail(RGS_E_INVALID, "null pointer");
+	if (V == 0) return RGS_OK;
+	cull_kernel<<<(unsigned)((V + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(V, vertices, n_views, H, W, proj, dilated, keep);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "dtu cull", kNonFinitePoint);
+}
+
+}  // extern "C"

@@ -13,6 +13,8 @@
 //       (coordinate) maps.  Gradients are gathered through shared memory, so the result is deterministic.
 //
 // All maps are planar fp32 [C,H,W] as the rasterizer writes them.  Scalar sums are accumulated in double.
+//
+// This file also holds the C-ABI entry points rgs_ssim_l1_* and rgs_normal_consistency (include/rgs_b200.h).
 #include "rgs_common.cuh"
 
 namespace rgs {
@@ -298,36 +300,70 @@ Window make_window() {
 
 }  // namespace
 
-void launch_ssim_l1_forward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, float* dmaps, double* sums,
-                            cudaStream_t s) {
+}  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+int32_t rgs_ssim_l1_forward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt, float* dmaps,
+                                 double* sums, void* cuda_stream) {
+	if (planes < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");
+	if (row_lo < 0 || row_hi > H || row_lo > row_hi) return fail(RGS_E_INVALID, "row range out of the image");
+	if (!img || !gt || !sums) return fail(RGS_E_INVALID, "null pointer");
+	if (planes > 65535) return fail(RGS_E_INVALID, "too many image planes");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
 	cudaMemsetAsync(sums, 0, 2 * sizeof(double), s);
-	if (row_hi <= row_lo) return;
-	const int by0 = row_lo / TH, by1 = (row_hi + TH - 1) / TH;
-	const dim3 grid((W + TW - 1) / TW, by1 - by0, planes);
-	ssim_l1_forward_kernel<<<grid, 256, 0, s>>>(H, W, row_lo, row_hi, by0, make_window(), img, gt, dmaps, (size_t)planes * H * W, sums);
-	count_launch();
+	if (row_hi > row_lo) {
+		const int by0 = row_lo / TH, by1 = (row_hi + TH - 1) / TH;
+		const dim3 grid((W + TW - 1) / TW, by1 - by0, planes);
+		ssim_l1_forward_kernel<<<grid, 256, 0, s>>>(H, W, row_lo, row_hi, by0, make_window(), img, gt, dmaps, (size_t)planes * H * W, sums);
+		count_launch();
+	}
+	return cuda_status(cudaGetLastError(), "ssim l1 forward");
 }
 
-void launch_ssim_l1_backward(int planes, int H, int W, int row_lo, int row_hi, const float* img, const float* gt, const float* dmaps, float w_ssim,
-                             float w_l1, const float* upstream, float* d_img, cudaStream_t s) {
-	if (row_hi <= row_lo) return;
-	const int by0 = max(0, row_lo - SR) / TH, by1 = (min(H, row_hi + SR) + TH - 1) / TH;
-	const dim3 grid((W + TW - 1) / TW, by1 - by0, planes);
-	ssim_l1_backward_kernel<<<grid, 256, 0, s>>>(H, W, row_lo, row_hi, by0, make_window(), img, gt, dmaps, (size_t)planes * H * W, w_ssim, w_l1, upstream,
-	                                             d_img);
-	count_launch();
+int32_t rgs_ssim_l1_backward_rows(int32_t planes, int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, const float* img, const float* gt,
+                                  const float* dmaps, float w_ssim, float w_l1, const float* upstream, float* d_img, void* cuda_stream) {
+	if (planes < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");
+	if (row_lo < 0 || row_hi > H || row_lo > row_hi) return fail(RGS_E_INVALID, "row range out of the image");
+	if (!img || !gt || !dmaps || !d_img) return fail(RGS_E_INVALID, "null pointer");
+	if (planes > 65535) return fail(RGS_E_INVALID, "too many image planes");
+	if (row_hi > row_lo) {
+		const int by0 = max(0, row_lo - SR) / TH, by1 = (min(H, row_hi + SR) + TH - 1) / TH;
+		const dim3 grid((W + TW - 1) / TW, by1 - by0, planes);
+		ssim_l1_backward_kernel<<<grid, 256, 0, (cudaStream_t)cuda_stream>>>(H, W, row_lo, row_hi, by0, make_window(), img, gt, dmaps, (size_t)planes * H * W,
+		                                                                     w_ssim, w_l1, upstream, d_img);
+		count_launch();
+	}
+	return cuda_status(cudaGetLastError(), "ssim l1 backward");
 }
 
-void launch_normal_consistency(int H, int W, bool from_depth, float inv_fx, float inv_fy, float cx, float cy, const float* rendered_normal,
-                               const float* map_e, const float* map_m, float w_e, float w_m, double* loss_sum, float* d_normal, float* d_e, float* d_m,
-                               cudaStream_t s) {
+int32_t rgs_ssim_l1_forward(int32_t planes, int32_t H, int32_t W, const float* img, const float* gt, float* dmaps, double* sums, void* cuda_stream) {
+	return rgs_ssim_l1_forward_rows(planes, H, W, 0, H, img, gt, dmaps, sums, cuda_stream);
+}
+
+int32_t rgs_ssim_l1_backward(int32_t planes, int32_t H, int32_t W, const float* img, const float* gt, const float* dmaps, float w_ssim, float w_l1,
+                             const float* upstream, float* d_img, void* cuda_stream) {
+	return rgs_ssim_l1_backward_rows(planes, H, W, 0, H, img, gt, dmaps, w_ssim, w_l1, upstream, d_img, cuda_stream);
+}
+
+int32_t rgs_normal_consistency(int32_t H, int32_t W, int32_t from_depth, float inv_fx, float inv_fy, float cx, float cy, const float* rendered_normal,
+                               const float* map_expected, const float* map_median, float w_expected, float w_median, double* loss_sum,
+                               float* d_normal, float* d_expected, float* d_median, void* cuda_stream) {
+	if (H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");
+	if (!rendered_normal || !map_expected || !map_median || !loss_sum || !d_normal || !d_expected || !d_median) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
 	cudaMemsetAsync(loss_sum, 0, sizeof(double), s);
 	const dim3 grid((W + NT - 1) / NT, (H + NT - 1) / NT);
 	if (from_depth)
-		normal_consistency_kernel<true><<<grid, 256, 0, s>>>(H, W, inv_fx, inv_fy, cx, cy, rendered_normal, map_e, map_m, w_e, w_m, loss_sum, d_normal, d_e, d_m);
+		normal_consistency_kernel<true><<<grid, 256, 0, s>>>(H, W, inv_fx, inv_fy, cx, cy, rendered_normal, map_expected, map_median, w_expected, w_median,
+		                                                     loss_sum, d_normal, d_expected, d_median);
 	else
-		normal_consistency_kernel<false><<<grid, 256, 0, s>>>(H, W, inv_fx, inv_fy, cx, cy, rendered_normal, map_e, map_m, w_e, w_m, loss_sum, d_normal, d_e, d_m);
+		normal_consistency_kernel<false><<<grid, 256, 0, s>>>(H, W, inv_fx, inv_fy, cx, cy, rendered_normal, map_expected, map_median, w_expected, w_median,
+		                                                      loss_sum, d_normal, d_expected, d_median);
 	count_launch();
+	return cuda_status(cudaGetLastError(), "normal consistency");
 }
 
-}  // namespace rgs
+}  // extern "C"

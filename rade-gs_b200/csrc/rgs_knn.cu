@@ -18,6 +18,8 @@
 //      below that lane's third-best.  A visited leaf is loaded once (one point per lane) and broadcast with shuffles.
 //      The traversal stack lives one entry per lane in a register (entry k in lane k), so it needs no local memory;
 //      its depth is bounded by the tree height, at most 26 for P < 2^31.
+//
+// This file also holds the C-ABI entry points rgs_knn_mean_dist2 (include/rgs_b200.h).
 #include <algorithm>
 
 #include <cub/cub.cuh>
@@ -307,8 +309,6 @@ KnnScratch carve_knn(char* base, int P, size_t* total) {
 	return k;
 }
 
-}  // namespace
-
 size_t knn_scratch_bytes(int P) {
 	size_t total = 0;
 	carve_knn(nullptr, P, &total);
@@ -348,4 +348,20 @@ cudaError_t launch_knn_mean_dist2(int P, const float* points, float* out, char* 
 	return cudaGetLastError();
 }
 
+}  // namespace
 }  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+int32_t rgs_knn_mean_dist2(int32_t P, const float* points, float* mean_dist2, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (P < 0) return fail(RGS_E_INVALID, "negative point count");
+	if (P == 0) return RGS_OK;
+	if (!points || !mean_dist2 || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, knn_scratch_bytes(P), buf, "knn scratch")) return rc;
+	return cuda_status(launch_knn_mean_dist2(P, points, mean_dist2, buf, (cudaStream_t)cuda_stream), "knn");
+}
+
+}  // extern "C"

@@ -13,6 +13,9 @@
 // groups (SBO) is 128 bytes and the stride between the two K halves of one k8 step (LBO) is rows * 16 bytes.  Stage
 // kt - 2 is refilled only after the barrier of iteration kt, when every warpgroup has retired its wgmma of kt - 2
 // (wgmma.wait_group 1 at the end of each iteration).
+//
+// This file also holds the C-ABI entry points rgs_lpips_* (include/rgs_b200.h).
+#include <algorithm>
 #include <cmath>
 
 #include "rgs_common.cuh"
@@ -346,35 +349,70 @@ cudaError_t launch_conv(int H, int W, int Cin, int Cout, const float* in, const 
 	return cudaGetLastError();
 }
 
+int lpips_distance_blocks(int HW) { return (HW + LD_PIX_PER_CTA - 1) / LD_PIX_PER_CTA; }   // fp64 partial sums the distance of one layer writes
+
 template <int C>
 void launch_distance_c(int HW, const float* feats, const float* lin, float* map, double* partial, cudaStream_t s) {
 	lpips_distance_kernel<C><<<lpips_distance_blocks(HW), LD_WARPS * 32, 0, s>>>(HW, feats, lin, map, partial);
 }
 
+// the activation sizes every LPIPS stage accepts: [2, H, W, C] with 2 H W C < 2^31 elements
+int lpips_size(int32_t H, int32_t W, int64_t C, int32_t min_side, const char* what) {
+	if (H < min_side || W < min_side)
+		return fail(RGS_E_INVALID, std::string(what) + ": the image must be at least " + std::to_string(min_side) + " x " + std::to_string(min_side) +
+		                               " pixels, got " + std::to_string(H) + " x " + std::to_string(W));
+	if ((int64_t)H * W * C * 2 > INT32_MAX) return fail(RGS_E_INVALID, std::string(what) + ": the activations exceed 2^31 elements");
+	return RGS_OK;
+}
+
 }  // namespace
+}  // namespace rgs
 
-int lpips_distance_blocks(int HW) { return (HW + LD_PIX_PER_CTA - 1) / LD_PIX_PER_CTA; }
+using namespace rgs;
 
-cudaError_t launch_lpips_input_conv(int H, int W, const float* x, const float* y, const float* weight, const float* bias, float* out, cudaStream_t s) {
-	lpips_input_conv_kernel<<<dim3((H * W + 127) / 128, 2), 128, 0, s>>>(H, W, x, y, weight, bias, out);
+extern "C" {
+
+int32_t rgs_lpips_input_conv(int32_t H, int32_t W, const float* x, const float* y, const float* weight, const float* bias, float* out, void* cuda_stream) {
+	if (const int rc = lpips_size(H, W, 64, 16, "lpips input conv")) return rc;
+	if (!x || !y || !weight || !bias || !out) return fail(RGS_E_INVALID, "null pointer");
+	lpips_input_conv_kernel<<<dim3((H * W + 127) / 128, 2), 128, 0, (cudaStream_t)cuda_stream>>>(H, W, x, y, weight, bias, out);
 	count_launch();
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "lpips input conv");
 }
 
-cudaError_t launch_lpips_conv3x3(int H, int W, int Cin, int Cout, const float* in, const float* weight, const float* bias, float* out, cudaStream_t s) {
-	return Cout % 128 == 0 ? launch_conv<128>(H, W, Cin, Cout, in, weight, bias, out, s) : launch_conv<64>(H, W, Cin, Cout, in, weight, bias, out, s);
+int32_t rgs_lpips_conv3x3(int32_t H, int32_t W, int32_t C_in, int32_t C_out, const float* in, const float* weight, const float* bias, float* out,
+                          void* cuda_stream) {
+	if (C_in <= 0 || C_in % 32 || C_in > 512 || C_out <= 0 || C_out % 64 || C_out > 512)
+		return fail(RGS_E_INVALID, "lpips conv3x3: C_in must be a multiple of 32 and C_out of 64, both at most 512");
+	if (const int rc = lpips_size(H, W, std::max(C_in, C_out), 1, "lpips conv3x3")) return rc;
+	if (!in || !weight || !bias || !out) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	return cuda_status(C_out % 128 == 0 ? launch_conv<128>(H, W, C_in, C_out, in, weight, bias, out, s) : launch_conv<64>(H, W, C_in, C_out, in, weight, bias, out, s),
+	                   "lpips conv3x3");
 }
 
-cudaError_t launch_lpips_maxpool(int H, int W, int C, const float* in, float* out, cudaStream_t s) {
+int32_t rgs_lpips_maxpool(int32_t H, int32_t W, int32_t C, const float* in, float* out, void* cuda_stream) {
+	if (C <= 0 || C % 4) return fail(RGS_E_INVALID, "lpips maxpool: C must be a positive multiple of 4");
+	if (const int rc = lpips_size(H, W, C, 2, "lpips maxpool")) return rc;
+	if (!in || !out) return fail(RGS_E_INVALID, "null pointer");
 	const int64_t total = (int64_t)2 * (H / 2) * (W / 2) * (C / 4);
 	if (total > 0) {
-		lpips_maxpool_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(H, W, C, in, out);
+		lpips_maxpool_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(H, W, C, in, out);
 		count_launch();
 	}
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "lpips maxpool");
 }
 
-cudaError_t launch_lpips_distance(int HW, int C, const float* feats, const float* lin, float* map, double* partial, double* mean, cudaStream_t s) {
+int32_t rgs_lpips_distance(int32_t H, int32_t W, int32_t C, const float* feats, const float* lin, float* map, double* mean, rgs_resize_fn resize,
+                           void* scratch_user, void* cuda_stream) {
+	if (C != 64 && C != 128 && C != 256 && C != 512) return fail(RGS_E_INVALID, "lpips distance: C must be 64, 128, 256 or 512");
+	if (const int rc = lpips_size(H, W, C, 1, "lpips distance")) return rc;
+	if (!feats || !lin || !map || !mean || !resize) return fail(RGS_E_INVALID, "null pointer");
+	const int HW = H * W;
+	char* buf = nullptr;
+	if (const int rc = grow(resize, scratch_user, sizeof(double) * lpips_distance_blocks(HW), buf, "lpips distance scratch")) return rc;
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	double* partial = reinterpret_cast<double*>(buf);
 	switch (C) {
 		case 64: launch_distance_c<64>(HW, feats, lin, map, partial, s); break;
 		case 128: launch_distance_c<128>(HW, feats, lin, map, partial, s); break;
@@ -383,7 +421,7 @@ cudaError_t launch_lpips_distance(int HW, int C, const float* feats, const float
 	}
 	lpips_mean_kernel<<<1, LM_THREADS, 0, s>>>(lpips_distance_blocks(HW), HW, partial, mean);
 	count_launch(2);
-	return cudaGetLastError();
+	return cuda_status(cudaGetLastError(), "lpips distance");
 }
 
-}  // namespace rgs
+}  // extern "C"

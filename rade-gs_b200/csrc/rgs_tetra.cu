@@ -14,6 +14,8 @@
 //              the vertices and the faces, one thread each.
 //   bisect     one thread per vertex.
 //   filter     one thread per vertex / face, a scan of the kept vertices and CUB's stable select of vertices and faces.
+//
+// This file also holds the C-ABI entry points rgs_tetra_* (include/rgs_b200.h).
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 
@@ -303,28 +305,7 @@ int bits_for(int64_t n) {   // bits to hold every value in [0, n)
 	return b;
 }
 
-}  // namespace
-
 // ---- launchers ----------------------------------------------------------------------------------------------------------
-
-cudaError_t launch_tetra_points(int P, const float* xyz, const float* scaling, const float* rotation, float* points, float* scales, cudaStream_t s) {
-	tetra_points_kernel<<<(unsigned)((P + 255) / 256), 256, 0, s>>>(P, xyz, scaling, rotation, points, scales);
-	count_launch();
-	return cudaGetLastError();
-}
-
-cudaError_t launch_tetra_cull_add(int64_t N, const float* alpha, const float* coord, int H, int W, const float* render7, const float* gt_mask, float* fin,
-                                  int32_t* weight, cudaStream_t s) {
-	tetra_cull_add_kernel<<<(unsigned)((N + 255) / 256), 256, 0, s>>>(N, alpha, coord, H, W, render7, gt_mask, fin, weight);
-	count_launch();
-	return cudaGetLastError();
-}
-
-cudaError_t launch_tetra_cull_finish(int64_t N, const float* fin, const int32_t* weight, float* sdf, cudaStream_t s) {
-	tetra_cull_finish_kernel<<<(unsigned)((N + 255) / 256), 256, 0, s>>>(N, fin, weight, sdf);
-	count_launch();
-	return cudaGetLastError();
-}
 
 // Phase 1 (sized by T): codes, valid flags, the valid tet ids and the select's temp.
 struct TetScratch1 {
@@ -460,12 +441,6 @@ cudaError_t launch_tetra_march_emit(int64_t T, const float* points, const float*
 	return cudaGetLastError();
 }
 
-cudaError_t launch_tetra_bisect(int64_t M, const float* mid_sdf, float* left, float* right, float* left_sdf, float* right_sdf, float* mid, cudaStream_t s) {
-	tetra_bisect_kernel<<<(unsigned)((M + 255) / 256), 256, 0, s>>>(M, mid_sdf, left, right, left_sdf, right_sdf, mid);
-	count_launch();
-	return cudaGetLastError();
-}
-
 struct FilterScratch {
 	int32_t *keep, *excl;
 	uint8_t* fkeep;
@@ -527,4 +502,113 @@ cudaError_t launch_tetra_filter(int M, const float* points, const float* ends, c
 	return cudaGetLastError();
 }
 
+}  // namespace
 }  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+int32_t rgs_tetra_points(int64_t P, const float* xyz, const float* scaling, const float* rotation, float* points, float* scales, void* cuda_stream) {
+	if (P < 0 || 9 * P > INT32_MAX) return fail(RGS_E_INVALID, "tetra points: Gaussian count out of range");
+	if (P == 0) return RGS_OK;
+	if (!xyz || !scaling || !rotation || !points || !scales) return fail(RGS_E_INVALID, "null pointer");
+	tetra_points_kernel<<<(unsigned)((P + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>((int)P, xyz, scaling, rotation, points, scales);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "tetra points");
+}
+
+int32_t rgs_tetra_cull_add(int64_t N, const float* alpha, const float* coord, int32_t H, int32_t W, const float* render7, const float* gt_mask,
+                           float* final_alpha, int32_t* weight, void* cuda_stream) {
+	if (N < 0 || H <= 0 || W <= 0) return fail(RGS_E_INVALID, "tetra cull: negative point count or empty image");
+	if (N == 0) return RGS_OK;
+	if (!alpha || !coord || !render7 || !final_alpha || !weight) return fail(RGS_E_INVALID, "null pointer");
+	tetra_cull_add_kernel<<<(unsigned)((N + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(N, alpha, coord, H, W, render7, gt_mask, final_alpha, weight);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "tetra cull");
+}
+
+int32_t rgs_tetra_cull_finish(int64_t N, const float* final_alpha, const int32_t* weight, float* sdf, void* cuda_stream) {
+	if (N < 0) return fail(RGS_E_INVALID, "tetra cull: negative point count");
+	if (N == 0) return RGS_OK;
+	if (!final_alpha || !weight || !sdf) return fail(RGS_E_INVALID, "null pointer");
+	tetra_cull_finish_kernel<<<(unsigned)((N + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(N, final_alpha, weight, sdf);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "tetra cull finish");
+}
+
+int32_t rgs_tetra_marching(int64_t N, const float* points, const float* sdf, const float* scales, int64_t T, const int64_t* tets, rgs_resize_fn resize,
+                           rgs_tetra_march_out* out, void* cuda_stream) {
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	out->num_vertices = out->num_faces = 0;
+	if (N < 0 || N > INT32_MAX || T < 0 || T > INT32_MAX) return fail(RGS_E_INVALID, "tetra marching: point or tet count out of range");
+	if ((N > 0 && (!points || !sdf || !scales)) || (T > 0 && !tets)) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int rc;
+	int32_t V = 0, M = 0, F = 0;
+	char* s1 = nullptr;
+	if (T > 0) {
+		int32_t bad = 0;
+		if ((rc = grow(resize, out->scratch_user, tetra_march_scratch1_bytes(T), s1, "tetra marching scratch")) != RGS_OK ||
+		    (rc = cuda_status(launch_tetra_march_valid(T, N, tets, sdf, s1, &bad, &V, s), "tetra marching")) != RGS_OK)
+			return rc;
+		if (bad) return fail(RGS_E_INVALID, "tetra marching: a tet index lies outside [0, N)");
+		if (V > (INT32_MAX - 255) / 6) return fail(RGS_E_INVALID, "tetra marching: too many valid tets (6 x valid must stay below 2^31)");
+	}
+	char* s2 = nullptr;
+	if (V > 0) {
+		if ((rc = grow(resize, out->sort_user, tetra_march_scratch2_bytes(V), s2, "tetra marching scratch")) != RGS_OK ||
+		    (rc = cuda_status(launch_tetra_march_sort(T, N, tets, sdf, V, s1, s2, &M, &F, s), "tetra marching")) != RGS_OK)
+			return rc;
+	}
+	char *interp, *ends, *end_sdf, *end_scl, *faces;
+	if ((rc = grow(resize, out->interp_user, (size_t)M * 2 * sizeof(int64_t), interp, "tetra marching")) != RGS_OK ||
+	    (rc = grow(resize, out->ends_user, (size_t)M * 6 * sizeof(float), ends, "tetra marching")) != RGS_OK ||
+	    (rc = grow(resize, out->end_sdf_user, (size_t)M * 2 * sizeof(float), end_sdf, "tetra marching")) != RGS_OK ||
+	    (rc = grow(resize, out->end_scales_user, (size_t)M * 2 * sizeof(float), end_scl, "tetra marching")) != RGS_OK ||
+	    (rc = grow(resize, out->faces_user, (size_t)F * 3 * sizeof(int64_t), faces, "tetra marching")) != RGS_OK)
+		return rc;
+	out->num_vertices = M;
+	out->num_faces = F;
+	if (V == 0) return RGS_OK;
+	return cuda_status(launch_tetra_march_emit(T, points, sdf, scales, V, s1, s2, N, reinterpret_cast<int64_t*>(interp), reinterpret_cast<float*>(ends),
+	                                          reinterpret_cast<float*>(end_sdf), reinterpret_cast<float*>(end_scl), reinterpret_cast<int64_t*>(faces), s),
+	                  "tetra marching");
+}
+
+int32_t rgs_tetra_bisect(int64_t M, const float* mid_sdf, float* left, float* right, float* left_sdf, float* right_sdf, float* mid, void* cuda_stream) {
+	if (M < 0) return fail(RGS_E_INVALID, "tetra bisect: negative vertex count");
+	if (M == 0) return RGS_OK;
+	if (!left || !right || !mid || (mid_sdf && (!left_sdf || !right_sdf))) return fail(RGS_E_INVALID, "null pointer");
+	tetra_bisect_kernel<<<(unsigned)((M + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(M, mid_sdf, left, right, left_sdf, right_sdf, mid);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "tetra bisect");
+}
+
+int32_t rgs_tetra_filter(int64_t M, const float* points, const float* ends, const float* end_scales, int64_t F, const int64_t* faces, rgs_resize_fn resize,
+                         rgs_tetra_filter_out* out, void* cuda_stream) {
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	out->num_vertices = out->num_faces = 0;
+	if (M < 0 || M > INT32_MAX || F < 0 || F > INT32_MAX) return fail(RGS_E_INVALID, "tetra filter: vertex or face count out of range");
+	if ((M > 0 && (!points || !ends || !end_scales)) || (F > 0 && !faces)) return fail(RGS_E_INVALID, "null pointer");
+	if (M == 0 && F > 0) return fail(RGS_E_INVALID, "tetra filter: faces without vertices");
+	char *verts, *fout, *buf;
+	int rc;
+	if ((rc = grow(resize, out->vertices_user, (size_t)M * 3 * sizeof(float), verts, "tetra filter")) != RGS_OK ||
+	    (rc = grow(resize, out->faces_user, (size_t)F * 3 * sizeof(int64_t), fout, "tetra filter")) != RGS_OK)
+		return rc;
+	if (M == 0) return RGS_OK;
+	int64_t nv = 0, nf = 0;
+	int32_t bad = 0;
+	if ((rc = grow(resize, out->scratch_user, tetra_filter_scratch_bytes((int)M, F), buf, "tetra filter scratch")) != RGS_OK ||
+	    (rc = cuda_status(launch_tetra_filter((int)M, points, ends, end_scales, F, faces, buf, reinterpret_cast<float*>(verts),
+	                                          reinterpret_cast<int64_t*>(fout), &nv, &nf, &bad, (cudaStream_t)cuda_stream),
+	                      "tetra filter")) != RGS_OK)
+		return rc;
+	if (bad) return fail(RGS_E_INVALID, "tetra filter: a face index lies outside [0, M)");
+	out->num_vertices = nv;
+	out->num_faces = nf;
+	return RGS_OK;
+}
+
+}  // extern "C"

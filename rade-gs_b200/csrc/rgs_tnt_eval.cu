@@ -13,6 +13,8 @@
 //              holds one warp and the launch keeps going around it.
 //   moments    two passes (sums, then centred sums), each a fixed tree: 1024 points per block, 4 per thread in a fixed
 //              order, a shared-memory halving tree, then one block over the partials.  The launch shape depends on N only.
+//
+// This file also holds the C-ABI entry points rgs_tnt_* (include/rgs_b200.h).
 #include <cub/cub.cuh>
 
 #include "rgs_common.cuh"
@@ -325,8 +327,6 @@ __global__ void __launch_bounds__(MOM_THREADS) tnt_mom_final_kernel(int64_t P, c
 	}
 }
 
-}  // namespace
-
 static Xform make_xform(const double* T) {
 	Xform x;
 	for (int k = 0; k < 12; k++) x.m[k] = T ? T[k] : 0.0;
@@ -385,13 +385,6 @@ cudaError_t launch_tnt_crop(int N, const double* pts, const double* xform, int a
 	RGS_TRY(cudaStreamSynchronize(s));
 	*num_kept = (int64_t)h[0];
 	if (h[1]) return cudaErrorInvalidValue;
-	return cudaGetLastError();
-}
-
-cudaError_t launch_tnt_transform(int64_t N, double* pts, const double* xform, cudaStream_t s) {
-	if (N == 0) return cudaSuccess;
-	tnt_xform_kernel<<<(unsigned)((N + 255) / 256), 256, 0, s>>>(N, pts, make_xform(xform));
-	count_launch();
 	return cudaGetLastError();
 }
 
@@ -510,4 +503,99 @@ cudaError_t launch_tnt_moments(int64_t N, const double* src, int64_t M, const do
 	return cudaGetLastError();
 }
 
+}  // namespace
 }  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+static int tnt_check_transform(const double* T, const char* what) {
+	if (!T) return RGS_OK;
+	for (int k = 0; k < 16; k++)
+		if (!std::isfinite(T[k])) return fail(RGS_E_INVALID, std::string(what) + ": the transform has a NaN or infinite entry");
+	if (T[12] != 0.0 || T[13] != 0.0 || T[14] != 0.0 || T[15] != 1.0) return fail(RGS_E_INVALID, std::string(what) + ": the transform's last row must be (0 0 0 1)");
+	return RGS_OK;
+}
+
+int32_t rgs_tnt_crop(int64_t N, const double* points, const double* transform, const rgs_tnt_crop_volume* volume, uint8_t* kept, double* cropped,
+                     int64_t* num_kept, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (N < 0 || N > INT32_MAX) return fail(RGS_E_INVALID, "tnt crop: point count out of range");
+	if (!num_kept) return fail(RGS_E_INVALID, "null pointer");
+	*num_kept = 0;
+	if (const int rc = tnt_check_transform(transform, "tnt crop")) return rc;
+	if (volume) {
+		if (volume->orthogonal_axis < 0 || volume->orthogonal_axis > 2) return fail(RGS_E_INVALID, "tnt crop: orthogonal_axis must be 0, 1 or 2");
+		if (volume->num_vertices < 3 || volume->num_vertices > 2048) return fail(RGS_E_INVALID, "tnt crop: the polygon needs 3 to 2048 vertices");
+		if (!volume->polygon) return fail(RGS_E_INVALID, "null pointer");
+		if (std::isnan(volume->axis_min) || std::isnan(volume->axis_max)) return fail(RGS_E_INVALID, "tnt crop: axis_min / axis_max is NaN");
+	}
+	if (N == 0) return RGS_OK;
+	if (!points || !kept || !cropped || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, tnt_crop_scratch_bytes((int)N), buf, "tnt crop scratch")) return rc;
+	const cudaError_t e = launch_tnt_crop((int)N, points, transform, volume ? volume->orthogonal_axis : 0, volume ? volume->axis_min : 0.0,
+	                                      volume ? volume->axis_max : 0.0, volume ? volume->num_vertices : 0, volume ? volume->polygon : nullptr, kept,
+	                                      cropped, num_kept, buf, (cudaStream_t)cuda_stream);
+	return cuda_status(e, "tnt crop", kNonFinitePoint);
+}
+
+int32_t rgs_tnt_transform(int64_t N, double* points, const double* transform, void* cuda_stream) {
+	if (N < 0 || N > INT32_MAX) return fail(RGS_E_INVALID, "tnt transform: point count out of range");
+	if (!transform) return fail(RGS_E_INVALID, "null pointer");
+	if (const int rc = tnt_check_transform(transform, "tnt transform")) return rc;
+	if (N > 0 && !points) return fail(RGS_E_INVALID, "null pointer");
+	if (N == 0) return RGS_OK;
+	tnt_xform_kernel<<<(unsigned)((N + 255) / 256), 256, 0, (cudaStream_t)cuda_stream>>>(N, points, make_xform(transform));
+	count_launch();
+	return cuda_status(cudaGetLastError(), "tnt transform", kNonFinitePoint);
+}
+
+int32_t rgs_tnt_voxel_downsample(int64_t N, const double* points, double voxel, rgs_resize_fn resize, rgs_tnt_voxel_out* out, void* cuda_stream) {
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	out->num_voxels = 0;
+	if (N < 0 || N > INT32_MAX) return fail(RGS_E_INVALID, "tnt voxel: point count out of range");
+	if (!(std::isfinite(voxel) && voxel > 0.0)) return fail(RGS_E_INVALID, "tnt voxel: voxel size must be positive and finite");
+	if (N > 0 && !points) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int rc;
+	double lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0}, origin[3] = {0, 0, 0};
+	if (N > 0) {
+		char* bbuf;
+		int64_t bad = 0;
+		if ((rc = grow(resize, out->scratch_user, tnt_bounds_scratch_bytes(), bbuf, "tnt voxel scratch")) != RGS_OK ||
+		    (rc = cuda_status(launch_tnt_bounds((int)N, points, bbuf, lo, hi, &bad, s), "tnt voxel")) != RGS_OK)
+			return rc;
+		if (bad) return fail(RGS_E_INVALID, "tnt voxel: a point has a NaN or infinite coordinate");
+		for (int a = 0; a < 3; a++) {
+			origin[a] = lo[a] - voxel * 0.5;
+			const double top = std::floor((hi[a] - origin[a]) / voxel);
+			if (!(top < 2097152.0)) return fail(RGS_E_INVALID, "tnt voxel: more than 2^21 voxels along an axis");
+		}
+	}
+	char* buf = nullptr;
+	int32_t V = 0;
+	if (N > 0 && ((rc = grow(resize, out->scratch_user, tnt_voxel_scratch_bytes((int)N), buf, "tnt voxel scratch")) != RGS_OK ||
+	              (rc = cuda_status(launch_tnt_voxel_sort((int)N, points, origin, voxel, buf, &V, s), "tnt voxel")) != RGS_OK))
+		return rc;
+	out->num_voxels = V;
+	char *means, *counts;
+	if ((rc = grow(resize, out->means_user, (size_t)V * 3 * sizeof(double), means, "tnt voxel")) != RGS_OK ||
+	    (rc = grow(resize, out->counts_user, (size_t)V * sizeof(int64_t), counts, "tnt voxel")) != RGS_OK)
+		return rc;
+	if (V == 0) return RGS_OK;
+	return cuda_status(launch_tnt_voxel_mean((int)N, points, V, buf, reinterpret_cast<double*>(means), reinterpret_cast<int64_t*>(counts), s), "tnt voxel", kNonFinitePoint);
+}
+
+int32_t rgs_tnt_icp_moments(int64_t N, const double* source, int64_t M, const double* target, const double* dist, const int64_t* index, double threshold,
+                            double* moments, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (N < 0 || M < 0 || N > INT32_MAX || M > INT32_MAX) return fail(RGS_E_INVALID, "tnt moments: point count out of range");
+	if (std::isnan(threshold)) return fail(RGS_E_INVALID, "tnt moments: the threshold is NaN");
+	if (!moments || !scratch || (N > 0 && (!source || !dist || !index)) || (M > 0 && !target)) return fail(RGS_E_INVALID, "null pointer");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, tnt_moments_scratch_bytes(N), buf, "tnt moments scratch")) return rc;
+	return cuda_status(launch_tnt_moments(N, source, M, target, dist, index, threshold, buf, moments, (cudaStream_t)cuda_stream), "tnt moments",
+	                   "a point or a distance is NaN or infinite");
+}
+
+}  // extern "C"

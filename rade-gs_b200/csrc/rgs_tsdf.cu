@@ -15,6 +15,8 @@
 //              order and grid capacity.
 //   normals    (vertex, triangle) pairs stably radix-sorted by vertex, so every vertex sums its face normals in ascending
 //              triangle order: no float atomics.
+//
+// This file also holds the C-ABI entry points rgs_tsdf_* (include/rgs_b200.h).
 #include <cub/cub.cuh>
 
 #include "rgs_common.cuh"
@@ -548,9 +550,7 @@ __global__ void __launch_bounds__(256) tsdf_normals_kernel(int64_t V, const floa
 
 unsigned blocks_for(int64_t n) { return (unsigned)((n + 255) / 256); }
 
-}  // namespace
-
-// ---- host launchers (argument checks are in rgs_api.cu) ---------------------------------------------------------------
+// ---- host launchers ----------------------------------------------------------------------------------------------------
 
 Cam make_cam(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c) {
 	Cam k;
@@ -614,12 +614,6 @@ cudaError_t launch_tsdf_integrate(const rgs_tsdf_grid& g, const rgs_tsdf_camera&
 	tsdf_claim_kernel<<<blocks_for(n), 256, 0, s>>>(g, n, bc, call_id, slot);
 	tsdf_integrate_kernel<<<(unsigned)n, INTEGRATE_THREADS, 0, s>>>(g, k, bc, slot, depth, color);
 	count_launch(3);
-	return cudaGetLastError();
-}
-
-cudaError_t launch_tsdf_rehash(const rgs_tsdf_grid& g, const uint64_t* old_keys, const int32_t* old_vals, int64_t old_slots, cudaStream_t s) {
-	tsdf_rehash_kernel<<<blocks_for(old_slots), 256, 0, s>>>(g, old_keys, old_vals, old_slots);
-	count_launch();
 	return cudaGetLastError();
 }
 
@@ -764,4 +758,162 @@ cudaError_t launch_tsdf_normals(int64_t V, const float* verts, int64_t F, const 
 	return cudaGetLastError();
 }
 
+}  // namespace
 }  // namespace rgs
+
+using namespace rgs;
+
+extern "C" {
+
+static bool pow2(int64_t n) { return n > 0 && (n & (n - 1)) == 0; }
+static bool finite_pos(float x) { return std::isfinite(x) && x > 0.0f; }
+
+static int tsdf_grid_check(const rgs_tsdf_grid* g) {
+	if (!g) return fail(RGS_E_INVALID, "null grid");
+	if (!finite_pos(g->voxel_size)) return fail(RGS_E_INVALID, "voxel_size must be positive and finite");
+	if (g->capacity <= 0 || g->capacity > (INT32_MAX / (RGS_TSDF_BLOCK_RES * RGS_TSDF_BLOCK_RES * RGS_TSDF_BLOCK_RES)))
+		return fail(RGS_E_INVALID, "grid capacity must be in [1, 524287] blocks");
+	if (!pow2(g->hash_slots) || g->hash_slots < 2 * g->capacity) return fail(RGS_E_INVALID, "hash_slots must be a power of two >= 2 * capacity");
+	if (!pow2(g->frame_slots) || g->frame_slots < 2 || g->frame_slots > ((int64_t)1 << 31))
+		return fail(RGS_E_INVALID, "frame_slots must be a power of two in [2, 2^31]");
+	if (!g->hash_keys || !g->hash_values || !g->tsdf || !g->weight || !g->color || !g->stamps || !g->frame_keys || !g->frame_list || !g->counters)
+		return fail(RGS_E_INVALID, "null grid array");
+	return RGS_OK;
+}
+
+static int tsdf_camera_check(const rgs_tsdf_grid* g, const rgs_tsdf_camera* c) {
+	if (!c) return fail(RGS_E_INVALID, "null camera");
+	if (c->width <= 0 || c->height <= 0) return fail(RGS_E_INVALID, "image size must be positive");
+	if (!std::isfinite(c->fx) || !std::isfinite(c->fy) || c->fx == 0.0f || c->fy == 0.0f || !std::isfinite(c->cx) || !std::isfinite(c->cy))
+		return fail(RGS_E_INVALID, "intrinsics must be finite with nonzero focal lengths");
+	for (int i = 0; i < 9; i++)
+		if (!std::isfinite(c->R[i])) return fail(RGS_E_INVALID, "extrinsic must be finite");
+	for (int i = 0; i < 3; i++)
+		if (!std::isfinite(c->t[i])) return fail(RGS_E_INVALID, "extrinsic must be finite");
+	if (!finite_pos(c->depth_scale) || !finite_pos(c->depth_max) || !finite_pos(c->trunc_voxel_multiplier))
+		return fail(RGS_E_INVALID, "depth_scale, depth_max and trunc_voxel_multiplier must be positive and finite");
+	// camera centre +- (depth_max + trunc) must stay inside the block-key range (the keys must never wrap)
+	const double reach = (double)c->depth_max + (double)c->trunc_voxel_multiplier * (double)g->voxel_size;
+	const double bs = (double)g->voxel_size * RGS_TSDF_BLOCK_RES;
+	for (int k = 0; k < 3; k++) {
+		const double ck = -((double)c->R[k] * c->t[0] + (double)c->R[3 + k] * c->t[1] + (double)c->R[6 + k] * c->t[2]);
+		const double lo = std::floor((ck - reach) / bs), hi = std::floor((ck + reach) / bs);
+		if (!(lo >= -(1 << 20) + 1 && hi <= (1 << 20) - 2))
+			return fail(RGS_E_INVALID, "camera out of the grid's key range: centre +- (depth_max + trunc) must lie within 2^20 - 2 blocks of the origin");
+	}
+	return RGS_OK;
+}
+
+// counters[0..3] to the host; fails when an earlier call left the grid incomplete
+static int tsdf_read_counters(const rgs_tsdf_grid* g, int32_t* cnt, cudaStream_t s) {
+	cudaError_t e = cudaMemcpyAsync(cnt, g->counters, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+	return cuda_status(e, "tsdf");
+}
+
+static int tsdf_flags_check(const int32_t* cnt) {
+	if (cnt[2] & RGS_TSDF_BAD_COORD) return fail(RGS_E_INVALID, "tsdf: an integrate call was given a block coordinate outside [-2^20, 2^20)");
+	if (cnt[2] & RGS_TSDF_OVERFLOW) return fail(RGS_E_INVALID, "tsdf: an integrate call found no free block slot; the grid is incomplete");
+	return RGS_OK;
+}
+
+int64_t rgs_tsdf_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, const float* depth, int32_t* block_coords, int64_t* allocated,
+                       rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc == RGS_OK) rc = tsdf_camera_check(grid, cam);
+	if (rc != RGS_OK) return rc;
+	if (!depth || !block_coords || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int32_t cnt[4];
+	if ((rc = cuda_status(launch_tsdf_touch(*grid, *cam, depth, cnt, s), "tsdf touch")) != RGS_OK) return rc;
+	if ((rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
+	if (allocated) *allocated = cnt[0];
+	if (cnt[3] || cnt[1] > grid->frame_slots / 2) return fail(RGS_E_CAPACITY, "tsdf touch: more blocks than the frame-local hash holds");
+	const int64_t n = cnt[1];
+	if (n == 0) return 0;
+	char* buf;
+	if ((rc = grow(scratch, scratch_user, tsdf_touch_scratch_bytes(n), buf, "tsdf scratch")) != RGS_OK) return rc;
+	if ((rc = cuda_status(launch_tsdf_touch_sort(*grid, n, block_coords, buf, s), "tsdf touch")) != RGS_OK) return rc;
+	return n;
+}
+
+int32_t rgs_tsdf_integrate(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, int64_t n, const int32_t* block_coords, const float* depth,
+                           const float* color, int32_t call_id, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc == RGS_OK) rc = tsdf_camera_check(grid, cam);
+	if (rc != RGS_OK) return rc;
+	if (n < 0 || n > INT32_MAX) return fail(RGS_E_INVALID, "block count out of range");
+	if (call_id <= 0) return fail(RGS_E_INVALID, "call_id must be positive");
+	if (n == 0) return RGS_OK;
+	if (!block_coords || !depth || !color || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf;
+	if ((rc = grow(scratch, scratch_user, (size_t)n * sizeof(int32_t), buf, "tsdf scratch")) != RGS_OK) return rc;
+	return cuda_status(launch_tsdf_integrate(*grid, *cam, n, block_coords, depth, color, call_id, reinterpret_cast<int32_t*>(buf), (cudaStream_t)cuda_stream),
+	                 "tsdf integrate");
+}
+
+int32_t rgs_tsdf_rehash(const rgs_tsdf_grid* grid, const uint64_t* old_keys, const int32_t* old_values, int64_t old_slots, void* cuda_stream) {
+	const int rc = tsdf_grid_check(grid);
+	if (rc != RGS_OK) return rc;
+	if (old_slots < 0) return fail(RGS_E_INVALID, "negative slot count");
+	if (old_slots == 0) return RGS_OK;
+	if (!old_keys || !old_values) return fail(RGS_E_INVALID, "null pointer");
+	tsdf_rehash_kernel<<<blocks_for(old_slots), 256, 0, (cudaStream_t)cuda_stream>>>(*grid, old_keys, old_values, old_slots);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "tsdf rehash");
+}
+
+int64_t rgs_tsdf_active_blocks(const rgs_tsdf_grid* grid, uint64_t* keys, int32_t* pool_index, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc != RGS_OK) return rc;
+	if (!keys || !pool_index || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int32_t cnt[4];
+	if ((rc = tsdf_read_counters(grid, cnt, s)) != RGS_OK || (rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
+	const int N = cnt[0];
+	if (N == 0) return 0;
+	char* buf;
+	if ((rc = grow(scratch, scratch_user, tsdf_active_scratch_bytes(N), buf, "tsdf scratch")) != RGS_OK) return rc;
+	if ((rc = cuda_status(launch_tsdf_active(*grid, N, keys, pool_index, buf, s), "tsdf active blocks")) != RGS_OK) return rc;
+	return N;
+}
+
+int32_t rgs_tsdf_extract(const rgs_tsdf_grid* grid, float weight_threshold, rgs_resize_fn resize, rgs_tsdf_mesh_out* out, void* scratch_user,
+                         void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc != RGS_OK) return rc;
+	if (!resize || !out) return fail(RGS_E_INVALID, "null pointer");
+	if (std::isnan(weight_threshold)) return fail(RGS_E_INVALID, "weight_threshold is NaN");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	int32_t cnt[4];
+	if ((rc = tsdf_read_counters(grid, cnt, s)) != RGS_OK || (rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
+	const int N = cnt[0];
+	int64_t totals[2] = {0, 0};
+	char* buf = nullptr;
+	if (N > 0) {
+		if ((rc = grow(resize, scratch_user, tsdf_extract_scratch_bytes(*grid, N), buf, "tsdf scratch")) != RGS_OK) return rc;
+		if ((rc = cuda_status(launch_tsdf_extract_count(*grid, N, weight_threshold, buf, totals, s), "tsdf extract")) != RGS_OK) return rc;
+	}
+	out->num_vertices = totals[0];
+	out->num_triangles = totals[1];
+	char *v, *c, *t;
+	if ((rc = grow(resize, out->vertices_user, (size_t)totals[0] * 3 * sizeof(float), v, "tsdf mesh")) != RGS_OK ||
+	    (rc = grow(resize, out->colors_user, (size_t)totals[0] * 3 * sizeof(float), c, "tsdf mesh")) != RGS_OK ||
+	    (rc = grow(resize, out->triangles_user, (size_t)totals[1] * 3 * sizeof(int32_t), t, "tsdf mesh")) != RGS_OK)
+		return rc;
+	if (N == 0) return RGS_OK;
+	return cuda_status(launch_tsdf_extract_emit(*grid, N, buf, reinterpret_cast<float*>(v), reinterpret_cast<float*>(c), reinterpret_cast<int32_t*>(t), s),
+	                 "tsdf extract");
+}
+
+int32_t rgs_tsdf_vertex_normals(int64_t V, const float* vertices, int64_t F, const int32_t* triangles, float* normals, rgs_resize_fn scratch,
+                                void* scratch_user, void* cuda_stream) {
+	if (V < 0 || F < 0 || V > INT32_MAX || 3 * F > INT32_MAX) return fail(RGS_E_INVALID, "vertex / triangle count out of range");
+	if (V == 0) return F == 0 ? (int32_t)RGS_OK : fail(RGS_E_INVALID, "triangles without vertices");
+	if (!vertices || !normals || !scratch || (F > 0 && !triangles)) return fail(RGS_E_INVALID, "null pointer");
+	char* buf;
+	if (const int rc = grow(scratch, scratch_user, tsdf_normals_scratch_bytes(V, F), buf, "tsdf scratch")) return rc;
+	return cuda_status(launch_tsdf_normals(V, vertices, F, triangles, normals, buf, (cudaStream_t)cuda_stream), "tsdf vertex normals");
+}
+
+}  // extern "C"
