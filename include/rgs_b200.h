@@ -733,6 +733,87 @@ int32_t rgs_lpips_maxpool(int32_t H, int32_t W, int32_t C, const float* in, floa
 int32_t rgs_lpips_distance(int32_t H, int32_t W, int32_t C, const float* feats, const float* lin, float* map, double* mean, rgs_resize_fn resize,
                            void* scratch_user, void* cuda_stream);
 
+/* ---- contracted-space TSDF mesh of unbounded scenes (utils/mesh_utils.py:163-271 extract_mesh_unbounded, :23-44
+ *      post_process_mesh; utils/mcube_utils.py:17-95 marching_cubes_with_contraction) ----
+ * Every fp32 value below is one IEEE operation rounded on its own, in the order written (no FMA contraction); |x| is
+ * sqrtf((x.x x.x + x.y x.y) + x.z x.z).  Points are fp32 [N, 3] on the device, row-major.  Every output is the same bits on
+ * every run; no stage reads memory it did not write except its inputs.
+ *
+ * Normalisation (host, rade_gs_b200.unbounded, with the reference's numpy expressions): c2w = numpy's inv of the fp32
+ * world_view_transform^T (an fp32 result), poses = c2w[:3] @ diag(1, -1, -1, 1) in float64, center = the point nearest
+ * to the optical axes, radius = min |c2w[:3, 3] - center|, voxel_size = 2 radius / resolution (float64).  Where the
+ * reference combines these float64 scalars with fp32 tensors the tensor keeps fp32 and the scalar is rounded to fp32;
+ * the kernels take c = fp32(center), r = fp32(radius), trunc0 = fp32(5 voxel_size) and compute (x - c) / r as one
+ * division (the reference on CUDA multiplies by fp32(1 / r) instead, torch's division by a scalar: within one rounding).
+ * R = min(quantile_0.95(|contract((x - c) / r)|) + 0.01, 1.9): numpy's quantile and sum over the fp32 norms that
+ * rgs_unbounded_contract returns (no 2^24 limit), in numpy's dtype (float32 under numpy >= 2, float64 under numpy 1), as the
+ * reference computes it; the crop bounds and samples are numpy's linspace of that R, rounded to fp32.
+ *
+ * rgs_unbounded_contract: inverse = 0: q = (p - c) / r, m = |q|, out = q if m < 1 else (2 - 1 / m) * (q / m); norms (may be
+ *   NULL) = |out|.  inverse = 1 (inv_contraction and the clip): m = |p|, u = p if m < 1 else (1 / (2 - m)) * (p / m),
+ *   out = clip(u r + c, -max_range, max_range) (NaN stays NaN); norms = |out|.  With c = 0, r = 1 the two are the
+ *   reference's contract and uncontract exactly.
+ * rgs_unbounded_sdf (the hot path): sample (i, j, k) of an n^3 crop, stored at (i n + j) n + k, is s = (xs[i], ys[j], zs[k])
+ *   (the caller passes numpy's linspace rounded to fp32).  p = uncontract(s) r + c (as above, no clip).  trunc =
+ *   trunc0, times 1 / (2 - min(|p|, 1.9f)) when |p| > 1 (the world-space norm, as the reference writes it; NaN stays NaN).
+ *   Per view v in order: h_j = ((p.x M[0][j] + p.y M[1][j]) + p.z M[2][j]) + M[3][j] with M the row-major 4x4
+ *   full_proj_transform; u = h_0 / h_3, v = h_1 / h_3; the view counts iff -1 < u < 1, -1 < v < 1 and h_3 > 0.  Depth is
+ *   grid_sample(bilinear, border, align_corners=True): ix = ((u + 1) / 2) (W - 1) clamped to [0, W - 1] (likewise iy),
+ *   x0 = floor(ix), x1 = x0 + 1, weights nw = (x1 - ix)(y1 - iy), ne = (ix - x0)(y1 - iy), sw = (x1 - ix)(iy - y0),
+ *   se = (ix - x0)(iy - y0), d = 0 + nw D + ne D + sw D + se D in that order, skipping corners outside the image.
+ *   sdf = d - h_3; the view is kept iff sdf > -trunc; then t <- (t w + clamp(sdf / trunc, -1, 1)) / (w + 1), w <- w + 1,
+ *   from t = 1, w = 1.  The output is t.  depth fp32 [V, H, W], full_proj fp32 [V, 4, 4], 1 <= n <= 640.
+ * rgs_unbounded_colors: the same projection, masks and bilinear weights at each point p (no contraction) with trunc = trunc0;
+ *   each kept view updates col_k <- (col_k w + rgb_k) / (w + 1), w <- w + 1, from col = 0, w = 1.  rgb fp32 [V, 3, H, W].
+ * rgs_unbounded_mcubes: an n^3 crop (layout as rgs_unbounded_sdf, 2 <= n <= 640) with lattice point (i, j, k) at
+ *   lo + (i, j, k) sp, with the spacing sp given (the reference's (x_max - x_min) / (n - 1), computed by the caller in
+ *   numpy's dtype: float32 under numpy >= 2).  A point is inside iff its value < 0 (0 and NaN are outside).  The
+ *   cell at (i, j, k) < n - 1 uses the triangle table of rgs_tsdf_extract (corner c = x + 2y + 4z, edge e along axis e / 4):
+ *   every triangle's right-hand normal points toward increasing values (free space).  The vertex of a sign-change lattice
+ *   edge from g along axis a is owned by g: component a is (g_a + t) sp_a + lo_a, the others g_k sp_k + lo_k, with
+ *   t = f(g) / (f(g) - f(g + e_a)), all fp64 with each operation rounded.  Vertices fp64 [V, 3] in (point, axis) order,
+ *   triangles int32 [F, 3] in (cell, table order).  A crop without a sign change gives an empty mesh (the reference's skip
+ *   of crops with min > 0 or max < 0 gives the same).  One stream synchronisation inside.
+ * rgs_unbounded_merge (trimesh merge_vertices(digits_vertex=6), restated as this rule): key = (rint(x 1e6), rint(y 1e6),
+ *   rint(z 1e6)) (fp64 product, ties to even), each in [-2^21, 2^21) or the call fails.  Vertices with equal keys merge
+ *   into the first of them in input order, which keeps its unrounded coordinates, rounded to fp32 (.float()).  Survivors
+ *   keep their input order.  Triangles are renumbered and kept, also when they become degenerate.  One synchronisation.
+ * rgs_unbounded_clusters (Open3D cluster_connected_triangles + the removals of post_process_mesh): two triangles are
+ *   connected iff they share an edge as an unordered vertex pair (a vertex contact does not connect; a repeated index
+ *   forms the edge (a, a)).  threshold = max(sizes_ascending[C - k], 50) for 1 <= k <= C, max(smallest size, 50) for k = 0,
+ *   and 50 when k > C (the reference raises IndexError there).  Triangles of clusters smaller than the threshold go, then
+ *   vertices no remaining triangle uses (order kept), then triangles with a repeated index.  The outputs are the old
+ *   indices of the kept vertices (int32, ascending) and the kept triangles renumbered (int32 [F', 3], order kept).  Two
+ *   stream synchronisations inside.
+ * Triangle indices must lie in [0, V): the merge and the clusters return RGS_E_INVALID otherwise. */
+#define RGS_UNBOUNDED_MAX_CROP 640
+typedef struct rgs_unbounded_mesh_out {
+	void* vertices_user;        /* fp64 [V, 3] through resize */
+	void* triangles_user;       /* int32 [F, 3] through resize */
+	int64_t num_vertices, num_triangles;
+} rgs_unbounded_mesh_out;
+typedef struct rgs_unbounded_clusters_out {
+	void* vertex_index_user;    /* int32 [V'] through resize */
+	void* triangles_user;       /* int32 [F', 3] through resize */
+	int64_t num_vertices, num_triangles, num_clusters, threshold;
+} rgs_unbounded_clusters_out;
+/* center (host) fp32 [3], radius > 0, max_range > 0 (inverse only; +inf for none).  out fp32 [n, 3], norms fp32 [n] or NULL. */
+int32_t rgs_unbounded_contract(int64_t n, const float* points, const float center[3], float radius, int32_t inverse, float max_range, float* out, float* norms,
+                               void* cuda_stream);
+int32_t rgs_unbounded_sdf(int32_t n, const float* xs, const float* ys, const float* zs, int32_t V, int32_t H, int32_t W, const float* full_proj,
+                          const float* depth, const float center[3], float radius, float trunc, float* sdf, void* cuda_stream);
+int32_t rgs_unbounded_colors(int64_t N, const float* points, int32_t V, int32_t H, int32_t W, const float* full_proj, const float* depth, const float* rgb,
+                             float trunc, float* colors, void* cuda_stream);
+/* lo, spacing: host fp64 [3]. */
+int32_t rgs_unbounded_mcubes(int32_t n, const float* sdf, const double lo[3], const double spacing[3], rgs_resize_fn resize, rgs_unbounded_mesh_out* out,
+                             void* scratch_user, void* cuda_stream);
+/* vertices fp64 [V, 3], triangles int32 [F, 3] -> triangles_out int32 [F, 3] (caller-allocated), merged vertices fp32 [U, 3]
+ * through resize(vertices_user), U in *num_merged (host). */
+int32_t rgs_unbounded_merge(int64_t V, const double* vertices, int64_t F, const int32_t* triangles, int32_t* triangles_out, rgs_resize_fn resize,
+                            void* vertices_user, int64_t* num_merged, void* scratch_user, void* cuda_stream);
+int32_t rgs_unbounded_clusters(int64_t V, int64_t F, const int32_t* triangles, int64_t cluster_to_keep, rgs_resize_fn resize, rgs_unbounded_clusters_out* out,
+                               void* scratch_user, void* cuda_stream);
+
 /* ---- densify-and-prune and opacity reset (reference scene/gaussian_model.py:495-513 reset_opacity, :662-741 densify_and_prune) ----
  * Inputs per Gaussian (fp32, device): grad_accum, grad_accum_abs, denom [P] (the [P,1] statistics), raw scaling [P,3], raw
  * opacity [P], rotation [P,4], xyz [P,3]; 0 < P < 2^31.

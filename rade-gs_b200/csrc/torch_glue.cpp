@@ -17,6 +17,7 @@
 #include <torch/extension.h>
 
 #include <algorithm>
+#include <array>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -1354,6 +1355,94 @@ std::tuple<torch::Tensor, torch::Tensor> LpipsDistance(const torch::Tensor& feat
 	return std::make_tuple(map, mean);
 }
 
+// ---- unbounded mesh stages (rgs_unbounded_*; Python side rade_gs_b200.unbounded) -------------------------------------------
+
+std::array<float, 3> vec3f(const std::vector<double>& v, const char* name) {
+	TORCH_CHECK(v.size() == 3, name, " must have 3 values");
+	return {(float)v[0], (float)v[1], (float)v[2]};  // round to nearest, as np.float32
+}
+
+// points f32 [N,3] -> (out f32 [N,3], norms f32 [N])
+std::tuple<torch::Tensor, torch::Tensor> UnboundedContract(const torch::Tensor& points, const std::vector<double>& center, double radius, bool inverse,
+                                                           double max_range) {
+	const torch::Tensor p = arg(points, "points", torch::kFloat32, {-1, 3}, "[N, 3]");
+	const c10::cuda::CUDAGuard guard(p.device());
+	const std::array<float, 3> c = vec3f(center, "center");
+	torch::Tensor out = new_empty({p.size(0), 3}, p.options()), norms = new_empty({p.size(0)}, p.options());
+	check(rgs_unbounded_contract(p.size(0), p.data_ptr<float>(), c.data(), (float)radius, inverse, (float)max_range, out.data_ptr<float>(), norms.data_ptr<float>(),
+	                             at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(out, norms);
+}
+
+// xs, ys, zs f32 [n], full_proj f32 [V,4,4], depth f32 [V,H,W] -> sdf f32 [n,n,n]
+torch::Tensor UnboundedSdf(const torch::Tensor& xs, const torch::Tensor& ys, const torch::Tensor& zs, const torch::Tensor& full_proj, const torch::Tensor& depth,
+                           const std::vector<double>& center, double radius, double trunc) {
+	const torch::Tensor x = arg(xs, "xs", torch::kFloat32, {-1}, "[n]"), y = arg(ys, "ys", torch::kFloat32, {x.size(0)}, "[n] like xs", &x),
+	                    z = arg(zs, "zs", torch::kFloat32, {x.size(0)}, "[n] like xs", &x),
+	                    pr = arg(full_proj, "full_proj", torch::kFloat32, {-1, 4, 4}, "[V, 4, 4]", &x),
+	                    d = arg(depth, "depth", torch::kFloat32, {pr.size(0), -1, -1}, "[V, H, W] with V like full_proj", &x);
+	const c10::cuda::CUDAGuard guard(x.device());
+	const std::array<float, 3> c = vec3f(center, "center");
+	const int64_t n = x.size(0);
+	TORCH_CHECK(n >= 1 && n <= RGS_UNBOUNDED_MAX_CROP, "crop size must be in [1, ", RGS_UNBOUNDED_MAX_CROP, "], got ", n);
+	torch::Tensor sdf = new_empty({n, n, n}, x.options());
+	check(rgs_unbounded_sdf((int32_t)n, x.data_ptr<float>(), y.data_ptr<float>(), z.data_ptr<float>(), (int32_t)pr.size(0), (int32_t)d.size(1), (int32_t)d.size(2),
+	                        pr.data_ptr<float>(), d.data_ptr<float>(), c.data(), (float)radius, (float)trunc, sdf.data_ptr<float>(),
+	                        at::cuda::getCurrentCUDAStream().stream()));
+	return sdf;
+}
+
+// points f32 [N,3], full_proj f32 [V,4,4], depth f32 [V,H,W], rgb f32 [V,3,H,W] -> colors f32 [N,3]
+torch::Tensor UnboundedColors(const torch::Tensor& points, const torch::Tensor& full_proj, const torch::Tensor& depth, const torch::Tensor& rgb, double trunc) {
+	const torch::Tensor p = arg(points, "points", torch::kFloat32, {-1, 3}, "[N, 3]"),
+	                    pr = arg(full_proj, "full_proj", torch::kFloat32, {-1, 4, 4}, "[V, 4, 4]", &p),
+	                    d = arg(depth, "depth", torch::kFloat32, {pr.size(0), -1, -1}, "[V, H, W] with V like full_proj", &p),
+	                    c = arg(rgb, "rgb", torch::kFloat32, {pr.size(0), 3, d.size(1), d.size(2)}, "[V, 3, H, W] like depth", &p);
+	const c10::cuda::CUDAGuard guard(p.device());
+	torch::Tensor out = new_empty({p.size(0), 3}, p.options());
+	check(rgs_unbounded_colors(p.size(0), p.data_ptr<float>(), (int32_t)pr.size(0), (int32_t)d.size(1), (int32_t)d.size(2), pr.data_ptr<float>(), d.data_ptr<float>(),
+	                           c.data_ptr<float>(), (float)trunc, out.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
+// sdf f32 [n,n,n], lo / spacing 3 doubles -> (vertices f64 [V,3], triangles int32 [F,3])
+std::tuple<torch::Tensor, torch::Tensor> UnboundedMcubes(const torch::Tensor& sdf, const std::vector<double>& lo, const std::vector<double>& spacing) {
+	const torch::Tensor f = arg(sdf, "sdf", torch::kFloat32, {-1, -1, -1}, "[n, n, n]");
+	TORCH_CHECK(f.size(1) == f.size(0) && f.size(2) == f.size(0), "sdf must be [n, n, n], got ", f.sizes());
+	TORCH_CHECK(lo.size() == 3 && spacing.size() == 3, "lo and spacing must have 3 values");
+	TORCH_CHECK(f.size(0) >= 2 && f.size(0) <= RGS_UNBOUNDED_MAX_CROP, "crop size must be in [2, ", RGS_UNBOUNDED_MAX_CROP, "], got ", f.size(0));
+	const c10::cuda::CUDAGuard guard(f.device());
+	torch::Tensor verts = bytes(f), tris = bytes(f), scratch = bytes(f);
+	rgs_unbounded_mesh_out out{&verts, &tris, 0, 0};
+	check(rgs_unbounded_mcubes((int32_t)f.size(0), f.data_ptr<float>(), lo.data(), spacing.data(), resize_cb, &out, &scratch, at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(rows(verts, torch::kFloat64, out.num_vertices, {3}), rows(tris, torch::kInt32, out.num_triangles, {3}));
+}
+
+// vertices f64 [V,3], triangles int32 [F,3] -> (vertices f32 [U,3], triangles int32 [F,3])
+std::tuple<torch::Tensor, torch::Tensor> UnboundedMerge(const torch::Tensor& vertices, const torch::Tensor& triangles) {
+	const torch::Tensor v = arg(vertices, "vertices", torch::kFloat64, {-1, 3}, "[V, 3]"), t = arg(triangles, "triangles", torch::kInt32, {-1, 3}, "[F, 3]", &v);
+	const c10::cuda::CUDAGuard guard(v.device());
+	torch::Tensor merged = bytes(v), scratch = bytes(v), tout = new_empty({t.size(0), 3}, t.options());
+	int64_t U = 0;
+	check(rgs_unbounded_merge(v.size(0), v.data_ptr<double>(), t.size(0), t.data_ptr<int32_t>(), tout.data_ptr<int32_t>(), resize_cb, &merged, &U, &scratch,
+	                          at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(rows(merged, torch::kFloat32, U, {3}), tout);
+}
+
+// triangles int32 [F,3] over num_vertices vertices -> (kept vertex indices int32 [V'], triangles int32 [F',3],
+// {num_clusters, threshold})
+std::tuple<torch::Tensor, torch::Tensor, py::dict> UnboundedClusters(int64_t num_vertices, const torch::Tensor& triangles, int64_t cluster_to_keep) {
+	const torch::Tensor t = arg(triangles, "triangles", torch::kInt32, {-1, 3}, "[F, 3]");
+	const c10::cuda::CUDAGuard guard(t.device());
+	torch::Tensor vidx = bytes(t), tout = bytes(t), scratch = bytes(t);
+	rgs_unbounded_clusters_out out{&vidx, &tout, 0, 0, 0, 0};
+	check(rgs_unbounded_clusters(num_vertices, t.size(0), t.data_ptr<int32_t>(), cluster_to_keep, resize_cb, &out, &scratch, at::cuda::getCurrentCUDAStream().stream()));
+	py::dict st;
+	st["num_clusters"] = out.num_clusters;
+	st["threshold"] = out.threshold;
+	return std::make_tuple(rows(vidx, torch::kInt32, out.num_vertices, {}), rows(tout, torch::kInt32, out.num_triangles, {3}), st);
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1470,6 +1559,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	lp.def("conv3x3", &LpipsConv3x3, py::arg("input"), py::arg("weight"), py::arg("bias"), py::arg("buffer") = py::none());
 	lp.def("maxpool", &LpipsMaxpool, py::arg("input"), py::arg("buffer") = py::none());
 	lp.def("distance", &LpipsDistance, py::arg("feats"), py::arg("lin"));
+	// contracted-space TSDF mesh of unbounded scenes: a private submodule behind rade_gs_b200.unbounded
+	py::module_ ub = m.def_submodule("_unbounded", "unbounded-scene mesh stages behind rade_gs_b200.unbounded");
+	ub.def("contract", &UnboundedContract, py::arg("points"), py::arg("center"), py::arg("radius"), py::arg("inverse"), py::arg("max_range"));
+	ub.def("sdf", &UnboundedSdf, py::arg("xs"), py::arg("ys"), py::arg("zs"), py::arg("full_proj"), py::arg("depth"), py::arg("center"), py::arg("radius"),
+	       py::arg("trunc"));
+	ub.def("colors", &UnboundedColors, py::arg("points"), py::arg("full_proj"), py::arg("depth"), py::arg("rgb"), py::arg("trunc"));
+	ub.def("mcubes", &UnboundedMcubes, py::arg("sdf"), py::arg("lo"), py::arg("spacing"));
+	ub.def("merge", &UnboundedMerge, py::arg("vertices"), py::arg("triangles"));
+	ub.def("clusters", &UnboundedClusters, py::arg("num_vertices"), py::arg("triangles"), py::arg("cluster_to_keep"));
 	m.def("grad_stride",[](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });
