@@ -437,6 +437,50 @@ int32_t rgs_tsdf_extract(const rgs_tsdf_grid* grid, float weight_threshold, rgs_
 int32_t rgs_tsdf_vertex_normals(int64_t V, const float* vertices, int64_t F, const int32_t* triangles, float* normals, rgs_resize_fn scratch,
                                 void* scratch_user, void* cuda_stream);
 
+/* ---- bounded TSDF of the 2DGS-derived extractor (reference utils/mesh_utils.py:118-160 extract_mesh_bounded, there
+ *      Open3D's legacy ScalableTSDFVolume with RGB8 colour on the CPU; :272-285 export_image) ----
+ * The volume is an rgs_tsdf_grid (16^3 voxel units = the grid's blocks, same keys, hash, pools, growth and counters as
+ * above); the functions below replace touch and integrate, and rgs_tsdf_extract is reused.  Every stored value is fixed
+ * bit for bit; fp32 operations are rounded one by one in the order written (no FMA contraction).  Open3D is not a
+ * reference here: where its rule is not known, the rule below is chosen, and bit parity with Open3D is not a goal.
+ *
+ * RGBD (rgs_scalable_rgbd; create_from_color_and_depth(depth_scale=1, depth_trunc, convert_rgb_to_intensity=False) of the
+ * reference's np.asarray(rgb * 255, dtype=np.uint8) and its masked depth).  rgb fp32 [3, H, W] -> color uint8 [H, W, 3]:
+ *   byte = B(rgb * 255.0f) (one fp32 product), B(x) = the low 8 bits of the int32 truncation of x when -2^31 < x < 2^31,
+ *   else 0 (NaN included): numpy's float32 -> uint8 cast on x86-64 (cvttss2si), so 1.01 -> 1, -0.01 -> 254, NaN -> 0.
+ *   depth fp32 [H, W] -> depth_out: d = 0 where mask (fp32 [H, W], may be NULL) < 0.5; then d = 0 where (double)d >=
+ *   depth_trunc (chosen: >=).  NaN depth stays NaN and is skipped below, as every d <= 0.
+ * Touch (rgs_scalable_touch; the legacy volume's unit allocation).  Pixels (u, v) with u, v = 0 mod 4 and d = depth[v, u]
+ *   > 0: x = ((u - cx) d) / fx, y = ((v - cy) d) / fy (integer pixel coordinates), q = (x, y, d) - t, p_k = (R_0k q.x +
+ *   R_1k q.y) + R_2k q.z (chosen: fp32 R^T (p - t), not a double inverse); lo_k = floor((p_k - sdf_trunc) / (16 voxel_size)),
+ *   hi_k = floor((p_k + sdf_trunc) / (16 voxel_size)); every unit of the box [lo, hi] is touched (a pixel whose box leaves
+ *   the key range touches nothing).  Units come back in ascending key order, with rgs_tsdf_touch's frame hash, counters and
+ *   RGS_E_CAPACITY protocol.  The camera's depth_scale, depth_max and trunc_voxel_multiplier are not read; sdf_trunc is the
+ *   absolute truncation (positive, finite).
+ * Integrate (rgs_scalable_integrate).  The units are inserted and claimed as in rgs_tsdf_integrate; then every voxel of
+ *   them, one thread each, at its centre p = ((float)g + 0.5f) voxel_size (g the integer grid point; the sum is exact for
+ *   |g| < 2^23):  x_c = ((R_00 p.x + R_01 p.y) + R_02 p.z) + t_0 (likewise y_c, z_c); skipped unless z_c > 0;
+ *   u = floor(((x_c / z_c) fx + cx) + 0.5), v likewise (the rounded projection), accepted iff in [0, W) x [0, H);
+ *   skipped unless d = depth[v, u] > 0; xn = (u - cx) / fx, yn = (v - cy) / fy, sdf = (d - z_c) sqrtf((1 + xn xn) + yn yn)
+ *   (IEEE sqrt); skipped unless sdf > -sdf_trunc; then tsdf_obs = min(1, sdf / sdf_trunc), tsdf <- (w tsdf + tsdf_obs) /
+ *   (w + 1), each colour channel col <- (w col + (float)byte) / (w + 1) (fp32 on 0..255; chosen), w <- w + 1.
+ *   The principal point is used as given: the reference's cx = W / 2 is half a pixel from the rasterizer's pixel centres.
+ * Extract: rgs_tsdf_extract with weight_threshold = 1 (weights are whole counts, so a corner of weight 0 is invalid); the
+ *   caller then adds 0.5f voxel_size to every vertex component (one fp32 addition: vertices sit on voxel centres) and
+ *   divides every colour by 255.0f (one fp32 division).
+ * Image export (rgs_scalable_image_u8; save_img_u8): image fp32 [3, H, W] -> out uint8 [H, W, 3],
+ *   y = x scale + offset (two roundings), 0 if NaN, clipped to [0, 1], byte = (int)(y * 255.0f) (truncation).
+ * No host synchronisation except rgs_scalable_touch's one counter read. */
+int32_t rgs_scalable_rgbd(int32_t H, int32_t W, const float* rgb, const float* depth, const float* mask, double depth_trunc, uint8_t* color,
+                          float* depth_out, void* cuda_stream);
+int32_t rgs_scalable_image_u8(int32_t H, int32_t W, const float* image, float scale, float offset, uint8_t* out, void* cuda_stream);
+/* depth fp32 [H, W].  unit_coords int32 [frame_slots / 2, 3]; returns the count, RGS_E_CAPACITY or another negative status. */
+int64_t rgs_scalable_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, float sdf_trunc, const float* depth, int32_t* unit_coords,
+                           int64_t* allocated, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+/* unit_coords int32 [n, 3], depth fp32 [H, W], color uint8 [H, W, 3]; call_id as rgs_tsdf_integrate. */
+int32_t rgs_scalable_integrate(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, float sdf_trunc, int64_t n, const int32_t* unit_coords,
+                               const float* depth, const uint8_t* color, int32_t call_id, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+
 /* ---- DTU evaluation: the chamfer distances of dtu_eval/eval.py and the mask culling of evaluate_dtu_mesh.py:82-138 ----
  * All arithmetic is IEEE fp64 with every operation rounded on its own (no FMA contraction), in the order written; a - b is
  * one rounded subtraction.  Points are fp64 [N, 3] on the device, row-major.  The squared pair distance is

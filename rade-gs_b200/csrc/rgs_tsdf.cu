@@ -15,6 +15,10 @@
 //              order and grid capacity.
 //   normals    (vertex, triangle) pairs stably radix-sorted by vertex, so every vertex sums its face normals in ascending
 //              triangle order: no float atomics.
+//   scalable   the bounded TSDF of the reference's GaussianExtractor (Open3D's legacy ScalableTSDFVolume, RGB8) on the same
+//              grid: an RGBD kernel (numpy's uint8 wrap, mask, depth_trunc), a touch over every 4th pixel, and an integrate
+//              kernel at voxel centres with the ray-distance SDF, after the same insert and claim; rgs_tsdf_extract as is.
+//              Also the 8-bit conversion of the image export.
 //
 // This file also holds the C-ABI entry points rgs_tsdf_* (include/rgs_b200.h).
 #include <cub/cub.cuh>
@@ -75,6 +79,27 @@ struct Cam {
 
 // ---- touch ------------------------------------------------------------------------------------------------------------
 
+// the box of blocks [lo, hi] into the frame-local hash; new keys appended to the list
+__device__ inline void touch_box(const float lo[3], const float hi[3], uint64_t* __restrict__ fkeys, uint64_t fmask, uint64_t* __restrict__ flist,
+                                 int64_t fcap, int32_t* __restrict__ counters) {
+	for (int k = 0; k < 3; k++)
+		if (!(lo[k] >= (float)KEY_LO && hi[k] <= (float)KEY_HI)) return;  // also rejects NaN
+	for (int bz = (int)lo[2]; bz <= (int)hi[2]; bz++)
+		for (int by = (int)lo[1]; by <= (int)hi[1]; by++)
+			for (int bx = (int)lo[0]; bx <= (int)hi[0]; bx++) {
+				const uint64_t key = pack_key(bx, by, bz);
+				bool fresh = false;
+				if (hash_insert(fkeys, fmask, key, fresh) < 0) {
+					atomicOr(counters + 3, 1);  // frame hash full
+					return;
+				}
+				if (fresh) {
+					const int n = atomicAdd(counters + 1, 1);
+					if (n < fcap) flist[n] = key;
+				}
+			}
+}
+
 __global__ void __launch_bounds__(256) tsdf_touch_kernel(Cam c, const float* __restrict__ depth, uint64_t* __restrict__ fkeys, uint64_t fmask,
                                                          uint64_t* __restrict__ flist, int64_t fcap, int32_t* __restrict__ counters) {
 	const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -95,22 +120,60 @@ __global__ void __launch_bounds__(256) tsdf_touch_kernel(Cam c, const float* __r
 			hi[k] = s ? fmaxf(hi[k], b) : b;
 		}
 	}
-	for (int k = 0; k < 3; k++)
-		if (!(lo[k] >= (float)KEY_LO && hi[k] <= (float)KEY_HI)) return;  // also rejects NaN
-	for (int bz = (int)lo[2]; bz <= (int)hi[2]; bz++)
-		for (int by = (int)lo[1]; by <= (int)hi[1]; by++)
-			for (int bx = (int)lo[0]; bx <= (int)hi[0]; bx++) {
-				const uint64_t key = pack_key(bx, by, bz);
-				bool fresh = false;
-				if (hash_insert(fkeys, fmask, key, fresh) < 0) {
-					atomicOr(counters + 3, 1);  // frame hash full
-					return;
-				}
-				if (fresh) {
-					const int n = atomicAdd(counters + 1, 1);
-					if (n < fcap) flist[n] = key;
-				}
-			}
+	touch_box(lo, hi, fkeys, fmask, flist, fcap, counters);
+}
+
+// ---- scalable volume (Open3D's legacy ScalableTSDFVolume with RGB8 colour) ---------------------------------------------
+
+// numpy's float32 -> uint8 cast on x86-64: truncation to int32 (cvttss2si, which gives INT_MIN for NaN and |x| >= 2^31),
+// then the low byte.  A CUDA float-to-int conversion saturates instead, so the out-of-range cases are spelled out.
+__device__ inline uint8_t numpy_u8(float x) { return (x > -2147483648.0f && x < 2147483648.0f) ? (uint8_t)(int32_t)x : (uint8_t)0; }
+
+__global__ void __launch_bounds__(256) scalable_rgbd_kernel(int64_t P, const float* __restrict__ rgb, const float* __restrict__ depth,
+                                                            const float* __restrict__ mask, double depth_trunc, uint8_t* __restrict__ color,
+                                                            float* __restrict__ dout) {
+	const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= P) return;
+#pragma unroll
+	for (int k = 0; k < 3; k++) color[3 * i + k] = numpy_u8(__fmul_rn(rgb[k * P + i], 255.0f));
+	float d = depth[i];
+	if (mask && mask[i] < 0.5f) d = 0.0f;
+	if ((double)d >= depth_trunc) d = 0.0f;
+	dout[i] = d;
+}
+
+// save_img_u8: (clip(nan_to_num(x * scale + offset), 0, 1) * 255).astype(uint8), [3, H, W] -> [H, W, 3]
+__global__ void __launch_bounds__(256) scalable_image_u8_kernel(int64_t P, const float* __restrict__ img, float scale, float offset,
+                                                                uint8_t* __restrict__ out) {
+	const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= P) return;
+#pragma unroll
+	for (int k = 0; k < 3; k++) {
+		const float x = __fadd_rn(__fmul_rn(img[k * P + i], scale), offset);
+		const float y = isnan(x) ? 0.0f : fminf(fmaxf(x, 0.0f), 1.0f);
+		out[3 * i + k] = (uint8_t)(int32_t)__fmul_rn(y, 255.0f);
+	}
+}
+
+// every 4th pixel in both axes, unprojected at its integer coordinates; the units of the box around p +- sdf_trunc
+__global__ void __launch_bounds__(256) scalable_touch_kernel(Cam c, const float* __restrict__ depth, uint64_t* __restrict__ fkeys, uint64_t fmask,
+                                                             uint64_t* __restrict__ flist, int64_t fcap, int32_t* __restrict__ counters) {
+	const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	const int sw = (c.W + 3) / 4, sh = (c.H + 3) / 4;
+	if (i >= (int64_t)sw * sh) return;
+	const int px = 4 * (int)(i % sw), py = 4 * (int)(i / sw);
+	const float d = depth[(size_t)py * c.W + px];
+	if (!(d > 0.0f)) return;
+	const float q0 = __fsub_rn(__fdiv_rn(__fmul_rn(__fsub_rn((float)px, c.cx), d), c.fx), c.t[0]);
+	const float q1 = __fsub_rn(__fdiv_rn(__fmul_rn(__fsub_rn((float)py, c.cy), d), c.fy), c.t[1]);
+	const float q2 = __fsub_rn(d, c.t[2]);
+	float lo[3], hi[3];
+	for (int k = 0; k < 3; k++) {
+		const float pw = __fadd_rn(__fadd_rn(__fmul_rn(c.R[k], q0), __fmul_rn(c.R[3 + k], q1)), __fmul_rn(c.R[6 + k], q2));
+		lo[k] = floorf(__fdiv_rn(__fsub_rn(pw, c.trunc), c.bs));
+		hi[k] = floorf(__fdiv_rn(__fadd_rn(pw, c.trunc), c.bs));
+	}
+	touch_box(lo, hi, fkeys, fmask, flist, fcap, counters);
 }
 
 __global__ void __launch_bounds__(256) tsdf_decode_kernel(int n, const uint64_t* __restrict__ keys, int32_t* __restrict__ out) {
@@ -200,6 +263,43 @@ __global__ void __launch_bounds__(INTEGRATE_THREADS) tsdf_integrate_kernel(rgs_t
 		ts[v] = __fdiv_rn(__fadd_rn(__fmul_rn(w0, ts[v]), obs), w1);
 #pragma unroll
 		for (int k = 0; k < 3; k++) cs[3 * v + k] = __fdiv_rn(__fadd_rn(__fmul_rn(w0, cs[3 * v + k]), color[3 * pix + k]), w1);
+		ws[v] = w1;
+	}
+}
+
+// the scalable volume's update: samples at voxel centres, the rounded projection, the SDF as a distance along the ray
+__global__ void __launch_bounds__(INTEGRATE_THREADS) scalable_integrate_kernel(rgs_tsdf_grid g, Cam c, const int32_t* __restrict__ bc,
+                                                                               const int32_t* __restrict__ slot, const float* __restrict__ depth,
+                                                                               const uint8_t* __restrict__ color) {
+	const int64_t b = blockIdx.x;
+	const int32_t idx = slot[b];
+	if (idx < 0) return;
+	const int bx = bc[3 * b], by = bc[3 * b + 1], bz = bc[3 * b + 2];
+	float* __restrict__ ts = g.tsdf + (size_t)idx * BV;
+	float* __restrict__ ws = g.weight + (size_t)idx * BV;
+	float* __restrict__ cs = g.color + (size_t)idx * BV * 3;
+	for (int v = threadIdx.x; v < BV; v += INTEGRATE_THREADS) {
+		const float px = __fmul_rn(__fadd_rn((float)(bx * RES + (v & 15)), 0.5f), c.vs);
+		const float py = __fmul_rn(__fadd_rn((float)(by * RES + (v >> 4 & 15)), 0.5f), c.vs);
+		const float pz = __fmul_rn(__fadd_rn((float)(bz * RES + (v >> 8)), 0.5f), c.vs);
+		const float xc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(c.R[0], px), __fmul_rn(c.R[1], py)), __fmul_rn(c.R[2], pz)), c.t[0]);
+		const float yc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(c.R[3], px), __fmul_rn(c.R[4], py)), __fmul_rn(c.R[5], pz)), c.t[1]);
+		const float zc = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(c.R[6], px), __fmul_rn(c.R[7], py)), __fmul_rn(c.R[8], pz)), c.t[2]);
+		if (!(zc > 0.0f)) continue;
+		const float u = floorf(__fadd_rn(__fadd_rn(__fmul_rn(__fdiv_rn(xc, zc), c.fx), c.cx), 0.5f));
+		const float w = floorf(__fadd_rn(__fadd_rn(__fmul_rn(__fdiv_rn(yc, zc), c.fy), c.cy), 0.5f));
+		if (!(u >= 0.0f && u < (float)c.W && w >= 0.0f && w < (float)c.H)) continue;
+		const size_t pix = (size_t)w * c.W + (size_t)u;
+		const float d = depth[pix];
+		if (!(d > 0.0f)) continue;
+		const float xn = __fdiv_rn(__fsub_rn(u, c.cx), c.fx), yn = __fdiv_rn(__fsub_rn(w, c.cy), c.fy);
+		const float sdf = __fmul_rn(__fsub_rn(d, zc), __fsqrt_rn(__fadd_rn(__fadd_rn(1.0f, __fmul_rn(xn, xn)), __fmul_rn(yn, yn))));
+		if (!(sdf > -c.trunc)) continue;
+		const float obs = fminf(1.0f, __fdiv_rn(sdf, c.trunc));
+		const float w0 = ws[v], w1 = __fadd_rn(w0, 1.0f);
+		ts[v] = __fdiv_rn(__fadd_rn(__fmul_rn(w0, ts[v]), obs), w1);
+#pragma unroll
+		for (int k = 0; k < 3; k++) cs[3 * v + k] = __fdiv_rn(__fadd_rn(__fmul_rn(w0, cs[3 * v + k]), (float)color[3 * pix + k]), w1);
 		ws[v] = w1;
 	}
 }
@@ -474,14 +574,25 @@ size_t tsdf_touch_scratch_bytes(int64_t n) {
 	return cv.size();
 }
 
+// the scalable volume's camera: trunc is the absolute sdf_trunc
+Cam make_scalable_cam(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c, float sdf_trunc) {
+	Cam k = make_cam(g, c);
+	k.trunc = sdf_trunc;
+	return k;
+}
+
 // phase 1: the frame-local hash and list; counters_host receives counters[0..3] (the one host read of a view)
-cudaError_t launch_tsdf_touch(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c, const float* depth, int32_t* counters_host, cudaStream_t s) {
-	const Cam k = make_cam(g, c);
+cudaError_t launch_tsdf_touch(const rgs_tsdf_grid& g, const Cam& k, bool scalable, const float* depth, int32_t* counters_host, cudaStream_t s) {
 	RGS_TRY(cudaMemsetAsync(g.frame_keys, 0xff, (size_t)g.frame_slots * sizeof(uint64_t), s));
 	RGS_TRY(cudaMemsetAsync(g.counters + 1, 0, sizeof(int32_t), s));
 	RGS_TRY(cudaMemsetAsync(g.counters + 3, 0, sizeof(int32_t), s));
-	const int64_t P = (int64_t)c.width * c.height;
-	tsdf_touch_kernel<<<blocks_for(P), 256, 0, s>>>(k, depth, g.frame_keys, (uint64_t)g.frame_slots - 1, g.frame_list, g.frame_slots / 2, g.counters);
+	if (scalable) {
+		const int64_t P = (int64_t)((k.W + 3) / 4) * ((k.H + 3) / 4);
+		scalable_touch_kernel<<<blocks_for(P), 256, 0, s>>>(k, depth, g.frame_keys, (uint64_t)g.frame_slots - 1, g.frame_list, g.frame_slots / 2, g.counters);
+	} else {
+		const int64_t P = (int64_t)k.W * k.H;
+		tsdf_touch_kernel<<<blocks_for(P), 256, 0, s>>>(k, depth, g.frame_keys, (uint64_t)g.frame_slots - 1, g.frame_list, g.frame_slots / 2, g.counters);
+	}
 	count_launch();
 	RGS_TRY(cudaGetLastError());
 	RGS_TRY(cudaMemcpyAsync(counters_host, g.counters, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
@@ -502,13 +613,27 @@ cudaError_t launch_tsdf_touch_sort(const rgs_tsdf_grid& g, int64_t n, int32_t* o
 	return cudaGetLastError();
 }
 
+// insert the n blocks, then give each to the one coordinate that claims it in this call (slot[i], -1 for the others)
+void insert_and_claim(const rgs_tsdf_grid& g, int64_t n, const int32_t* bc, int32_t call_id, int32_t* slot, cudaStream_t s) {
+	tsdf_insert_kernel<<<blocks_for(n), 256, 0, s>>>(g, n, bc);
+	tsdf_claim_kernel<<<blocks_for(n), 256, 0, s>>>(g, n, bc, call_id, slot);
+	count_launch(2);
+}
+
 cudaError_t launch_tsdf_integrate(const rgs_tsdf_grid& g, const rgs_tsdf_camera& c, int64_t n, const int32_t* bc, const float* depth, const float* color,
                                   int32_t call_id, int32_t* slot, cudaStream_t s) {
 	const Cam k = make_cam(g, c);
-	tsdf_insert_kernel<<<blocks_for(n), 256, 0, s>>>(g, n, bc);
-	tsdf_claim_kernel<<<blocks_for(n), 256, 0, s>>>(g, n, bc, call_id, slot);
+	insert_and_claim(g, n, bc, call_id, slot, s);
 	tsdf_integrate_kernel<<<(unsigned)n, INTEGRATE_THREADS, 0, s>>>(g, k, bc, slot, depth, color);
-	count_launch(3);
+	count_launch();
+	return cudaGetLastError();
+}
+
+cudaError_t launch_scalable_integrate(const rgs_tsdf_grid& g, const Cam& k, int64_t n, const int32_t* bc, const float* depth, const uint8_t* color,
+                                      int32_t call_id, int32_t* slot, cudaStream_t s) {
+	insert_and_claim(g, n, bc, call_id, slot, s);
+	scalable_integrate_kernel<<<(unsigned)n, INTEGRATE_THREADS, 0, s>>>(g, k, bc, slot, depth, color);
+	count_launch();
 	return cudaGetLastError();
 }
 
@@ -676,7 +801,8 @@ static int tsdf_grid_check(const rgs_tsdf_grid* g) {
 	return RGS_OK;
 }
 
-static int tsdf_camera_check(const rgs_tsdf_grid* g, const rgs_tsdf_camera* c) {
+// image size, intrinsics and extrinsic (the checks both volumes share)
+static int tsdf_pinhole_check(const rgs_tsdf_camera* c) {
 	if (!c) return fail(RGS_E_INVALID, "null camera");
 	if (c->width <= 0 || c->height <= 0) return fail(RGS_E_INVALID, "image size must be positive");
 	if (!std::isfinite(c->fx) || !std::isfinite(c->fy) || c->fx == 0.0f || c->fy == 0.0f || !std::isfinite(c->cx) || !std::isfinite(c->cy))
@@ -685,6 +811,11 @@ static int tsdf_camera_check(const rgs_tsdf_grid* g, const rgs_tsdf_camera* c) {
 		if (!std::isfinite(c->R[i])) return fail(RGS_E_INVALID, "extrinsic must be finite");
 	for (int i = 0; i < 3; i++)
 		if (!std::isfinite(c->t[i])) return fail(RGS_E_INVALID, "extrinsic must be finite");
+	return RGS_OK;
+}
+
+static int tsdf_camera_check(const rgs_tsdf_grid* g, const rgs_tsdf_camera* c) {
+	if (const int rc = tsdf_pinhole_check(c)) return rc;
 	if (!finite_pos(c->depth_scale) || !finite_pos(c->depth_max) || !finite_pos(c->trunc_voxel_multiplier))
 		return fail(RGS_E_INVALID, "depth_scale, depth_max and trunc_voxel_multiplier must be positive and finite");
 	// camera centre +- (depth_max + trunc) must stay inside the block-key range (the keys must never wrap)
@@ -712,15 +843,12 @@ static int tsdf_flags_check(const int32_t* cnt) {
 	return RGS_OK;
 }
 
-int64_t rgs_tsdf_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, const float* depth, int32_t* block_coords, int64_t* allocated,
-                       rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
-	int rc = tsdf_grid_check(grid);
-	if (rc == RGS_OK) rc = tsdf_camera_check(grid, cam);
-	if (rc != RGS_OK) return rc;
-	if (!depth || !block_coords || !scratch) return fail(RGS_E_INVALID, "null pointer");
-	const cudaStream_t s = (cudaStream_t)cuda_stream;
+// the touch of either volume after its argument checks: frame hash, counters, capacity protocol, sorted decode
+static int64_t tsdf_touch_run(const rgs_tsdf_grid* grid, const Cam& k, bool scalable, const float* depth, int32_t* block_coords, int64_t* allocated,
+                              rgs_resize_fn scratch, void* scratch_user, cudaStream_t s) {
+	int rc;
 	int32_t cnt[4];
-	if ((rc = cuda_status(launch_tsdf_touch(*grid, *cam, depth, cnt, s), "tsdf touch")) != RGS_OK) return rc;
+	if ((rc = cuda_status(launch_tsdf_touch(*grid, k, scalable, depth, cnt, s), "tsdf touch")) != RGS_OK) return rc;
 	if ((rc = tsdf_flags_check(cnt)) != RGS_OK) return rc;
 	if (allocated) *allocated = cnt[0];
 	if (cnt[3] || cnt[1] > grid->frame_slots / 2) return fail(RGS_E_CAPACITY, "tsdf touch: more blocks than the frame-local hash holds");
@@ -730,6 +858,67 @@ int64_t rgs_tsdf_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, co
 	if ((rc = grow(scratch, scratch_user, tsdf_touch_scratch_bytes(n), buf, "tsdf scratch")) != RGS_OK) return rc;
 	if ((rc = cuda_status(launch_tsdf_touch_sort(*grid, n, block_coords, buf, s), "tsdf touch")) != RGS_OK) return rc;
 	return n;
+}
+
+int64_t rgs_tsdf_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, const float* depth, int32_t* block_coords, int64_t* allocated,
+                       rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	int rc = tsdf_grid_check(grid);
+	if (rc == RGS_OK) rc = tsdf_camera_check(grid, cam);
+	if (rc != RGS_OK) return rc;
+	if (!depth || !block_coords || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	return tsdf_touch_run(grid, make_cam(*grid, *cam), false, depth, block_coords, allocated, scratch, scratch_user, (cudaStream_t)cuda_stream);
+}
+
+int32_t rgs_scalable_rgbd(int32_t H, int32_t W, const float* rgb, const float* depth, const float* mask, double depth_trunc, uint8_t* color,
+                          float* depth_out, void* cuda_stream) {
+	if (H < 0 || W < 0) return fail(RGS_E_INVALID, "image size must not be negative");
+	if (std::isnan(depth_trunc)) return fail(RGS_E_INVALID, "depth_trunc is NaN");
+	const int64_t P = (int64_t)H * W;
+	if (P == 0) return RGS_OK;
+	if (!rgb || !depth || !color || !depth_out) return fail(RGS_E_INVALID, "null pointer");
+	scalable_rgbd_kernel<<<blocks_for(P), 256, 0, (cudaStream_t)cuda_stream>>>(P, rgb, depth, mask, depth_trunc, color, depth_out);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "scalable rgbd");
+}
+
+int32_t rgs_scalable_image_u8(int32_t H, int32_t W, const float* image, float scale, float offset, uint8_t* out, void* cuda_stream) {
+	if (H < 0 || W < 0) return fail(RGS_E_INVALID, "image size must not be negative");
+	const int64_t P = (int64_t)H * W;
+	if (P == 0) return RGS_OK;
+	if (!image || !out) return fail(RGS_E_INVALID, "null pointer");
+	scalable_image_u8_kernel<<<blocks_for(P), 256, 0, (cudaStream_t)cuda_stream>>>(P, image, scale, offset, out);
+	count_launch();
+	return cuda_status(cudaGetLastError(), "scalable image_u8");
+}
+
+static int scalable_check(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, float sdf_trunc) {
+	int rc = tsdf_grid_check(grid);
+	if (rc == RGS_OK) rc = tsdf_pinhole_check(cam);
+	if (rc == RGS_OK && !finite_pos(sdf_trunc)) rc = fail(RGS_E_INVALID, "sdf_trunc must be positive and finite");
+	return rc;
+}
+
+int64_t rgs_scalable_touch(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, float sdf_trunc, const float* depth, int32_t* unit_coords,
+                           int64_t* allocated, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	if (const int rc = scalable_check(grid, cam, sdf_trunc)) return rc;
+	if (!depth || !unit_coords || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	return tsdf_touch_run(grid, make_scalable_cam(*grid, *cam, sdf_trunc), true, depth, unit_coords, allocated, scratch, scratch_user,
+	                      (cudaStream_t)cuda_stream);
+}
+
+int32_t rgs_scalable_integrate(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, float sdf_trunc, int64_t n, const int32_t* unit_coords,
+                               const float* depth, const uint8_t* color, int32_t call_id, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream) {
+	int rc = scalable_check(grid, cam, sdf_trunc);
+	if (rc != RGS_OK) return rc;
+	if (n < 0 || n > INT32_MAX) return fail(RGS_E_INVALID, "block count out of range");
+	if (call_id <= 0) return fail(RGS_E_INVALID, "call_id must be positive");
+	if (n == 0) return RGS_OK;
+	if (!unit_coords || !depth || !color || !scratch) return fail(RGS_E_INVALID, "null pointer");
+	char* buf;
+	if ((rc = grow(scratch, scratch_user, (size_t)n * sizeof(int32_t), buf, "tsdf scratch")) != RGS_OK) return rc;
+	return cuda_status(launch_scalable_integrate(*grid, make_scalable_cam(*grid, *cam, sdf_trunc), n, unit_coords, depth, color, call_id,
+	                                             reinterpret_cast<int32_t*>(buf), (cudaStream_t)cuda_stream),
+	                   "scalable integrate");
 }
 
 int32_t rgs_tsdf_integrate(const rgs_tsdf_grid* grid, const rgs_tsdf_camera* cam, int64_t n, const int32_t* block_coords, const float* depth,

@@ -1068,6 +1068,72 @@ torch::Tensor TsdfVertexNormals(const torch::Tensor& vertices, const torch::Tens
 	return normals;
 }
 
+// ---- bounded TSDF, Open3D's legacy ScalableTSDFVolume (rgs_scalable_*; Python side rade_gs_b200.tsdf.ScalableTSDFVolume) ------
+
+// rgb f32 [3,H,W], depth f32 [1,H,W] or [H,W], mask (None or H*W floats) -> (color uint8 [H,W,3], depth f32 [H,W])
+std::tuple<torch::Tensor, torch::Tensor> ScalableRgbd(const torch::Tensor& rgb, const torch::Tensor& depth, double depth_trunc,
+                                                     const c10::optional<torch::Tensor>& mask) {
+	const torch::Tensor c = arg(rgb, "rgb", torch::kFloat32, {3, -1, -1}, "[3, H, W]");
+	const int64_t H = c.size(1), W = c.size(2);
+	const torch::Tensor d = arg(depth, "depth", torch::kFloat32, {}, "", &c);
+	TORCH_CHECK(d.numel() == H * W && (d.dim() == 2 || (d.dim() == 3 && d.size(0) == 1)), "depth must be [1, H, W] or [H, W] like rgb ", c.sizes(),
+	            ", got ", d.sizes());
+	torch::Tensor m;
+	if (mask && mask->defined()) {
+		m = arg(*mask, "mask", torch::kFloat32, {}, "", &c);
+		TORCH_CHECK(m.numel() == H * W, "mask must have H * W = ", H * W, " values, got ", m.sizes());
+	}
+	TORCH_CHECK(H <= INT32_MAX && W <= INT32_MAX, "image too large");
+	const c10::cuda::CUDAGuard guard(c.device());
+	torch::Tensor col = new_empty({H, W, 3}, c.options().dtype(torch::kUInt8)), dout = new_empty({H, W}, c.options());
+	check(rgs_scalable_rgbd((int32_t)H, (int32_t)W, c.data_ptr<float>(), d.data_ptr<float>(), m.defined() ? m.data_ptr<float>() : nullptr, depth_trunc,
+	                        col.data_ptr<uint8_t>(), dout.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(col, dout);
+}
+
+// image f32 [3,H,W] -> uint8 [H,W,3] as save_img_u8 converts image * scale + offset
+torch::Tensor ScalableImageU8(const torch::Tensor& image, double scale, double offset) {
+	const torch::Tensor x = arg(image, "image", torch::kFloat32, {3, -1, -1}, "[3, H, W]");
+	TORCH_CHECK(x.size(1) <= INT32_MAX && x.size(2) <= INT32_MAX, "image too large");
+	const c10::cuda::CUDAGuard guard(x.device());
+	torch::Tensor out = new_empty({x.size(1), x.size(2), 3}, x.options().dtype(torch::kUInt8));
+	check(rgs_scalable_image_u8((int32_t)x.size(1), (int32_t)x.size(2), x.data_ptr<float>(), (float)scale, (float)offset, out.data_ptr<uint8_t>(),
+	                            at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
+// returns (number of touched units, or -1 when the frame-local hash is full; unit coordinates int32 [n, 3]; allocated units)
+std::tuple<int64_t, torch::Tensor, int64_t> ScalableTouch(const py::object& volume, const torch::Tensor& depth, const torch::Tensor& intrinsic,
+                                                          const torch::Tensor& extrinsic, double sdf_trunc) {
+	const torch::Tensor keys = grid_array(volume, "hash_keys", torch::kInt64);
+	const c10::cuda::CUDAGuard guard(keys.device());
+	const torch::Tensor d = arg(depth, "depth", torch::kFloat32, {-1, -1}, "[H, W]", &keys, REJECT);
+	const rgs_tsdf_grid g = tsdf_grid(volume);
+	const rgs_tsdf_camera c = tsdf_camera(d, intrinsic, extrinsic, 1.0, 1.0, 1.0);
+	torch::Tensor out = new_empty({g.frame_slots / 2, 3}, keys.options().dtype(torch::kInt32)), scratch = bytes(keys);
+	int64_t allocated = 0;
+	const int64_t n = rgs_scalable_touch(&g, &c, (float)sdf_trunc, d.data_ptr<float>(), out.data_ptr<int32_t>(), &allocated, resize_cb, &scratch,
+	                                     at::cuda::getCurrentCUDAStream().stream());
+	if (n == RGS_E_CAPACITY) return std::make_tuple((int64_t)-1, out.narrow(0, 0, 0), allocated);
+	check(n);
+	return std::make_tuple(n, out.narrow(0, 0, n).clone(), allocated);
+}
+
+void ScalableIntegrate(const py::object& volume, const torch::Tensor& unit_coords, const torch::Tensor& depth, const torch::Tensor& color,
+                       const torch::Tensor& intrinsic, const torch::Tensor& extrinsic, double sdf_trunc, int call_id) {
+	const torch::Tensor keys = grid_array(volume, "hash_keys", torch::kInt64);
+	const c10::cuda::CUDAGuard guard(keys.device());
+	arg(unit_coords, "unit_coords", torch::kInt32, {-1, 3}, "[N, 3]", &keys, REJECT);
+	const torch::Tensor d = arg(depth, "depth", torch::kFloat32, {-1, -1}, "[H, W]", &keys, REJECT),
+	                    col = arg(color, "color", torch::kUInt8, {-1, -1, 3}, "[H, W, 3]", &keys, REJECT);
+	TORCH_CHECK(col.size(0) == d.size(0) && col.size(1) == d.size(1), "color and depth must have the same [H, W]");
+	const rgs_tsdf_grid g = tsdf_grid(volume);
+	const rgs_tsdf_camera c = tsdf_camera(d, intrinsic, extrinsic, 1.0, 1.0, 1.0);
+	torch::Tensor scratch = bytes(keys);
+	check(rgs_scalable_integrate(&g, &c, (float)sdf_trunc, unit_coords.size(0), unit_coords.data_ptr<int32_t>(), d.data_ptr<float>(), col.data_ptr<uint8_t>(),
+	                             call_id, resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
+}
+
 // ---- DTU evaluation (rgs_dtu_*; Python side rade_gs_b200.dtu_eval) -------------------------------------------------------
 
 // vertices f64 [V,3], faces int32 [F,3] -> the vertices followed by the surface samples, f64 [V + S, 3]
@@ -1534,6 +1600,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("tsdf_active_blocks", &TsdfActiveBlocks);
 	m.def("tsdf_extract", &TsdfExtract);
 	m.def("tsdf_vertex_normals", &TsdfVertexNormals);
+	// bounded TSDF (Open3D's legacy ScalableTSDFVolume): a private submodule behind rade_gs_b200.tsdf.ScalableTSDFVolume
+	py::module_ sc = m.def_submodule("_scalable_tsdf", "bounded-TSDF stages behind rade_gs_b200.tsdf.ScalableTSDFVolume");
+	sc.def("rgbd", &ScalableRgbd, py::arg("rgb"), py::arg("depth"), py::arg("depth_trunc"), py::arg("mask") = py::none());
+	sc.def("image_u8", &ScalableImageU8, py::arg("image"), py::arg("scale") = 1.0, py::arg("offset") = 0.0);
+	sc.def("touch", &ScalableTouch, py::arg("volume"), py::arg("depth"), py::arg("intrinsic"), py::arg("extrinsic"), py::arg("sdf_trunc"));
+	sc.def("integrate", &ScalableIntegrate, py::arg("volume"), py::arg("unit_coords"), py::arg("depth"), py::arg("color"), py::arg("intrinsic"),
+	       py::arg("extrinsic"), py::arg("sdf_trunc"), py::arg("call_id"));
 	m.def("dtu_sample_mesh", &DtuSampleMesh, py::arg("vertices"), py::arg("faces"), py::arg("density"));
 	m.def("dtu_radius_downsample", &DtuRadiusDownsample, py::arg("points"), py::arg("radius"));
 	m.def("dtu_nearest", &DtuNearest, py::arg("reference"), py::arg("query"));

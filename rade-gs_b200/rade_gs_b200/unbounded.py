@@ -9,6 +9,14 @@ and trimesh / Open3D on the host.  It is the TSDF path for unbounded captures (M
 
 ``extract_mesh_unbounded_maps`` takes the maps and cameras directly, for callers without a ``GaussianModel``.
 
+The same extractor has the reference's bounded half (utils/mesh_utils.py:118-160, :272-285)::
+
+    ex.export_image(out_dir)                                # renders/, gt/, vis/depth_*.tiff, vis/normal_*.png
+    mesh = ex.extract_mesh_bounded(voxel_size=0.004, sdf_trunc=0.02, depth_trunc=3)   # tsdf.ScalableTSDFVolume
+
+where the reference's own class fails: it reads ``gt_alpha_mask`` (RaDe-GS's Camera holds ``gt_mask``; that is read
+here) and calls ``save_img_u8`` / ``save_img_f32`` without importing them.
+
 Stages (the arithmetic of each is fixed bit for bit by the contract at ``rgs_unbounded_*`` in include/rgs_b200.h; the
 kernels are in csrc/rgs_unbounded.cu):
 
@@ -32,18 +40,22 @@ Deliberate differences from the reference:
     free space (positive SDF);
   * ``post_process_mesh`` with fewer than ``cluster_to_keep`` clusters keeps every cluster of at least 50 triangles (the
     reference raises IndexError);
-  * ``reconstruction()`` keeps only the maps the mesh reads (RGB and median depth) and keeps them on the GPU.
+  * ``reconstruction()`` keeps only the maps the meshes and the export read (RGB, median depth and normals) and keeps
+    them on the GPU; the alpha and depth-normal maps are not kept, so ``export_image`` writes no depth-normal PNGs;
+  * the bounded mesh (see ``tsdf.ScalableTSDFVolume``) uses the repository's watertight triangle table, its own
+    deterministic vertex and triangle order and fp32 colour averages, and leaves the stored depth maps unmasked.
 """
 from __future__ import annotations
 
 import math
+import os
 
 import numpy as np
 import torch
 
 from diff_gaussian_rasterization import _C
 
-from .tsdf import TriangleMesh
+from .tsdf import ScalableTSDFVolume, TriangleMesh, rgbd_from_color_and_depth
 
 CROP = 512                # the reference's crop edge (marching_cubes_with_contraction's cropN)
 MAX_RANGE = 32.0          # world-space clip of the vertices (its max_range)
@@ -172,6 +184,15 @@ def extract_mesh_unbounded_maps(depths: torch.Tensor, rgbs: torch.Tensor, world_
     return TriangleMesh(world, triangles, colors)
 
 
+def open3d_camera(cam):
+    """(intrinsic 3x3 float64, world->camera extrinsic 4x4 float64) of a view as the reference's ``to_cam_open3d`` builds
+    them: cx = W / 2, cy = H / 2, fx = W / (2 tan(FoVx / 2)), fy = H / (2 tan(FoVy / 2)), extrinsic =
+    world_view_transform^T."""
+    W, H = cam.image_width, cam.image_height
+    K = np.array([[W / (2 * math.tan(cam.FoVx / 2.)), 0, W / 2], [0, H / (2 * math.tan(cam.FoVy / 2.)), H / 2], [0, 0, 1]], np.float64)
+    return K, np.asarray(cam.world_view_transform.T.detach().cpu().numpy(), np.float64)
+
+
 def post_process_mesh(mesh: TriangleMesh, cluster_to_keep: int = 1000) -> TriangleMesh:
     """Drop small connected clusters (triangles joined by shared edges): keep clusters of at least
     max(k-th largest size, 50) triangles, then drop unreferenced vertices and degenerate triangles.  With fewer than
@@ -207,25 +228,76 @@ class GaussianExtractor:
     def clean(self):
         self.depthmaps = []
         self.rgbmaps = []
+        self.normals = []
         self.viewpoint_stack = []
 
     @torch.no_grad()
     def reconstruction(self, viewpoint_stack):
-        """Render every view; keep render()'s "render" [3, H, W] and "median_depth" [1, H, W] on the GPU."""
+        """Render every view; keep render()'s "render" [3, H, W], "median_depth" [1, H, W] and the normalised "normal"
+        [3, H, W] on the GPU: 7 floats per pixel per view (the normals, which only ``export_image`` reads, are 3 of them; they
+        are kept when render() returns "normal" for every view)."""
         self.clean()
         self.viewpoint_stack = list(viewpoint_stack)
         if not self.viewpoint_stack:
             raise ValueError("reconstruction needs at least one view")
-        rgbs, depths = [], []
+        rgbs, depths, normals = [], [], []
         for cam in self.viewpoint_stack:
             pkg = self._render(cam, self.gaussians, self._pipe, self._background, self.kernel_size)
             rgbs.append(pkg["render"].detach().float())
             depths.append(pkg["median_depth"].detach().float())
+            if "normal" in pkg:
+                normals.append(torch.nn.functional.normalize(pkg["normal"].detach().float(), dim=0))
         shapes = {tuple(d.shape[-2:]) for d in depths}
         if len(shapes) != 1:
             raise ValueError(f"all views must have one size, got {sorted(shapes)}")
         self.rgbmaps = torch.stack(rgbs)
         self.depthmaps = torch.stack(depths)
+        self.normals = torch.stack(normals) if len(normals) == len(depths) else []
+
+    @torch.no_grad()
+    def extract_mesh_bounded(self, voxel_size=0.004, sdf_trunc=0.02, depth_trunc=3, mask_backgrond=True) -> TriangleMesh:
+        """The bounded TSDF mesh "used in the paper": every view fused into a ``tsdf.ScalableTSDFVolume`` with the
+        reference's camera (cx = W / 2, cy = H / 2, fx = W / (2 tan(FoVx / 2)), extrinsic = world_view_transform^T).
+        With ``mask_backgrond`` (the reference's spelling), depth is dropped where the camera's ``gt_mask`` < 0.5.  The
+        stored depth maps are not changed (the reference zeroes them in place, so its later ``export_image`` writes the
+        masked depth)."""
+        if not len(self.viewpoint_stack):
+            raise ValueError("call reconstruction() first")
+        volume = ScalableTSDFVolume(voxel_length=voxel_size, sdf_trunc=sdf_trunc)
+        for i, cam in enumerate(self.viewpoint_stack):
+            mask = getattr(cam, "gt_mask", None) if mask_backgrond else None
+            color, depth = rgbd_from_color_and_depth(self.rgbmaps[i], self.depthmaps[i], depth_trunc, mask)
+            volume.integrate(color, depth, *open3d_camera(cam))
+        return volume.extract_triangle_mesh()
+
+    @torch.no_grad()
+    def export_image(self, path):
+        """Write ``renders/`` and ``gt/`` (8-bit PNGs of the render and of ``original_image[:3]``), ``vis/depth_*.tiff``
+        (float32 median depth) and ``vis/normal_*.png`` (normal * 0.5 + 0.5) as the reference's save_img_u8 /
+        save_img_f32 write them: (clip(nan_to_num(x), 0, 1) * 255).astype(uint8) on the GPU, then PIL encodes.  The
+        reference's ``vis/depth_normal_*.png`` is not written: its depth normals are not kept."""
+        from PIL import Image
+
+        if not len(self.viewpoint_stack):
+            raise ValueError("call reconstruction() first")
+        if len(self.normals) != len(self.viewpoint_stack):
+            raise ValueError("export_image needs the normal maps: render() must return \"normal\" for every view")
+        S = _C._scalable_tsdf
+        dirs = {k: os.path.join(path, k) for k in ("renders", "gt", "vis")}
+        for d in dirs.values():
+            os.makedirs(d, exist_ok=True)
+
+        def png(img, name):
+            with open(name, "wb") as f:
+                Image.fromarray(img.cpu().numpy()).save(f, "PNG")
+
+        for idx, cam in enumerate(self.viewpoint_stack):
+            gt = cam.original_image[0:3].detach().to(self.rgbmaps.device, torch.float32).contiguous()
+            png(S.image_u8(gt), os.path.join(dirs["gt"], f"{idx:05d}.png"))
+            png(S.image_u8(self.rgbmaps[idx]), os.path.join(dirs["renders"], f"{idx:05d}.png"))
+            with open(os.path.join(dirs["vis"], f"depth_{idx:05d}.tiff"), "wb") as f:
+                Image.fromarray(torch.nan_to_num(self.depthmaps[idx][0]).cpu().numpy()).save(f, "TIFF")
+            png(S.image_u8(self.normals[idx], 0.5, 0.5), os.path.join(dirs["vis"], f"normal_{idx:05d}.png"))
 
     @torch.no_grad()
     def extract_mesh_unbounded(self, resolution: int = 1024) -> TriangleMesh:
