@@ -609,6 +609,56 @@ int32_t rgs_tnt_voxel_downsample(int64_t N, const double* points, double voxel, 
 int32_t rgs_tnt_icp_moments(int64_t N, const double* source, int64_t M, const double* target, const double* dist, const int64_t* index, double threshold,
                             double* moments, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
 
+/* ---- Tanks and Temples mesh cull (reference eval_tnt/cull_mesh.py: extract_depth_from_mesh, Mesher.point_masks) ----
+ * Every operation below is one IEEE fp32 operation rounded to nearest on its own, in the order written (no contraction);
+ * so every output bit is fixed.  w2c (host, fp32 [12]) is rows 0..2 of the world-to-camera matrix, row-major; the Python
+ * layer (rade_gs_b200.tnt_cull) forms it as the fp64 inverse of the fp32-rounded 4x4 pose, rounded to fp32.  A point p
+ * maps to camera coordinates X_r = ((m_r0 x + m_r1 y) + m_r2 z) + m_r3.  The camera looks down +Z (OpenCV): pixel column
+ * u = fx X / Z + cx, row v = fy Y / Z + cy, the model of pyrender's IntrinsicsCamera.
+ *
+ * rgs_tnt_mesh_depth: vertices fp32 [V, 3] and faces int32 [F, 3] on the device; depth fp32 [H, W] (device) receives the
+ *   camera-space Z of the nearest surface at each pixel centre, 0 where nothing is drawn.  Homogeneous rasterization, with
+ *   no back-face culling and no clip:
+ *   - A, B, C: the face's vertices in camera coordinates.  The face draws nothing when a coordinate is not finite, when
+ *     every Z < znear, when every Z > zfar, or when num = ((n_x A_x + n_y A_y) + n_z A_z) is 0 (zero-area or edge-on
+ *     faces), with n = (B - A) x (C - A) and a x b = (a_y b_z - a_z b_y, a_z b_x - a_x b_z, a_x b_y - a_y b_x).
+ *   - Bounding box, of the face clipped at Z = znear: for each edge (P, Q) in the order (A, B), (B, C), (C, A), the point
+ *     P when P_z >= znear, then, when exactly one of P_z, Q_z is < znear, the crossing point P + s (Q - P) with
+ *     s = (znear - P_z) / (Q_z - P_z), each coordinate P_i + (s (Q_i - P_i)).  Each point gives u = ((fx X) / Z) + cx and
+ *     v = ((fy Y) / Z) + cy; umin..vmax their extremes clamped with fmin(fmax(., -1), W) (H for v); the box is columns
+ *     max(floor(umin - 0.5), 0) .. min(ceil(umax - 0.5), W - 1), rows likewise; an empty box draws nothing.  The box only
+ *     limits the pixels tested: coverage is decided by the edge functions alone.
+ *   - Edge vectors, for (P, Q) = (A, B), (B, C), (C, A): c = (P + Q) x (Q - P), negated when num < 0.  Swapping P and Q
+ *     negates c exactly, so two faces sharing an edge evaluate exactly opposite edge functions on it.
+ *   - Pixel (x, y) of the box: dx = ((x + 0.5) - cx) / fx, dy = ((y + 0.5) - cy) / fy, e(c) = ((c_x dx) + (c_y dy)) + c_z.
+ *     It is inside when for every edge e > 0, or e == 0 and c is lexicographically positive (c_x > 0, or c_x == 0 and
+ *     c_y > 0, or c_x == c_y == 0 and c_z > 0): a pixel centre on a shared edge is drawn by exactly one of the two faces.
+ *   - Its depth is Z = num / e(n), the ray's hit on the face's plane (perspective-correct); kept when znear <= Z <= zfar.
+ *     The smallest kept Z per pixel wins (atomicMin on the bits of the positive float), so the result does not depend on
+ *     launch order, thread count or the work split, and two calls give identical bits.
+ *   Work split (no effect on the result): a box of at most 16 pixels is drawn by the face's own thread, one of at most
+ *   4096 by one CTA, larger ones by stripes of the whole grid.
+ *   Errors (RGS_E_INVALID with a message): V or F outside [0, 2^31), H or W outside [1, 32768], not 0 < znear < zfar,
+ *   non-finite intrinsics or fx, fy == 0, and a face index outside [0, V) (a device flag, read after drawing: one host read
+ *   per call when F > 0).  Scratch through `scratch` (8 bytes per face plus a few).
+ *
+ * rgs_tnt_visibility_count: points fp32 [N, 3], depth fp32 [H, W] (device, H, W >= 2), counts int32 [N] (device, added
+ *   to).  Mesher.point_masks for one view, eps the occlusion margin (0.005 in the reference):
+ *   - (X, Y, Z) as above; z = Z + 1e-8f; u = ((fx X) + (cx Z)) / z; v = ((fy Y) + (cy Z)) / z  (K @ cam with the zero
+ *     terms dropped; torch's matmul may fuse or reorder these products, which moves u, v, z by an ulp);
+ *   - in_frustum = u >= 0 and u <= W - 1 and v >= 0 and v <= H - 1 and z > 0; outside it the point is not counted;
+ *   - the grid: g_x = ((u * r_w) * 2) - 1 with r_w = 1.0f / (float)(W - 1) (torch on CUDA multiplies by the fp32
+ *     reciprocal of a host-scalar divisor; on the CPU it divides), g_y likewise;
+ *   - grid_sample(bilinear, padding_mode='border', align_corners=True): ix = ((g_x + 1) / 2) * (W - 1), clipped to
+ *     min(W - 1, max(ix, 0)), iy likewise; x0 = floor(ix), y0 = floor(iy), x1 = x0 + 1, y1 = y0 + 1; weights
+ *     nw = (x1 - ix)(y1 - iy), ne = (ix - x0)(y1 - iy), sw = (x1 - ix)(iy - y0), se = (ix - x0)(iy - y0); the sample is
+ *     s = 0, then s = s + D[y][x] * w for nw, ne, sw, se in that order, each corner skipped when x1 = W or y1 = H;
+ *   - seen = in_frustum and (s > 0 ? z < s + eps : true); counts[n] += seen. */
+int32_t rgs_tnt_mesh_depth(int64_t V, const float* vertices, int64_t F, const int32_t* faces, const float* w2c, float fx, float fy, float cx, float cy,
+                           int32_t H, int32_t W, float znear, float zfar, float* depth, rgs_resize_fn scratch, void* scratch_user, void* cuda_stream);
+int32_t rgs_tnt_visibility_count(int64_t N, const float* points, const float* depth, const float* w2c, float fx, float fy, float cx, float cy, int32_t H,
+                                 int32_t W, float eps, int32_t* counts, void* cuda_stream);
+
 /* ---- Tetrahedra mesh extraction: mesh_extract_tetrahedra.py, utils/tetmesh.py and GaussianModel.get_tetra_points ----
  * Arrays are fp32 / int32 / int64 on the device, row-major.  Stages 2-5 are fixed bit for bit: every fp32 operation below is
  * one IEEE operation rounded to nearest on its own (no FMA contraction unless an fma is written), in the order written;

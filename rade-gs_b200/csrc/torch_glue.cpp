@@ -1509,6 +1509,39 @@ std::tuple<torch::Tensor, torch::Tensor, py::dict> UnboundedClusters(int64_t num
 	return std::make_tuple(rows(vidx, torch::kInt32, out.num_vertices, {}), rows(tout, torch::kInt32, out.num_triangles, {3}), st);
 }
 
+// ---- Tanks and Temples mesh cull (rgs_tnt_mesh_depth / rgs_tnt_visibility_count; Python side rade_gs_b200.tnt_cull) --------
+
+std::array<float, 12> w2c_rows(const std::vector<double>& w2c) {
+	TORCH_CHECK(w2c.size() == 12, "w2c must hold rows 0..2 of the 4x4 (12 values), got ", w2c.size());
+	std::array<float, 12> m;
+	for (int k = 0; k < 12; k++) m[k] = (float)w2c[k];
+	return m;
+}
+
+// vertices f32 [V,3], faces int32 [F,3] -> depth f32 [H,W]
+torch::Tensor TntMeshDepth(const torch::Tensor& vertices, const torch::Tensor& faces, const std::vector<double>& w2c, double fx, double fy, double cx,
+                           double cy, int64_t H, int64_t W, double znear, double zfar) {
+	const torch::Tensor v = arg(vertices, "vertices", torch::kFloat32, {-1, 3}, "[V, 3]"), f = arg(faces, "faces", torch::kInt32, {-1, 3}, "[F, 3]", &v);
+	const c10::cuda::CUDAGuard guard(v.device());
+	const std::array<float, 12> m = w2c_rows(w2c);
+	TORCH_CHECK(H > 0 && W > 0 && H <= 32768 && W <= 32768, "H and W must lie in [1, 32768], got ", H, " x ", W);
+	torch::Tensor depth = new_empty({H, W}, v.options()), scratch = bytes(v);
+	check(rgs_tnt_mesh_depth(v.size(0), v.data_ptr<float>(), f.size(0), f.data_ptr<int32_t>(), m.data(), (float)fx, (float)fy, (float)cx, (float)cy, (int32_t)H,
+	                         (int32_t)W, (float)znear, (float)zfar, depth.data_ptr<float>(), resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
+	return depth;
+}
+
+// points f32 [N,3], depth f32 [H,W], counts int32 [N] (added to in place)
+void TntVisibilityCount(const torch::Tensor& points, const torch::Tensor& depth, const std::vector<double>& w2c, double fx, double fy, double cx, double cy,
+                        double eps, const torch::Tensor& counts) {
+	const torch::Tensor p = arg(points, "points", torch::kFloat32, {-1, 3}, "[N, 3]"), d = arg(depth, "depth", torch::kFloat32, {-1, -1}, "[H, W]", &p),
+	                    c = arg(counts, "counts", torch::kInt32, {p.size(0)}, "[N] like points", &p, REJECT);
+	const c10::cuda::CUDAGuard guard(p.device());
+	const std::array<float, 12> m = w2c_rows(w2c);
+	check(rgs_tnt_visibility_count(p.size(0), p.data_ptr<float>(), d.data_ptr<float>(), m.data(), (float)fx, (float)fy, (float)cx, (float)cy, (int32_t)d.size(0),
+	                               (int32_t)d.size(1), (float)eps, c.data_ptr<int32_t>(), at::cuda::getCurrentCUDAStream().stream()));
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1641,6 +1674,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	ub.def("mcubes", &UnboundedMcubes, py::arg("sdf"), py::arg("lo"), py::arg("spacing"));
 	ub.def("merge", &UnboundedMerge, py::arg("vertices"), py::arg("triangles"));
 	ub.def("clusters", &UnboundedClusters, py::arg("num_vertices"), py::arg("triangles"), py::arg("cluster_to_keep"));
+	// Tanks and Temples mesh cull: a private submodule behind rade_gs_b200.tnt_cull
+	py::module_ tc = m.def_submodule("_tnt_cull", "depth rasterizer and visibility count behind rade_gs_b200.tnt_cull");
+	tc.def("mesh_depth", &TntMeshDepth, py::arg("vertices"), py::arg("faces"), py::arg("w2c"), py::arg("fx"), py::arg("fy"), py::arg("cx"), py::arg("cy"),
+	       py::arg("H"), py::arg("W"), py::arg("znear"), py::arg("zfar"));
+	tc.def("visibility_count", &TntVisibilityCount, py::arg("points"), py::arg("depth"), py::arg("w2c"), py::arg("fx"), py::arg("fy"), py::arg("cx"),
+	       py::arg("cy"), py::arg("eps"), py::arg("counts"));
 	m.def("grad_stride",[](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });
