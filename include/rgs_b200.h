@@ -274,6 +274,20 @@ int32_t rgs_normal_consistency(int32_t H, int32_t W, int32_t from_depth, float i
                                const float* rendered_normal, const float* map_expected, const float* map_median,
                                float w_expected, float w_median, double* loss_sum, float* d_normal, float* d_expected,
                                float* d_median, void* cuda_stream);
+/* Row-sharded form (multi-GPU, ABI 3): rgs_normal_consistency for loss rows [row_lo, row_hi) of an H x W image, 0 <= row_lo <=
+ * row_hi <= H.  Every buffer is a window of whole rows, planar [C, rows, W]:
+ *   map_expected, map_median  rows [max(0, row_lo - 2), min(H, row_hi + 2))   (the stencils of the range and one row beyond)
+ *   rendered_normal           rows [max(0, row_lo - 1), min(H, row_hi + 1))
+ *   d_normal, d_expected, d_median                                             rows [row_lo, row_hi), fully written
+ * Rays, the image border (the outermost pixels keep a zero normal: error 1) and every stencil use the GLOBAL row index.  A pixel's
+ * gradient is complete: the stencils one row outside the range that read it are evaluated here too (their loss is not counted),
+ * so no gradient crosses a slab boundary.  Every per-pixel output is bit-identical to the whole-image call's value at that pixel;
+ * loss_sum (zeroed by the call) sums the range's rows and differs from the whole image's rows' sum in summation order only.
+ * row_lo == row_hi launches nothing and leaves loss_sum = 0. */
+int32_t rgs_normal_consistency_rows(int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, int32_t from_depth, float inv_fx, float inv_fy,
+                                    float cx, float cy, const float* rendered_normal, const float* map_expected, const float* map_median,
+                                    float w_expected, float w_median, double* loss_sum, float* d_normal, float* d_expected,
+                                    float* d_median, void* cuda_stream);
 
 /* ---- decoupled-appearance L1 loss (train.py:37-58 with GOF's AppearanceNetwork, scene/appearance_network.py) ----
  * The image is planar fp32 [3, H0, W0], H0, W0 >= 32.  The crop is H = H0 / 32 * 32 rows by W = W0 / 32 * 32 columns at

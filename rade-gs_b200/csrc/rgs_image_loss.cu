@@ -14,7 +14,7 @@
 //
 // All maps are planar fp32 [C,H,W] as the rasterizer writes them.  Scalar sums are accumulated in double.
 //
-// This file also holds the C-ABI entry points rgs_ssim_l1_* and rgs_normal_consistency (include/rgs_b200.h).
+// This file also holds the C-ABI entry points rgs_ssim_l1_* and rgs_normal_consistency* (include/rgs_b200.h).
 #include "rgs_common.cuh"
 
 namespace rgs {
@@ -183,22 +183,30 @@ __device__ __forceinline__ V3f vsub(V3f a, V3f b) { return {a.x - b.x, a.y - b.y
 __device__ __forceinline__ V3f vcross(V3f a, V3f b) { return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x}; }
 __device__ __forceinline__ float vdot(V3f a, V3f b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 
+// The rows one launch covers.  Loss rows [lo, hi) are counted and their gradients written; blocks start at tile row by0.  The
+// buffers are row windows of the image: the two maps hold rows [m_lo, m_lo + m_rows), the rendered normal [n_lo, n_lo + n_rows),
+// the outputs [lo, hi).  The whole image is lo = 0, hi = H with every window the whole image.
+struct NcRows {
+	int lo, hi, by0, m_lo, m_rows, n_lo, n_rows;
+};
+
 template <bool FROM_DEPTH>
-__global__ void __launch_bounds__(256) normal_consistency_kernel(int H, int W, float inv_fx, float inv_fy, float cx, float cy,
+__global__ void __launch_bounds__(256) normal_consistency_kernel(int H, int W, NcRows R, float inv_fx, float inv_fy, float cx, float cy,
                                                                   const float* __restrict__ rendered_normal, const float* __restrict__ map_e,
                                                                   const float* __restrict__ map_m, float w_e, float w_m, double* __restrict__ loss_sum,
                                                                   float* __restrict__ d_normal, float* __restrict__ d_e, float* __restrict__ d_m) {
 	__shared__ V3f sP[2][NP][NP];
 	__shared__ V3f sGx[2][NG][NG], sGy[2][NG][NG];  // dL/d(dx), dL/d(dy) of the stencil centred on that pixel
 	__shared__ float s_red[8];
-	const int x0 = blockIdx.x * NT, y0 = blockIdx.y * NT;
-	const size_t HW = (size_t)H * W;
+	const int x0 = blockIdx.x * NT, y0 = (blockIdx.y + R.by0) * NT;
+	const size_t MP = (size_t)R.m_rows * W, NPL = (size_t)R.n_rows * W, OP = (size_t)(R.hi - R.lo) * W;  // plane strides
 	for (int i = threadIdx.x; i < NP * NP; i += 256) {
 		const int r = i / NP, c = i - r * NP;
 		const int gy = y0 + r - 2, gx = x0 + c - 2;
 		V3f p0 = {0.f, 0.f, 0.f}, p1 = {0.f, 0.f, 0.f};
-		if (gy >= 0 && gy < H && gx >= 0 && gx < W) {
-			const size_t o = (size_t)gy * W + gx;
+		// rows outside the window feed only stencils whose results are not used
+		if (gy >= R.m_lo && gy < R.m_lo + R.m_rows && gx >= 0 && gx < W) {
+			const size_t o = (size_t)(gy - R.m_lo) * W + gx;
 			if (FROM_DEPTH) {
 				// rays_d = K^-1 (x + 0.5, y + 0.5, 1) (graphics_utils.py:101-109), points = depth * rays_d
 				const float rx = inv_fx * ((float)gx + 0.5f) + cx, ry = inv_fy * ((float)gy + 0.5f) + cy;
@@ -206,8 +214,8 @@ __global__ void __launch_bounds__(256) normal_consistency_kernel(int H, int W, f
 				p0 = {d0 * rx, d0 * ry, d0};
 				p1 = {d1 * rx, d1 * ry, d1};
 			} else {
-				p0 = {__ldg(map_e + o), __ldg(map_e + HW + o), __ldg(map_e + 2 * HW + o)};
-				p1 = {__ldg(map_m + o), __ldg(map_m + HW + o), __ldg(map_m + 2 * HW + o)};
+				p0 = {__ldg(map_e + o), __ldg(map_e + MP + o), __ldg(map_e + 2 * MP + o)};
+				p1 = {__ldg(map_m + o), __ldg(map_m + MP + o), __ldg(map_m + 2 * MP + o)};
 			}
 		}
 		sP[0][r][c] = p0;
@@ -220,11 +228,11 @@ __global__ void __launch_bounds__(256) normal_consistency_kernel(int H, int W, f
 		const int gy = y0 + r - 1, gx = x0 + c - 1;
 		const bool in_image = gy >= 0 && gy < H && gx >= 0 && gx < W;
 		const bool interior = gy >= 1 && gy < H - 1 && gx >= 1 && gx < W - 1;  // output[..., 1:-1, 1:-1] (graphics_utils.py:119)
-		const bool own = in_image && r >= 1 && r <= NT && c >= 1 && c <= NT;
+		const bool own = in_image && r >= 1 && r <= NT && c >= 1 && c <= NT && gy >= R.lo && gy < R.hi;
 		V3f rn = {0.f, 0.f, 0.f};
-		if (interior) {
-			const size_t o = (size_t)gy * W + gx;
-			rn = {__ldg(rendered_normal + o), __ldg(rendered_normal + HW + o), __ldg(rendered_normal + 2 * HW + o)};
+		if (interior && gy >= R.n_lo && gy < R.n_lo + R.n_rows) {
+			const size_t o = (size_t)(gy - R.n_lo) * W + gx;
+			rn = {__ldg(rendered_normal + o), __ldg(rendered_normal + NPL + o), __ldg(rendered_normal + 2 * NPL + o)};
 		}
 		V3f dn = {0.f, 0.f, 0.f};
 #pragma unroll
@@ -257,17 +265,17 @@ __global__ void __launch_bounds__(256) normal_consistency_kernel(int H, int W, f
 			sGy[k][r][c] = gdy;
 		}
 		if (own) {
-			const size_t o = (size_t)gy * W + gx;
-			d_normal[o] = dn.x; d_normal[HW + o] = dn.y; d_normal[2 * HW + o] = dn.z;
+			const size_t o = (size_t)(gy - R.lo) * W + gx;
+			d_normal[o] = dn.x; d_normal[OP + o] = dn.y; d_normal[2 * OP + o] = dn.z;
 		}
 	}
 	__syncthreads();
 	{
 		const int tx = threadIdx.x & (NT - 1), ty = threadIdx.x / NT;
 		const int gy = y0 + ty, gx = x0 + tx;
-		if (gy < H && gx < W) {
+		if (gy >= R.lo && gy < R.hi && gx < W) {
 			const int r = ty + 1, c = tx + 1;  // position in the NG region
-			const size_t o = (size_t)gy * W + gx;
+			const size_t o = (size_t)(gy - R.lo) * W + gx;
 #pragma unroll
 			for (int k = 0; k < 2; k++) {
 				// the stencil centred one row up (r-1) reads this pixel as its +row neighbour, the one a row down as its -row one
@@ -278,7 +286,7 @@ __global__ void __launch_bounds__(256) normal_consistency_kernel(int H, int W, f
 					const float rx = inv_fx * ((float)gx + 0.5f) + cx, ry = inv_fy * ((float)gy + 0.5f) + cy;
 					dst[o] = g.x * rx + g.y * ry + g.z;
 				} else {
-					dst[o] = g.x; dst[HW + o] = g.y; dst[2 * HW + o] = g.z;
+					dst[o] = g.x; dst[OP + o] = g.y; dst[2 * OP + o] = g.z;
 				}
 			}
 		}
@@ -348,22 +356,39 @@ int32_t rgs_ssim_l1_backward(int32_t planes, int32_t H, int32_t W, const float* 
 	return rgs_ssim_l1_backward_rows(planes, H, W, 0, H, img, gt, dmaps, w_ssim, w_l1, upstream, d_img, cuda_stream);
 }
 
+int32_t rgs_normal_consistency_rows(int32_t H, int32_t W, int32_t row_lo, int32_t row_hi, int32_t from_depth, float inv_fx, float inv_fy, float cx,
+                                    float cy, const float* rendered_normal, const float* map_expected, const float* map_median, float w_expected,
+                                    float w_median, double* loss_sum, float* d_normal, float* d_expected, float* d_median, void* cuda_stream) {
+	if (H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");
+	if (row_lo < 0 || row_hi > H || row_lo > row_hi) return fail(RGS_E_INVALID, "row range out of the image");
+	if (!loss_sum) return fail(RGS_E_INVALID, "null pointer");
+	const cudaStream_t s = (cudaStream_t)cuda_stream;
+	cudaMemsetAsync(loss_sum, 0, sizeof(double), s);
+	if (row_hi > row_lo) {
+		if (!rendered_normal || !map_expected || !map_median || !d_normal || !d_expected || !d_median) return fail(RGS_E_INVALID, "null pointer");
+		NcRows R;
+		R.lo = row_lo; R.hi = row_hi; R.by0 = row_lo / NT;
+		R.m_lo = max(0, row_lo - 2); R.m_rows = min(H, row_hi + 2) - R.m_lo;
+		R.n_lo = max(0, row_lo - 1); R.n_rows = min(H, row_hi + 1) - R.n_lo;
+		const dim3 grid((W + NT - 1) / NT, (row_hi + NT - 1) / NT - R.by0);
+		if (from_depth)
+			normal_consistency_kernel<true><<<grid, 256, 0, s>>>(H, W, R, inv_fx, inv_fy, cx, cy, rendered_normal, map_expected, map_median, w_expected,
+			                                                     w_median, loss_sum, d_normal, d_expected, d_median);
+		else
+			normal_consistency_kernel<false><<<grid, 256, 0, s>>>(H, W, R, inv_fx, inv_fy, cx, cy, rendered_normal, map_expected, map_median, w_expected,
+			                                                      w_median, loss_sum, d_normal, d_expected, d_median);
+		count_launch();
+	}
+	return cuda_status(cudaGetLastError(), "normal consistency");
+}
+
 int32_t rgs_normal_consistency(int32_t H, int32_t W, int32_t from_depth, float inv_fx, float inv_fy, float cx, float cy, const float* rendered_normal,
                                const float* map_expected, const float* map_median, float w_expected, float w_median, double* loss_sum,
                                float* d_normal, float* d_expected, float* d_median, void* cuda_stream) {
 	if (H <= 0 || W <= 0) return fail(RGS_E_INVALID, "image size must be positive");
 	if (!rendered_normal || !map_expected || !map_median || !loss_sum || !d_normal || !d_expected || !d_median) return fail(RGS_E_INVALID, "null pointer");
-	const cudaStream_t s = (cudaStream_t)cuda_stream;
-	cudaMemsetAsync(loss_sum, 0, sizeof(double), s);
-	const dim3 grid((W + NT - 1) / NT, (H + NT - 1) / NT);
-	if (from_depth)
-		normal_consistency_kernel<true><<<grid, 256, 0, s>>>(H, W, inv_fx, inv_fy, cx, cy, rendered_normal, map_expected, map_median, w_expected, w_median,
-		                                                     loss_sum, d_normal, d_expected, d_median);
-	else
-		normal_consistency_kernel<false><<<grid, 256, 0, s>>>(H, W, inv_fx, inv_fy, cx, cy, rendered_normal, map_expected, map_median, w_expected, w_median,
-		                                                      loss_sum, d_normal, d_expected, d_median);
-	count_launch();
-	return cuda_status(cudaGetLastError(), "normal consistency");
+	return rgs_normal_consistency_rows(H, W, 0, H, from_depth, inv_fx, inv_fy, cx, cy, rendered_normal, map_expected, map_median, w_expected, w_median,
+	                                   loss_sum, d_normal, d_expected, d_median, cuda_stream);
 }
 
 }  // extern "C"

@@ -704,6 +704,33 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> NormalCon
 	return std::make_tuple(loss, dn, de.view(map_expected.sizes()), dm.view(map_median.sizes()));
 }
 
+// Row-sharded form: loss rows [row_lo, row_hi) of an H-row image.  The maps hold rows [row_lo - 2, row_hi + 2) and the normal
+// rows [row_lo - 1, row_hi + 1), both clipped to the image; returns (loss_sum [1] float64, d_normal, d_expected, d_median), each
+// gradient [C, row_hi - row_lo, W].
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> NormalConsistencyRows(
+    const torch::Tensor& rendered_normal, const torch::Tensor& map_expected, const torch::Tensor& map_median, const bool from_depth, const double inv_fx,
+    const double inv_fy, const double cx, const double cy, const double w_expected, const double w_median, const int64_t H, const int64_t row_lo,
+    const int64_t row_hi) {
+	TORCH_CHECK(H > 0 && 0 <= row_lo && row_lo <= row_hi && row_hi <= H, "normal consistency rows: need 0 <= row_lo <= row_hi <= H, got [", row_lo, ", ",
+	            row_hi, ") of ", H);
+	const int64_t C = from_depth ? 1 : 3;
+	const int64_t m_rows = std::min(H, row_hi + 2) - std::max<int64_t>(0, row_lo - 2), n_rows = std::min(H, row_hi + 1) - std::max<int64_t>(0, row_lo - 1);
+	const torch::Tensor n = arg(rendered_normal, "rendered_normal", torch::kFloat32, {3, n_rows, -1}, "[3, rows row_lo - 1 .. row_hi + 1, W]");
+	const char* map_shape = from_depth ? "[1, rows row_lo - 2 .. row_hi + 2, W]" : "[3, rows row_lo - 2 .. row_hi + 2, W]";
+	const int64_t W = n.size(2);
+	const torch::Tensor e = arg(map_expected, "expected map", torch::kFloat32, {C, m_rows, W}, map_shape, &n),
+	                    m = arg(map_median, "median map", torch::kFloat32, {C, m_rows, W}, map_shape, &n);
+	const c10::cuda::CUDAGuard guard(n.device());
+	torch::Tensor loss = new_empty({1}, n.options().dtype(torch::kFloat64));
+	torch::Tensor dn = new_empty({3, row_hi - row_lo, W}, n.options()), de = new_empty({C, row_hi - row_lo, W}, n.options()),
+	              dm = new_empty({C, row_hi - row_lo, W}, n.options());
+	check(rgs_normal_consistency_rows((int)H, (int)W, (int)row_lo, (int)row_hi, from_depth ? 1 : 0, (float)inv_fx, (float)inv_fy, (float)cx, (float)cy,
+	                                  n.data_ptr<float>(), e.data_ptr<float>(), m.data_ptr<float>(), (float)w_expected, (float)w_median,
+	                                  loss.data_ptr<double>(), dn.data_ptr<float>(), de.data_ptr<float>(), dm.data_ptr<float>(),
+	                                  at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(loss, dn, de, dm);
+}
+
 // ---- decoupled-appearance L1 loss (train.py:37-58; rgs_appearance_*) -------------------------------------------------------
 
 // image [3,H0,W0] -> the center crop's bilinear downsample [3, H/32, W/32]
@@ -1680,6 +1707,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	       py::arg("H"), py::arg("W"), py::arg("znear"), py::arg("zfar"));
 	tc.def("visibility_count", &TntVisibilityCount, py::arg("points"), py::arg("depth"), py::arg("w2c"), py::arg("fx"), py::arg("fy"), py::arg("cx"),
 	       py::arg("cy"), py::arg("eps"), py::arg("counts"));
+	// slab-local forms of the training losses: a private submodule behind rade_gs_b200.multigpu
+	py::module_ sl = m.def_submodule("_slab", "row-sharded training-loss stages behind rade_gs_b200.multigpu");
+	sl.def("normal_consistency_rows", &NormalConsistencyRows, py::arg("rendered_normal"), py::arg("map_expected"), py::arg("map_median"),
+	       py::arg("from_depth"), py::arg("inv_fx"), py::arg("inv_fy"), py::arg("cx"), py::arg("cy"), py::arg("w_expected"), py::arg("w_median"), py::arg("H"),
+	       py::arg("row_lo"), py::arg("row_hi"));
 	m.def("grad_stride",[](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });

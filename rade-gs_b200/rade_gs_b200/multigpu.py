@@ -14,6 +14,7 @@ add up to the single-GPU answer.
 """
 from __future__ import annotations
 
+import math
 import os
 from typing import Callable, List, Sequence, Tuple
 
@@ -477,3 +478,151 @@ def slab_l1_ssim_loss(image: torch.Tensor, gt: torch.Tensor, lambda_dssim: float
         raise ValueError("slab-local SSIM needs slabs of at least 5 pixel rows on every rank (a shorter slab breaks the neighbour halo exchange)")
     fwd, bwd = kernels if kernels is not None else (_cuda_slab_fwd, _cuda_slab_bwd)
     return _SlabSsimL1.apply(image, gt, float(lambda_dssim), (int(pixel_rows[0]), int(pixel_rows[1])), rank, world_size, group, fwd, bwd)
+
+
+# ---- slab-local normal consistency (train.py:141-156) ------------------------------------------------------------------------
+NORMAL_HALO = 2   # a stencil reads its +-1 row neighbours, and a pixel's gradient comes from the stencils +-1 row away
+
+
+class _SlabNormalConsistency(torch.autograd.Function):
+    """train.py:141-156's `(1 - r) * mean(error[0]) + r * mean(error[1])` of the WHOLE image, evaluated slab by slab.  A rank counts
+    the error rows of its own slab.  Its kernel also evaluates the stencils one row beyond the slab, whose loss the neighbours count,
+    because they read the slab's pixels: every gradient is then complete on the rank that owns the pixel, and backward exchanges
+    nothing.  Forward receives 2 rows of both maps and of the normal from each neighbour (one exchange) and all-reduces one fp64
+    scalar.  `kernel(normal_win, e_win, m_win, from_depth, inv_fx, inv_fy, cx, cy, w_e, w_m, H, r0, r1)` -> (loss_sum [1] float64,
+    d_normal, d_e, d_m on rows [r0, r1)) takes the windows of include/rgs_b200.h's `rgs_normal_consistency_rows`."""
+
+    @staticmethod
+    def forward(ctx, normal, map_e, map_m, from_depth, cam, depth_ratio, H, rows, rank, world, group, kernel):
+        r0, r1 = rows
+        W = normal.shape[-1]
+        C = map_e.shape[0]
+        compact = normal.shape[-2] != H   # else full-size (the two coincide when one slab is the whole image)
+        own = (lambda t: t.detach()) if compact else (lambda t: t.detach()[:, r0:r1])
+        m_lo, m_hi = max(0, r0 - NORMAL_HALO), min(H, r1 + NORMAL_HALO)
+        n_lo, n_hi = max(0, r0 - 1), min(H, r1 + 1)
+        w_e, w_m = (1.0 - depth_ratio) / (H * W), depth_ratio / (H * W)
+        if r1 > r0:
+            # both maps and the normal in one row window, so that one exchange carries all their halo rows
+            win = normal.new_zeros(2 * C + 3, m_hi - m_lo, W)
+            a, b = r0 - m_lo, r1 - m_lo
+            win[:C, a:b], win[C:2 * C, a:b], win[2 * C:, a:b] = own(map_e), own(map_m), own(normal)
+            k = min(NORMAL_HALO, r1 - r0)
+            # a slab that ends at the image's last row has no neighbour below (later ranks' slabs are empty there)
+            _exchange_rows(win, (a, a + k), (b - k, b) if r1 < H else (b, b), (0, a), (b, m_hi - m_lo), rank, world, group, add=False)
+            loss, dn, de, dm = kernel(win[2 * C:, n_lo - m_lo:n_hi - m_lo].contiguous(), win[:C].contiguous(), win[C:2 * C].contiguous(), from_depth,
+                                      *cam, w_e, w_m, H, r0, r1)
+            loss = loss.clone()
+        else:
+            loss = torch.zeros(1, dtype=torch.float64, device=normal.device)
+            dn, de, dm = (normal.new_zeros(c, 0, W) for c in (3, C, C))
+        if world > 1:
+            dist.all_reduce(loss, group=group)
+        ctx.save_for_backward(dn, de, dm)
+        ctx.meta = (compact, H, r0, r1)
+        return loss[0].float()
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        compact, H, r0, r1 = ctx.meta
+
+        def place(d):
+            if compact:
+                return d * grad_out
+            out = d.new_zeros(d.shape[0], H, d.shape[2])
+            out[:, r0:r1] = d * grad_out
+            return out
+
+        return (*(place(d) for d in ctx.saved_tensors), None, None, None, None, None, None, None, None, None)
+
+
+def _cuda_normal_rows(normal_win, e_win, m_win, from_depth, inv_fx, inv_fy, cx, cy, w_e, w_m, H, r0, r1):
+    from diff_gaussian_rasterization import _C
+    return _C._slab.normal_consistency_rows(normal_win, e_win, m_win, from_depth, inv_fx, inv_fy, cx, cy, w_e, w_m, H, r0, r1)
+
+
+def _check_slab_rows(pixel_rows, all_pixel_rows, H, rank, world_size):
+    """Raise unless the slab rows suit the 2-row halo exchange.  With `all_pixel_rows` (every rank's rows, e.g.
+    `[(min(b * 16, H), min(e * 16, H)) for b, e in rast.slabs]`) every rank checks the whole partition and all raise the same error
+    before any collective.  Without it a rank sees only its own rows: a rank whose slab is too short raises, and its neighbours
+    then wait in the halo exchange for rows that never come."""
+    r0, r1 = int(pixel_rows[0]), int(pixel_rows[1])
+    if not 0 <= r0 <= r1 <= H:
+        raise ValueError(f"pixel rows [{r0}, {r1}) are not rows of a {H}-row image")
+    rows = [(r0, r1)]
+    if all_pixel_rows is not None:
+        rows = [(int(b), int(e)) for b, e in all_pixel_rows]
+        if len(rows) != world_size or rows[rank] != (r0, r1):
+            raise ValueError(f"all_pixel_rows must hold one row range per rank ({world_size}) with this rank's pixel_rows at index {rank}")
+        if rows[0][0] != 0 or rows[-1][1] != H or any(rows[i][1] != rows[i + 1][0] or rows[i][0] > rows[i][1] for i in range(len(rows) - 1)):
+            raise ValueError(f"all_pixel_rows must tile the image's {H} rows in rank order, got {rows}")
+    if world_size > 1:
+        short = [(b, e) for b, e in rows if e - b < NORMAL_HALO and e < H]
+        if short:
+            raise ValueError("slab-local normal consistency needs every slab that does not end at the image's last row to hold at least 2 pixel "
+                             f"rows (a shorter slab breaks the neighbour halo exchange); slabs {short} do not")
+    return r0, r1
+
+
+def _slab_normal_loss(normal, map_e, map_m, from_depth, cam, depth_ratio, H, pixel_rows, all_pixel_rows, rank, world_size, group, kernels,
+                      map_channels):
+    if world_size is None:
+        world_size = dist.get_world_size(group) if dist.is_initialized() else 1
+    if rank is None:
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+    r0, r1 = _check_slab_rows(pixel_rows, all_pixel_rows, H, rank, world_size)
+    if kernels is None and not (normal.is_cuda and map_e.is_cuda and map_m.is_cuda):
+        raise RuntimeError("slab-local normal consistency needs CUDA tensors: there is no CPU path")
+    W = normal.shape[-1]
+    for name, t, c in (("normal", normal, 3), ("expected map", map_e, map_channels), ("median map", map_m, map_channels)):
+        if t.dim() != 3 or t.shape[0] != c or t.shape[-1] != W or t.shape[-2] not in (H, r1 - r0):
+            raise ValueError(f"{name} must be [{c}, {H} or {r1 - r0} rows, {W}] (full-size or the slab's rows), got {tuple(t.shape)}")
+    if len({normal.shape[-2], map_e.shape[-2], map_m.shape[-2]}) != 1:
+        raise ValueError("the normal and both maps must all be full-size or all hold the slab's rows")
+    kernel = kernels if kernels is not None else _cuda_normal_rows
+    return _SlabNormalConsistency.apply(normal, map_e, map_m, from_depth, cam, float(depth_ratio), H, (r0, r1), rank, world_size, group, kernel)
+
+
+def _image_height(t, pixel_rows, image_height, world_size, group):
+    """The image's row count: `image_height`, else that of full-size maps.  Maps with the slab's row count are taken for compact
+    ones when there are several ranks, and then the height cannot be read from them."""
+    if image_height is not None:
+        return int(image_height)
+    if world_size is None:
+        world_size = dist.get_world_size(group) if dist.is_initialized() else 1
+    if world_size > 1 and t.shape[-2] == pixel_rows[1] - pixel_rows[0]:
+        raise ValueError("maps that hold only the slab's rows need image_height")
+    return int(t.shape[-2])
+
+
+def slab_depth_normal_consistency_loss(view, normal: torch.Tensor, expected_depth: torch.Tensor, median_depth: torch.Tensor,
+                                       pixel_rows: Tuple[int, int], depth_ratio: float = 0.6, image_height: int | None = None,
+                                       all_pixel_rows=None, rank: int | None = None, world_size: int | None = None, group=None,
+                                       kernels=None) -> torch.Tensor:
+    """`losses.depth_normal_consistency_loss` (train.py:141-156 with require_depth) for a row-sharded render.  The maps are
+    `ShardedGaussianRasterizer`'s: compact ([3 or 1, slab rows, W]) or full-size with this rank's slab rows `pixel_rows` filled.
+    `view` needs FoVx and FoVy; the image height is `image_height`, else `view.image_height`, else the maps' when they are
+    full-size.  Returns the whole image's loss, the same value on every rank; its gradient lands in this rank's rows only and is
+    complete there.  Every slab that does not end at the image's last row must hold at least 2 rows.  Pass `all_pixel_rows`, every
+    rank's row range, so that every rank refuses a partition that breaks this rule; without it only the rank with the short slab
+    raises and its neighbours block in the halo exchange."""
+    if image_height is None:
+        image_height = getattr(view, "image_height", None)
+    H = _image_height(normal, pixel_rows, image_height, world_size, group)
+    W = normal.shape[-1]
+    fx = W / (2 * math.tan(view.FoVx / 2.))
+    fy = H / (2 * math.tan(view.FoVy / 2.))
+    # entries of intrins_inv (utils/graphics_utils.py:101-105), as losses.depth_normal_consistency_loss passes them
+    cam = (1 / fx, 1 / fy, -W / (2 * fx), -H / (2 * fy))
+    return _slab_normal_loss(normal, expected_depth, median_depth, True, cam, depth_ratio, H, pixel_rows, all_pixel_rows, rank, world_size, group,
+                             kernels, 1)
+
+
+def slab_point_normal_consistency_loss(normal: torch.Tensor, expected_coord: torch.Tensor, median_coord: torch.Tensor, pixel_rows: Tuple[int, int],
+                                       depth_ratio: float = 0.6, image_height: int | None = None, all_pixel_rows=None, rank: int | None = None,
+                                       world_size: int | None = None, group=None, kernels=None) -> torch.Tensor:
+    """`losses.point_normal_consistency_loss` (train.py:141-156 with require_coord) for a row-sharded render; the maps as in
+    `slab_depth_normal_consistency_loss`, and so is `all_pixel_rows`.  Compact maps need `image_height`."""
+    H = _image_height(normal, pixel_rows, image_height, world_size, group)
+    return _slab_normal_loss(normal, expected_coord, median_coord, False, (0.0, 0.0, 0.0, 0.0), depth_ratio, H, pixel_rows, all_pixel_rows, rank,
+                             world_size, group, kernels, 3)
