@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define RGS_ABI_VERSION 3
+#define RGS_ABI_VERSION 4
 
 typedef enum rgs_status {
 	RGS_OK = 0,
@@ -202,13 +202,6 @@ typedef struct rgs_exchange rgs_exchange;
 int32_t rgs_exchange_create(int32_t rank, int32_t world, int64_t capacity_rows, int32_t row_floats, rgs_exchange** out,
                             void* ipc_handle /* host, RGS_IPC_HANDLE_BYTES */);
 int32_t rgs_exchange_connect(rgs_exchange* ex, const void* all_handles /* host, world * RGS_IPC_HANDLE_BYTES, rank-major */);
-/* Alternative to create + connect: the caller provides the windows (e.g. torch symmetric memory: cuMem VMM allocations mapped on every
- * rank, plus an NVLS multicast mapping).  window_ptrs[p] = this process's mapping of rank p's window, each rgs_exchange_window_bytes
- * long and zero-filled; multicast_ptr = multicast mapping of all windows or 0.  With a multicast mapping the spread phase issues ONE
- * store per 16 bytes and the NVSwitch replicates it (outbound traffic / world). */
-size_t rgs_exchange_window_bytes(int32_t world, int64_t capacity_rows, int32_t row_floats);
-int32_t rgs_exchange_attach(int32_t rank, int32_t world, int64_t capacity_rows, int32_t row_floats, const uint64_t* window_ptrs,
-                            uint64_t multicast_ptr, rgs_exchange** out);
 int32_t rgs_exchange_destroy(rgs_exchange* ex);
 float* rgs_exchange_accumulator(rgs_exchange* ex);     /* persistent local accumulator (all-zero between steps) */
 const float* rgs_exchange_result(rgs_exchange* ex);    /* summed rows, valid after rgs_backward_render_exchange on the same stream */
@@ -220,7 +213,6 @@ int32_t rgs_backward_render_exchange(const rgs_camera* cam, const rgs_gaussians*
 /* Synchronises the stream and returns 0 when every barrier so far completed, 1 + p when one gave up (after ~10 s) waiting for
  * rank p -- the rows of that step are then meaningless; callers fall back to a host-driven collective. */
 int32_t rgs_exchange_status(rgs_exchange* ex, void* cuda_stream);
-const char* rgs_exchange_last_error(void);
 
 /* Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:18-23, rasterizer_impl.cu:176-188). */
 int32_t rgs_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,

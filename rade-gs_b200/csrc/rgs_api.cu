@@ -396,7 +396,7 @@ int32_t rgs_backward_render_exchange(const rgs_camera* cam, const rgs_gaussians*
 		StageScope sc(ST_EXCHANGE, s);
 		rc = rgs_exchange_rows(ex, p.P, g.tiles_touched, in->radii, cuda_stream);
 	}
-	if (rc != RGS_OK) return fail(rc, rgs_exchange_last_error());
+	if (rc != RGS_OK) return rc;
 	return debug_sync(cam, s, "gradient exchange");
 }
 

@@ -38,7 +38,6 @@ struct PeerTable {
 	float* full[MAX_WORLD];
 	uint32_t* flags[MAX_WORLD];
 	uint8_t* mark[MAX_WORLD];  // [rows_per_rank_cap] per owned row: some rank pushed into it this step
-	float* full_multicast;  // NVLS multicast mapping of every rank's `full` (one store reaches all ranks), or nullptr
 };
 
 }  // namespace rgs
@@ -52,7 +51,6 @@ struct rgs_exchange {
 	size_t bytes, off_full, off_flags, off_mark;
 	char* peer_base[rgs::MAX_WORLD];
 	bool connected;
-	bool external;              // windows provided by the caller (rgs_exchange_attach): not opened / freed here
 	rgs::PeerTable tab;
 	float* acc_local;           // persistent local accumulator [capacity][row], kept all-zero between steps
 	uint8_t* dirty;             // [rows_per_rank_cap] owner-side: row was non-zero in `full` after the previous step
@@ -124,7 +122,7 @@ __global__ void exchange_barrier_kernel(int rank, int world, uint32_t epoch, Pee
 
 // The owner's pass: one thread per owned row reads its mark (set by the pushers) and its dirty flag (row was non-zero in `full`
 // after the previous step); the rows found by a warp are copied, RQ lanes at a time, from `sum` to the `full` array of EVERY rank
-// (one multicast store, or world plain stores) and `sum` is cleared.  Rows that carried something last step and nothing now are
+// (world plain stores) and `sum` is cleared.  Rows that carried something last step and nothing now are
 // rewritten with zeros once.
 template <int RQ>
 __global__ void __launch_bounds__(256) exchange_spread_kernel(int P, int rows_per_rank, int rank, int world, float4* __restrict__ my_sum,
@@ -144,14 +142,7 @@ __global__ void __launch_bounds__(256) exchange_spread_kernel(int P, int rows_pe
 			const float4 v = *src;
 			nz = !(v.x == 0.f && v.y == 0.f && v.z == 0.f && v.w == 0.f);
 			if (nz) *src = make_float4(0.f, 0.f, 0.f, 0.f);
-			if (tab.full_multicast != nullptr) {
-				// one 16-byte store on the multicast mapping: the NVSwitch replicates it into every rank's window (this rank's included)
-				asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(tab.full_multicast + (idx * RQ + lane) * 4), "f"(v.x),
-				             "f"(v.y), "f"(v.z), "f"(v.w)
-				             : "memory");
-			} else {
-				for (int p = 0; p < world; p++) reinterpret_cast<float4*>(tab.full[p])[idx * RQ + lane] = v;
-			}
+			for (int p = 0; p < world; p++) reinterpret_cast<float4*>(tab.full[p])[idx * RQ + lane] = v;
 		}
 		const unsigned row_nz = __ballot_sync(0xffffffffu, nz);
 		if (lane == 0) {
@@ -161,19 +152,9 @@ __global__ void __launch_bounds__(256) exchange_spread_kernel(int P, int rows_pe
 	}
 }
 
-static thread_local std::string x_error;
-static int xfail(int code, const std::string& msg) { x_error = msg; return code; }
-const char* exchange_last_error() { return x_error.c_str(); }
-
 }  // namespace rgs
 
 using namespace rgs;
-
-#define RGS_X_TRY(expr)                                                                                      \
-	do {                                                                                                     \
-		cudaError_t _e = (expr);                                                                             \
-		if (_e != cudaSuccess) return xfail(RGS_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
-	} while (0)
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static void layout(rgs_exchange* ex) {
@@ -185,82 +166,47 @@ static void layout(rgs_exchange* ex) {
 	ex->bytes = ex->off_mark + align_up((size_t)ex->rows_per_rank_cap, 256);
 }
 
+// The window, the local accumulator and the dirty flags, zeroed, and the window's IPC handle into `ipc_handle`.
+static int allocate(rgs_exchange* ex, void* ipc_handle) {
+	RGS_CUDA_TRY(cudaGetDevice(&ex->device));
+	layout(ex);
+	const size_t row = (size_t)ex->row_floats * sizeof(float);
+	RGS_CUDA_TRY(cudaMalloc((void**)&ex->base, ex->bytes));
+	RGS_CUDA_TRY(cudaMemset(ex->base, 0, ex->bytes));
+	RGS_CUDA_TRY(cudaMalloc((void**)&ex->acc_local, (size_t)ex->capacity * row));
+	RGS_CUDA_TRY(cudaMemset(ex->acc_local, 0, (size_t)ex->capacity * row));
+	RGS_CUDA_TRY(cudaMalloc((void**)&ex->dirty, (size_t)ex->rows_per_rank_cap));
+	RGS_CUDA_TRY(cudaMemset(ex->dirty, 0, (size_t)ex->rows_per_rank_cap));
+	RGS_CUDA_TRY(cudaDeviceSynchronize());
+	cudaIpcMemHandle_t h;
+	static_assert(sizeof(h) == RGS_IPC_HANDLE_BYTES, "IPC handle size");
+	RGS_CUDA_TRY(cudaIpcGetMemHandle(&h, ex->base));
+	memcpy(ipc_handle, &h, sizeof(h));
+	return RGS_OK;
+}
 
 extern "C" {
 
 int32_t rgs_exchange_create(int32_t rank, int32_t world, int64_t capacity_rows, int32_t row_floats, rgs_exchange** out, void* ipc_handle) {
-	if (!out || !ipc_handle) return xfail(RGS_E_INVALID, "null pointer");
-	if (world < 1 || world > MAX_WORLD || rank < 0 || rank >= world) return xfail(RGS_E_INVALID, "rank / world out of range (world <= 16)");
-	if (capacity_rows <= 0 || (row_floats != GRAD_FLOATS_BASE && row_floats != GRAD_FLOATS_COORD)) return xfail(RGS_E_INVALID, "capacity / row size");
+	if (!out || !ipc_handle) return fail(RGS_E_INVALID, "null pointer");
+	if (world < 1 || world > MAX_WORLD || rank < 0 || rank >= world) return fail(RGS_E_INVALID, "rank / world out of range (world <= 16)");
+	if (capacity_rows <= 0 || (row_floats != GRAD_FLOATS_BASE && row_floats != GRAD_FLOATS_COORD)) return fail(RGS_E_INVALID, "capacity / row size");
 	rgs_exchange* ex = new rgs_exchange();
 	memset(ex, 0, sizeof(*ex));
 	ex->rank = rank; ex->world = world; ex->capacity = capacity_rows; ex->row_floats = row_floats;
-	RGS_X_TRY(cudaGetDevice(&ex->device));
-	layout(ex);
-	const size_t row = (size_t)row_floats * sizeof(float);
-	RGS_X_TRY(cudaMalloc((void**)&ex->base, ex->bytes));
-	RGS_X_TRY(cudaMemset(ex->base, 0, ex->bytes));
-	RGS_X_TRY(cudaMalloc((void**)&ex->acc_local, (size_t)capacity_rows * row));
-	RGS_X_TRY(cudaMemset(ex->acc_local, 0, (size_t)capacity_rows * row));
-	RGS_X_TRY(cudaMalloc((void**)&ex->dirty, (size_t)ex->rows_per_rank_cap));
-	RGS_X_TRY(cudaMemset(ex->dirty, 0, (size_t)ex->rows_per_rank_cap));
-	RGS_X_TRY(cudaDeviceSynchronize());
-	cudaIpcMemHandle_t h;
-	static_assert(sizeof(h) == RGS_IPC_HANDLE_BYTES, "IPC handle size");
-	RGS_X_TRY(cudaIpcGetMemHandle(&h, ex->base));
-	memcpy(ipc_handle, &h, sizeof(h));
 	ex->last_P = -1;
-	*out = ex;
-	return RGS_OK;
-}
-
-size_t rgs_exchange_window_bytes(int32_t world, int64_t capacity_rows, int32_t row_floats) {
-	rgs_exchange tmp;
-	memset(&tmp, 0, sizeof(tmp));
-	tmp.world = world > 0 ? world : 1; tmp.capacity = capacity_rows; tmp.row_floats = row_floats;
-	layout(&tmp);
-	return tmp.bytes;
-}
-
-// Windows provided by the caller: window_ptrs[p] = this process's mapping of rank p's window (each rgs_exchange_window_bytes long,
-// ZERO-FILLED by the caller before any rank attaches), multicast_ptr = a multicast mapping of all of them or 0.  The product gets
-// both from torch's symmetric memory (cuMem VMM + NVLS multicast objects); the library only runs its kernels on the pointers.
-int32_t rgs_exchange_attach(int32_t rank, int32_t world, int64_t capacity_rows, int32_t row_floats, const uint64_t* window_ptrs,
-                            uint64_t multicast_ptr, rgs_exchange** out) {
-	if (!out || !window_ptrs) return xfail(RGS_E_INVALID, "null pointer");
-	if (world < 1 || world > MAX_WORLD || rank < 0 || rank >= world) return xfail(RGS_E_INVALID, "rank / world out of range (world <= 16)");
-	if (capacity_rows <= 0 || (row_floats != GRAD_FLOATS_BASE && row_floats != GRAD_FLOATS_COORD)) return xfail(RGS_E_INVALID, "capacity / row size");
-	rgs_exchange* ex = new rgs_exchange();
-	memset(ex, 0, sizeof(*ex));
-	ex->rank = rank; ex->world = world; ex->capacity = capacity_rows; ex->row_floats = row_floats;
-	RGS_X_TRY(cudaGetDevice(&ex->device));
-	layout(ex);
-	const size_t row = (size_t)row_floats * sizeof(float);
-	RGS_X_TRY(cudaMalloc((void**)&ex->acc_local, (size_t)capacity_rows * row));
-	RGS_X_TRY(cudaMemset(ex->acc_local, 0, (size_t)capacity_rows * row));
-	RGS_X_TRY(cudaMalloc((void**)&ex->dirty, (size_t)ex->rows_per_rank_cap));
-	RGS_X_TRY(cudaMemset(ex->dirty, 0, (size_t)ex->rows_per_rank_cap));
-	for (int p = 0; p < world; p++) {
-		ex->peer_base[p] = reinterpret_cast<char*>(window_ptrs[p]);
-		if (!ex->peer_base[p]) return xfail(RGS_E_INVALID, "null window pointer");
-		ex->tab.sum[p] = reinterpret_cast<float*>(ex->peer_base[p]);
-		ex->tab.full[p] = reinterpret_cast<float*>(ex->peer_base[p] + ex->off_full);
-		ex->tab.flags[p] = reinterpret_cast<uint32_t*>(ex->peer_base[p] + ex->off_flags);
-		ex->tab.mark[p] = reinterpret_cast<uint8_t*>(ex->peer_base[p] + ex->off_mark);
+	const int rc = allocate(ex, ipc_handle);
+	if (rc != RGS_OK) {
+		rgs_exchange_destroy(ex);   // frees what was allocated before the failing call
+		return rc;
 	}
-	ex->base = ex->peer_base[rank];
-	ex->tab.full_multicast = multicast_ptr ? reinterpret_cast<float*>(reinterpret_cast<char*>(multicast_ptr) + ex->off_full) : nullptr;
-	ex->external = true;
-	ex->connected = true;
-	ex->last_P = -1;
-	RGS_X_TRY(cudaDeviceSynchronize());
 	*out = ex;
 	return RGS_OK;
 }
 
 int32_t rgs_exchange_connect(rgs_exchange* ex, const void* all_handles) {
-	if (!ex || !all_handles) return xfail(RGS_E_INVALID, "null pointer");
-	if (ex->connected) return xfail(RGS_E_INVALID, "already connected");
+	if (!ex || !all_handles) return fail(RGS_E_INVALID, "null pointer");
+	if (ex->connected) return fail(RGS_E_INVALID, "already connected");
 	for (int p = 0; p < ex->world; p++) {
 		if (p == ex->rank) {
 			ex->peer_base[p] = ex->base;
@@ -268,7 +214,7 @@ int32_t rgs_exchange_connect(rgs_exchange* ex, const void* all_handles) {
 			cudaIpcMemHandle_t h;
 			memcpy(&h, (const char*)all_handles + (size_t)p * RGS_IPC_HANDLE_BYTES, sizeof(h));
 			void* ptr = nullptr;
-			RGS_X_TRY(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
+			RGS_CUDA_TRY(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
 			ex->peer_base[p] = (char*)ptr;
 		}
 		ex->tab.sum[p] = reinterpret_cast<float*>(ex->peer_base[p]);
@@ -283,10 +229,9 @@ int32_t rgs_exchange_connect(rgs_exchange* ex, const void* all_handles) {
 int32_t rgs_exchange_destroy(rgs_exchange* ex) {
 	if (!ex) return RGS_OK;
 	cudaDeviceSynchronize();
-	if (ex->connected && !ex->external)
-		for (int p = 0; p < ex->world; p++)
-			if (p != ex->rank && ex->peer_base[p]) cudaIpcCloseMemHandle(ex->peer_base[p]);
-	if (!ex->external) cudaFree(ex->base);
+	for (int p = 0; p < ex->world; p++)   // also the windows a failed rgs_exchange_connect opened before its failure
+		if (p != ex->rank && ex->peer_base[p]) cudaIpcCloseMemHandle(ex->peer_base[p]);
+	cudaFree(ex->base);
 	cudaFree(ex->acc_local);
 	cudaFree(ex->dirty);
 	delete ex;
@@ -307,21 +252,21 @@ static int* timeout_flag() {
 }
 
 int32_t rgs_exchange_rows(rgs_exchange* ex, int32_t P, const uint32_t* tiles_touched, const int32_t* radii, void* cuda_stream) {
-	if (!ex || !ex->connected) return xfail(RGS_E_INVALID, "exchange not connected");
-	if (P < 0 || P > ex->capacity) return xfail(RGS_E_INVALID, "more Gaussians than the exchange was created for: re-create it (collectively) with a larger capacity");
+	if (!ex || !ex->connected) return fail(RGS_E_INVALID, "exchange not connected");
+	if (P < 0 || P > ex->capacity) return fail(RGS_E_INVALID, "more Gaussians than the exchange was created for: re-create it (collectively) with a larger capacity");
 	if (P == 0) return RGS_OK;
-	if (!tiles_touched || !radii) return xfail(RGS_E_INVALID, "null pointer");
+	if (!tiles_touched || !radii) return fail(RGS_E_INVALID, "null pointer");
 	cudaStream_t s = (cudaStream_t)cuda_stream;
 	int* tf = timeout_flag();
-	if (!tf) return xfail(RGS_E_CUDA, "cudaHostAlloc failed");
-	if (*tf) return xfail(RGS_E_CUDA, "a previous exchange barrier timed out waiting for rank " + std::to_string(*tf - 1));
+	if (!tf) return fail(RGS_E_CUDA, "cudaHostAlloc failed");
+	if (*tf) return fail(RGS_E_CUDA, "a previous exchange barrier timed out waiting for rank " + std::to_string(*tf - 1));
 	const int rq = ex->row_floats / 4;
 	const int rows_per_rank = (P + ex->world - 1) / ex->world;
 	if (P != ex->last_P) {
 		// the row <-> Gaussian association changed (densification, first call): forget what `full` held.  Every rank sees the
 		// same sequence of P, so all do this in the same step; peers write into `full` only after the next barrier.
-		RGS_X_TRY(cudaMemsetAsync(ex->base + ex->off_full, 0, (size_t)ex->capacity * ex->row_floats * sizeof(float), s));
-		RGS_X_TRY(cudaMemsetAsync(ex->dirty, 0, (size_t)ex->rows_per_rank_cap, s));
+		RGS_CUDA_TRY(cudaMemsetAsync(ex->base + ex->off_full, 0, (size_t)ex->capacity * ex->row_floats * sizeof(float), s));
+		RGS_CUDA_TRY(cudaMemsetAsync(ex->dirty, 0, (size_t)ex->rows_per_rank_cap, s));
 		ex->last_P = P;   // (marks and `sum` are always left clear by the spread pass)
 	}
 	{
@@ -340,19 +285,17 @@ int32_t rgs_exchange_rows(rgs_exchange* ex, int32_t P, const uint32_t* tiles_tou
 	exchange_barrier_kernel<<<1, 32, 0, s>>>(ex->rank, ex->world, ++ex->epoch, ex->tab, tf);
 	count_launch(4);
 	cudaError_t e = cudaGetLastError();
-	if (e != cudaSuccess) return xfail(RGS_E_CUDA, cudaGetErrorString(e));
+	if (e != cudaSuccess) return fail(RGS_E_CUDA, cudaGetErrorString(e));
 	return RGS_OK;
 }
 
 // 0 = healthy; 1 + p = a barrier gave up waiting for rank p (after synchronising the stream the exchange ran on).
 int32_t rgs_exchange_status(rgs_exchange* ex, void* cuda_stream) {
-	if (!ex) return xfail(RGS_E_INVALID, "null exchange");
+	if (!ex) return fail(RGS_E_INVALID, "null exchange");
 	cudaError_t e = cudaStreamSynchronize((cudaStream_t)cuda_stream);
-	if (e != cudaSuccess) return xfail(RGS_E_CUDA, cudaGetErrorString(e));
+	if (e != cudaSuccess) return fail(RGS_E_CUDA, cudaGetErrorString(e));
 	int* tf = timeout_flag();
 	return tf ? *tf : 0;
 }
-
-const char* rgs_exchange_last_error(void) { return exchange_last_error(); }
 
 }  // extern "C"

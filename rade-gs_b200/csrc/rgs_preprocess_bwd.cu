@@ -9,8 +9,7 @@
 // Faithfulness notes (SURVEY.md appendix A):
 //   * the hand-derived, epsilon-regularised gradient of the mip coefficient is restated as is, INCLUDING the
 //     reference's aliasing bug: BACKWARD::preprocess receives dL_dconic where conic_opacity is expected
-//     (rasterizer_impl.cu:569 vs backward.h:94), so `combined_opacity` below is dL_dconic.w.  Set
-//     RGS_FIX_MIP_GRADIENT to use the true opacity*coef instead (off by default: parity first);
+//     (rasterizer_impl.cu:569 vs backward.h:94), so `combined_opacity` below is dL_dconic.w;
 //   * gradients are w.r.t. the quaternion as given (no normalisation inside, backward.cu:554);
 //   * Sigma's eigen-decomposition follows the reference's solver and stopping rules (see rgs_geom.cuh).
 #include "rgs_geom.cuh"
@@ -19,7 +18,7 @@ namespace rgs {
 
 // One Gaussian's parameter gradients from its accumulator row.  Writes every output of the row (zeros when not rendered / nothing received).
 __device__ __forceinline__ void preprocess_backward_row(const FwdParams& p, const GeomView& g, const int* __restrict__ radii,
-                                                        const float* __restrict__ grad_accum, const ParamGradOut& out, int fix_mip, const int idx) {
+                                                        const float* __restrict__ grad_accum, const ParamGradOut& out, const int idx) {
 	bool visible = radii[idx] > 0;
 
 	float o_means2D[3] = {0, 0, 0}, o_colors[3] = {0, 0, 0}, o_opacity = 0.f, o_mean3D[3] = {0, 0, 0};
@@ -225,8 +224,7 @@ __device__ __forceinline__ void preprocess_backward_row(const FwdParams& p, cons
 		}
 
 		// ---- mip-coefficient and conic backward (backward.cu:367-431) ----
-		// fixed mode reads the true opacity*coef that forward stored in the render record (slot 5)
-		const float combined_opacity = fix_mip ? g.records[(size_t)idx * rec_floats(p.coord) + 5] : dL_dconic.z;
+		const float combined_opacity = dL_dconic.z;
 		const float opacity = combined_opacity / (coef + 1e-6);
 		const float dL_dcoef = dL_dopacity * opacity;
 		const float dL_dsqrtcoef = dL_dcoef * 0.5 * 1. / (coef + 1e-6);
@@ -368,11 +366,11 @@ __device__ __forceinline__ void preprocess_backward_row(const FwdParams& p, cons
 // zero-filled by the launcher.  In a dense scene most rendered splats are occluded in any one view (C2: 84 %, C3: 92 % of the
 // visible ones receive nothing), and a warp of a thread-per-Gaussian kernel would run the whole chain if ANY of its 32 rows needed it.
 __global__ void __launch_bounds__(128, 4) preprocess_backward_rows_kernel(FwdParams p, GeomView g, const int* __restrict__ radii,
-                                                                        const float* __restrict__ grad_accum, ParamGradOut out, int fix_mip,
+                                                                        const float* __restrict__ grad_accum, ParamGradOut out,
                                                                         const uint32_t* __restrict__ list, const uint32_t* __restrict__ count) {
 	const int n = (int)*count;
 	for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < n; l += gridDim.x * blockDim.x)
-		preprocess_backward_row(p, g, radii, grad_accum, out, fix_mip, (int)list[l]);
+		preprocess_backward_row(p, g, radii, grad_accum, out, (int)list[l]);
 }
 
 // rows that need work: rendered and any non-zero (or NaN) entry in the accumulator row.  A warp owns 32 consecutive rows and reads them
@@ -569,7 +567,6 @@ void launch_backward_zero_fill(const FwdParams& p, ParamGradOut out, cudaStream_
 
 void launch_preprocess_backward(const FwdParams& p, GeomView g, const int* radii, const float* grad_accum, ParamGradOut out, cudaStream_t s,
                                 bool prefilled) {
-	static const int fix_mip = getenv("RGS_FIX_MIP_GRADIENT") != nullptr && atoi(getenv("RGS_FIX_MIP_GRADIENT")) != 0;
 	const bool has_sh = p.shs != nullptr && out.d_sh != nullptr && p.M > 0;
 	const int stride = (3 * p.M) | 1;
 	const size_t smem = (size_t)SH_WARPS * 32 * stride * sizeof(float);
@@ -587,7 +584,7 @@ void launch_preprocess_backward(const FwdParams& p, GeomView g, const int* radii
 	// the list length stays on the device (no host sync): grids sized for "every row listed", CTAs beyond the list leave at once
 	const int sms = sm_count();
 	const int rows_grid = min((p.P + 127) / 128, sms * 16);
-	preprocess_backward_rows_kernel<<<rows_grid, 128, 0, s>>>(p, g, radii, grad_accum, out, fix_mip, list, count);
+	preprocess_backward_rows_kernel<<<rows_grid, 128, 0, s>>>(p, g, radii, grad_accum, out, list, count);
 	count_launch(2 + 8 + (has_sh ? 1 : 0));
 	if (has_sh) {
 		if (smem > 48 * 1024) ensure_dynamic_smem(sh_backward_rows_kernel, smem, configured_rows);

@@ -489,30 +489,15 @@ std::tuple<int64_t, torch::Tensor> ExchangeCreate(const int rank, const int worl
 	const c10::cuda::CUDAGuard guard(c10::Device(c10::kCUDA, device));
 	rgs_exchange* ex = nullptr;
 	torch::Tensor handle = torch::zeros({RGS_IPC_HANDLE_BYTES}, torch::kUInt8);
-	if (rgs_exchange_create(rank, world, capacity_rows, row_floats, &ex, handle.data_ptr()) != RGS_OK) throw std::runtime_error(rgs_exchange_last_error());
+	check(rgs_exchange_create(rank, world, capacity_rows, row_floats, &ex, handle.data_ptr()));
 	return std::make_tuple((int64_t)reinterpret_cast<intptr_t>(ex), handle);
-}
-
-int64_t ExchangeWindowBytes(const int world, const int64_t capacity_rows, const int row_floats) {
-	return (int64_t)rgs_exchange_window_bytes(world, capacity_rows, row_floats);
-}
-
-int64_t ExchangeAttach(const int rank, const int world, const int64_t capacity_rows, const int row_floats, const std::vector<int64_t>& window_ptrs,
-                       const int64_t multicast_ptr, const int device) {
-	const c10::cuda::CUDAGuard guard(c10::Device(c10::kCUDA, device));
-	TORCH_CHECK((int)window_ptrs.size() == world, "one window pointer per rank");
-	std::vector<uint64_t> ptrs(window_ptrs.begin(), window_ptrs.end());
-	rgs_exchange* ex = nullptr;
-	if (rgs_exchange_attach(rank, world, capacity_rows, row_floats, ptrs.data(), (uint64_t)multicast_ptr, &ex) != RGS_OK)
-		throw std::runtime_error(rgs_exchange_last_error());
-	return (int64_t)reinterpret_cast<intptr_t>(ex);
 }
 
 void ExchangeConnect(const int64_t ex, const torch::Tensor& all_handles, const int device) {
 	const c10::cuda::CUDAGuard guard(c10::Device(c10::kCUDA, device));
 	torch::Tensor h = all_handles.to(torch::kCPU).contiguous();
 	TORCH_CHECK(h.scalar_type() == torch::kUInt8 && h.numel() % RGS_IPC_HANDLE_BYTES == 0, "handles must be a uint8 tensor [world, 64]");
-	if (rgs_exchange_connect(reinterpret_cast<rgs_exchange*>(ex), h.data_ptr()) != RGS_OK) throw std::runtime_error(rgs_exchange_last_error());
+	check(rgs_exchange_connect(reinterpret_cast<rgs_exchange*>(ex), h.data_ptr()));
 }
 
 // views of the exchange's persistent local accumulator / result rows, and the bare exchange step (self-check, tools)
@@ -529,12 +514,15 @@ torch::Tensor ExchangeResult(const int64_t ex, const int P, const int row_floats
 void ExchangeRows(const int64_t ex, const torch::Tensor& tiles_touched, const torch::Tensor& radii) {
 	const torch::Tensor t = arg(tiles_touched, "tiles_touched", torch::kInt32), r = arg(radii, "radii", torch::kInt32);
 	const c10::cuda::CUDAGuard guard(r.device());
-	if (rgs_exchange_rows(reinterpret_cast<rgs_exchange*>(ex), (int)r.numel(), reinterpret_cast<const uint32_t*>(t.data_ptr<int>()), r.data_ptr<int>(),
-	                      at::cuda::getCurrentCUDAStream().stream()) != RGS_OK)
-		throw std::runtime_error(rgs_exchange_last_error());
+	check(rgs_exchange_rows(reinterpret_cast<rgs_exchange*>(ex), (int)r.numel(), reinterpret_cast<const uint32_t*>(t.data_ptr<int>()), r.data_ptr<int>(),
+	                        at::cuda::getCurrentCUDAStream().stream()));
 }
 
-int ExchangeStatus(const int64_t ex) { return rgs_exchange_status(reinterpret_cast<rgs_exchange*>(ex), at::cuda::getCurrentCUDAStream().stream()); }
+int ExchangeStatus(const int64_t ex) {
+	const int rc = rgs_exchange_status(reinterpret_cast<rgs_exchange*>(ex), at::cuda::getCurrentCUDAStream().stream());
+	check(rc);
+	return rc;
+}
 
 void ExchangeDestroy(const int64_t ex) { rgs_exchange_destroy(reinterpret_cast<rgs_exchange*>(ex)); }
 
@@ -1595,8 +1583,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	m.def("rasterize_gaussians_backward_preprocess", &BackwardPreprocessCUDA);
 	m.def("exchange_create", &ExchangeCreate);
 	m.def("exchange_connect", &ExchangeConnect);
-	m.def("exchange_window_bytes", &ExchangeWindowBytes);
-	m.def("exchange_attach", &ExchangeAttach);
 	m.def("exchange_destroy", &ExchangeDestroy);
 	m.def("exchange_accumulator", &ExchangeAccumulator);
 	m.def("exchange_result", &ExchangeResult);

@@ -3,20 +3,19 @@
 Every rank holds the full Gaussian set and runs preprocess on all of it (identical on every rank); rank r bins,
 sorts and blends only the tile rows of its slab, so the union of the per-rank sorted lists is the reference's
 list.  Backward has exactly one exchange step: the packed screen-space gradient rows written by
-backward-render are plain sums over pixels, hence additive across slabs -- they are summed with ONE all-reduce
-(NCCL over NVLink on GPUs, gloo in the CPU tests) and only then turned into parameter gradients.  The reduce
-has to sit before backward-preprocess, not after it: with kernel_size > 0 that stage multiplies two
-accumulated quantities (the reference's mip-gradient aliasing, SURVEY.md A-14), so per-slab results would not
-add up to the single-GPU answer.
+backward-render are plain sums over pixels, hence additive across slabs -- they are summed once over the ranks
+and only then turned into parameter gradients.  The sum has to sit before backward-preprocess, not after it: with
+kernel_size > 0 that stage multiplies two accumulated quantities (the reference's mip-gradient aliasing, SURVEY.md
+A-14), so per-slab results would not add up to the single-GPU answer.
 
-`backward_two_stage` is written against three callables so that the same control flow is exercised on CPU
-(gloo + the oracle) and on GPUs (NCCL + the CUDA stages).
+The sum is `GradExchange`'s device-side peer exchange or, without one and as its fallback, one all-reduce
+(`allreduce_sum_`: NCCL on GPUs, gloo in the CPU tests, which run it with the oracle's stages in place of the CUDA ones).
 """
 from __future__ import annotations
 
 import math
 import os
-from typing import Callable, List, Sequence, Tuple
+from typing import List, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
@@ -70,67 +69,6 @@ def allreduce_sum_(t: torch.Tensor, group=None) -> torch.Tensor:
     return t
 
 
-def exchange_sum_(acc: torch.Tensor, group=None, mode: str | None = None) -> torch.Tensor:
-    """Sum of the slab-local accumulator rows [P, stride] over the ranks, in place, bit-identical on every rank.
-
-    ``dense`` (default, or ``RGS_GRAD_EXCHANGE``): one all-reduce of the whole tensor.
-    ``sparse`` (opt-in): a rank's rows are zero for every Gaussian that does not reach its slab (with 8 slabs a splat touches
-    1.25 of them on average), so each rank ships only its non-zero rows -- index + row, one all-gather -- and every rank
-    rebuilds the sum by adding the ranks' rows in rank order (fixed order: same bits everywhere, like an all-reduce).
-    Its two size exchanges with their host synchronisations and eight index_add_ passes can cost more than the all-reduce
-    they replace.  Kept because the control flow is the starting point for a fused device-side exchange (no host syncs).
-    """
-    if not (dist.is_available() and dist.is_initialized()):
-        return acc
-    W = dist.get_world_size(group)
-    if W == 1:
-        return acc
-    mode = mode or os.environ.get("RGS_GRAD_EXCHANGE", "dense")
-    if mode == "owner":
-        # Host-side mirror of the device exchange (csrc/rgs_exchange.cu), collective by collective: rows are owned in contiguous
-        # blocks of ceil(P / W); every block is reduced INTO its owner and the owner's sum is then copied to everybody -- one sum per
-        # row, the same bits on every rank.  (The device version moves only the rows that carry something; this one is dense and
-        # exists so that the ownership / reduce / spread logic runs under gloo in the CPU tests.)
-        P = acc.shape[0]
-        rpr = (P + W - 1) // W
-        for owner in range(W):
-            blk = acc[owner * rpr: min(P, (owner + 1) * rpr)]
-            if blk.numel():
-                dist.reduce(blk, dst=dist.get_global_rank(group, owner) if group is not None else owner, op=dist.ReduceOp.SUM, group=group)
-        for owner in range(W):
-            blk = acc[owner * rpr: min(P, (owner + 1) * rpr)]
-            if blk.numel():
-                dist.broadcast(blk, src=dist.get_global_rank(group, owner) if group is not None else owner, group=group)
-        return acc
-    if mode != "sparse":
-        dist.all_reduce(acc, op=dist.ReduceOp.SUM, group=group)
-        return acc
-    idx = torch.nonzero((acc != 0).any(dim=1)).squeeze(1)
-    n_mine = torch.tensor([idx.numel()], dtype=torch.int64, device=acc.device)
-    n_all = [torch.zeros_like(n_mine) for _ in range(W)]
-    dist.all_gather(n_all, n_mine, group=group)
-    counts = [int(c) for c in torch.cat(n_all).tolist()]  # same list on every rank: the branch below is taken by all or none
-    maxn, stride = max(counts), acc.shape[1]
-    rows = torch.zeros(maxn, stride, dtype=acc.dtype, device=acc.device)
-    ids = torch.zeros(maxn, dtype=torch.int32, device=acc.device)
-    rows[: idx.numel()] = acc[idx]
-    ids[: idx.numel()] = idx.to(torch.int32)
-    rows_all = torch.empty(W * maxn, stride, dtype=acc.dtype, device=acc.device)
-    ids_all = torch.empty(W * maxn, dtype=torch.int32, device=acc.device)
-    if dist.get_backend(group) == "nccl":
-        dist.all_gather_into_tensor(rows_all, rows, group=group)
-        dist.all_gather_into_tensor(ids_all, ids, group=group)
-    else:  # gloo (CPU tests) has no flat all-gather
-        dist.all_gather(list(rows_all.view(W, maxn, stride).unbind(0)), rows, group=group)
-        dist.all_gather(list(ids_all.view(W, maxn).unbind(0)), ids, group=group)
-    acc.zero_()
-    for r in range(W):  # rank order, own rows included: indices are unique within a rank, so each add is deterministic
-        k = counts[r]
-        if k:
-            acc.index_add_(0, ids_all[r * maxn: r * maxn + k].long(), rows_all[r * maxn: r * maxn + k])
-    return acc
-
-
 def broadcast_scene_(scene, src: int = 0, group=None):
     """Make a replicated scene (any object whose tensor attributes are the model / camera state) bit-identical on every rank by
     broadcasting rank `src`'s copy -- what a trainer does with its replicated parameters.  Data-parallel slabs only compose to the
@@ -153,8 +91,8 @@ class GradExchange:
     ``peer`` (default on CUDA with NCCL): the library's device-side exchange over peer memory (csrc/rgs_exchange.cu: touched
     rows are reduced into their owner rank with vector reductions through NVLink, the sums are spread to every rank, two
     flag barriers, no host synchronisation; bit-identical rows on all ranks).  torch.distributed is used ONCE, to all-gather
-    the 64-byte IPC handles.  ``dense`` (``RGS_GRAD_EXCHANGE=dense``, and the only mode off-GPU): stage 1 into a fresh tensor
-    + one NCCL / gloo all-reduce of the whole tensor.
+    the 64-byte IPC handles.  ``dense`` (``RGS_GRAD_EXCHANGE=dense``, and the only mode off-GPU or with one rank): stage 1 into
+    a fresh tensor + one NCCL / gloo all-reduce of the whole tensor.  Any other mode raises ``ValueError``.
 
     All ranks must create the object collectively and call ``backward_render`` the same number of times with the same P.
     """
@@ -164,6 +102,8 @@ class GradExchange:
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         mode = mode or os.environ.get("RGS_GRAD_EXCHANGE", "peer")
+        if mode not in ("peer", "dense"):
+            raise ValueError(f"gradient exchange mode must be 'peer' or 'dense', got {mode!r}")
         if self.world == 1 or self.device.type != "cuda":
             mode = "dense"
         self.mode, self.capacity, self.row_floats, self._ex = mode, int(capacity_rows), int(row_floats), None
@@ -171,22 +111,12 @@ class GradExchange:
         if mode == "peer":
             from diff_gaussian_rasterization import _C
             idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
-            if os.environ.get("RGS_EXCHANGE_WINDOW", "ipc") == "symm":
-                # opt-in: windows from torch's symmetric memory (cuMem VMM) with an NVLS multicast mapping -> the spread phase
-                # issues one store per 16 bytes and the NVSwitch replicates it; any failure falls back to the CUDA-IPC windows
-                try:
-                    self._attach_symmetric(_C, idx)
-                except Exception as e:  # noqa: BLE001
-                    import warnings
-                    warnings.warn(f"symmetric-memory windows unavailable ({type(e).__name__}: {e}); using CUDA IPC windows")
-                    self._ex = None
-            if self._ex is None:
-                self._ex, handle = _C.exchange_create(self.rank, self.world, self.capacity, self.row_floats, idx)
-                mine = handle.to(self.device)
-                gathered = [torch.empty_like(mine) for _ in range(self.world)]
-                dist.all_gather(gathered, mine, group=group)
-                _C.exchange_connect(self._ex, torch.stack(gathered).cpu(), idx)
-                self.window = "cuda-ipc"
+            self._ex, handle = _C.exchange_create(self.rank, self.world, self.capacity, self.row_floats, idx)
+            mine = handle.to(self.device)
+            gathered = [torch.empty_like(mine) for _ in range(self.world)]
+            dist.all_gather(gathered, mine, group=group)
+            _C.exchange_connect(self._ex, torch.stack(gathered).cpu(), idx)
+            self.window = "cuda-ipc"
             dist.barrier(group=group)   # nobody pushes before every rank has mapped every window
             why = self._self_check(_C, idx)
             if why is not None:         # the same verdict on every rank (all-reduced): fall back together
@@ -196,20 +126,6 @@ class GradExchange:
                 self.mode = "dense"
 
     fallback_reason = None
-
-    def _attach_symmetric(self, C, idx):
-        import torch.distributed._symmetric_memory as symm_mem
-        nbytes = int(C.exchange_window_bytes(self.world, self.capacity, self.row_floats))
-        buf = symm_mem.empty(nbytes, dtype=torch.uint8, device=torch.device("cuda", idx))
-        g = self.group if self.group is not None else dist.group.WORLD
-        hdl = symm_mem.rendezvous(buf, g.group_name)
-        buf.zero_()
-        torch.cuda.synchronize()
-        dist.barrier(group=self.group)
-        mc = int(hdl.multicast_ptr) if getattr(hdl, "multicast_ptr", 0) else 0
-        self._ex = C.exchange_attach(self.rank, self.world, self.capacity, self.row_floats, [int(p) for p in hdl.buffer_ptrs], mc, idx)
-        self._symm = (buf, hdl)   # keep the allocation alive
-        self.window = "symmetric-memory" + (" + NVLS multicast" if mc else " (no multicast)")
 
     def _self_check(self, C, idx):
         """Two synthetic exchange steps with a known answer before the object is trusted: rank r touches every 3rd row starting at
@@ -256,8 +172,7 @@ class GradExchange:
         """stage 1 (`rasterize_gaussians_backward_render` arguments) + exchange -> summed accumulator rows [P, row_floats]."""
         if self.mode == "peer":
             return C.rasterize_gaussians_backward_render_exchange(self._ex, *stage1_args)
-        acc = C.rasterize_gaussians_backward_render(*stage1_args)
-        return exchange_sum_(acc, self.group, mode="dense")
+        return allreduce_sum_(C.rasterize_gaussians_backward_render(*stage1_args), self.group)
 
     def close(self):
         if self._ex is not None:
@@ -266,13 +181,6 @@ class GradExchange:
                 dist.barrier(group=self.group)   # peers may still be reading / writing this rank's window
             _C.exchange_destroy(self._ex)
             self._ex = None
-
-
-def backward_two_stage(stage1_render: Callable[[], torch.Tensor], stage2_preprocess: Callable[[torch.Tensor], tuple], group=None):
-    """slab-local scatter -> one exchange of the accumulator rows -> replicated parameter gradients."""
-    acc = stage1_render()
-    exchange_sum_(acc, group)
-    return stage2_preprocess(acc)
 
 
 class _ShardedRasterize(torch.autograd.Function):
@@ -305,11 +213,10 @@ class _ShardedRasterize(torch.autograd.Function):
             f = _forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh)
             return _C.rasterize_gaussians_backward_preprocess(acc, *f[:2], radii, *f[2:18], geom, *f[19:])
 
-        if ctx.exchange is not None:   # device-side exchange (or its dense fallback) owned by the caller
-            grads = stage2(ctx.exchange.backward_render(_C, *stage1_args))
-        else:
-            grads = backward_two_stage(lambda: _C.rasterize_gaussians_backward_render(*stage1_args), stage2, ctx.group)
-        g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot = grads
+        # the device-side exchange (or its dense fallback) owned by the caller, else one all-reduce
+        acc = (ctx.exchange.backward_render(_C, *stage1_args) if ctx.exchange is not None
+               else allreduce_sum_(_C.rasterize_gaussians_backward_render(*stage1_args), ctx.group))
+        g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot = stage2(acc)
         return g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, None, None, None, None, None
 
 

@@ -116,8 +116,7 @@ def test_cpu_tensors_are_refused_with_a_cuda_message(name):
 
 def test_every_tensor_entry_is_covered():
     import diff_gaussian_rasterization as dgr
-    handles = {"exchange_create", "exchange_connect", "exchange_window_bytes", "exchange_attach", "exchange_destroy", "exchange_accumulator",
-               "exchange_result", "exchange_status"}
+    handles = {"exchange_create", "exchange_connect", "exchange_destroy", "exchange_accumulator", "exchange_result", "exchange_status"}
     scalars = {"grad_stride", "set_poison", "launch_count", "abi_version", "stage_timing", "stage_times"}
     exported = {n for n in dir(dgr._C) if not n.startswith("_")}
     assert exported - handles - scalars == set(ENTRIES)

@@ -1,8 +1,7 @@
 """World-size-2 test of the multi-GPU control flow on CPU (gloo): slab-local scatter -> ONE all-reduce of the
 screen-space gradient rows -> replicated parameter gradients.  The CUDA stages are replaced by the oracle's
 (oracle.render_backward / oracle.preprocess_backward), the control flow under test is
-rade_gs_b200.multigpu.backward_two_stage / allreduce_sum_ / partition_tile_rows -- the same code the GPU path runs
-with NCCL."""
+rade_gs_b200.multigpu.allreduce_sum_ / partition_tile_rows -- the same code the GPU path runs with NCCL."""
 import math
 import os
 import sys
@@ -58,14 +57,14 @@ def _worker(rank, world, port, case, tmpdir):
                 o += w
             return oracle.preprocess_backward(inp, fwd, sg)
 
-        out = multigpu.backward_two_stage(stage1, stage2)
+        out = stage2(multigpu.allreduce_sum_(stage1()))
         np.savez(os.path.join(tmpdir, f"rank{rank}.npz"), **{k: v for k, v in out.items()})
     finally:
         dist.destroy_process_group()
 
 
 @pytest.mark.parametrize("case", [c for c in ("depth_ks01", "coord_ks0") if c in GOLDEN_CASES])
-def test_two_rank_backward_equals_single(case, tmp_path):
+def test_two_rank_all_reduced_backward_equals_single(case, tmp_path):
     import oracle
     port = 29500 + (os.getpid() % 2000)
     mp.spawn(_worker, args=(2, port, case, str(tmp_path)), nprocs=2, join=True)
@@ -85,6 +84,18 @@ def test_allreduce_is_noop_without_process_group():
     from rade_gs_b200.multigpu import allreduce_sum_
     t = torch.arange(6.0)
     assert torch.equal(allreduce_sum_(t.clone()), t)
+
+
+def test_unknown_exchange_mode_is_refused(monkeypatch):
+    """`peer` and `dense` are the only modes; anything else is refused, also on one process where the mode becomes dense."""
+    from rade_gs_b200.multigpu import GradExchange
+    with pytest.raises(ValueError, match="bogus"):
+        GradExchange(10, 16, "cpu", mode="bogus")
+    monkeypatch.setenv("RGS_GRAD_EXCHANGE", "bogus")
+    with pytest.raises(ValueError, match="bogus"):
+        GradExchange(10, 16, "cpu")
+    monkeypatch.setenv("RGS_GRAD_EXCHANGE", "dense")
+    assert GradExchange(10, 16, "cpu").mode == "dense"
 
 
 def _gather_worker(rank, world, port, tmpdir):
@@ -143,29 +154,23 @@ def _exchange_worker(rank, world, port, tmpdir):
             if density > 0:
                 acc[17] = float(rank + 1)  # a row every rank contributes to
             out[case + "_in"] = acc.clone()
-            out[case + "_sparse"] = multigpu.exchange_sum_(acc.clone(), mode="sparse")
-            out[case + "_dense"] = multigpu.exchange_sum_(acc.clone(), mode="dense")
-            out[case + "_owner"] = multigpu.exchange_sum_(acc.clone(), mode="owner")   # host mirror of the device-side exchange
-            out[case + "_auto"] = multigpu.exchange_sum_(acc.clone())  # default: dense
+            out[case + "_dense"] = multigpu.allreduce_sum_(acc.clone())
+            out[case + "_group"] = multigpu.allreduce_sum_(acc.clone(), dist.group.WORLD)   # an explicit group, as the rasterizer passes it
         torch.save(out, os.path.join(tmpdir, f"exchange{rank}.pt"))
     finally:
         dist.destroy_process_group()
 
 
 @pytest.mark.parametrize("world", [2, 3])
-def test_sparse_row_exchange_equals_the_all_reduce(world, tmp_path):
+def test_row_all_reduce_equals_the_sum_over_ranks(world, tmp_path):
     port = 33500 + (os.getpid() % 2000) + world
     mp.spawn(_exchange_worker, args=(world, port, str(tmp_path)), nprocs=world, join=True)
     res = [torch.load(tmp_path / f"exchange{r}.pt") for r in range(world)]
     for case in ("typical", "empty_rank", "full"):
         total = sum(r[case + "_in"].double() for r in res)
         for r in res:
-            assert torch.equal(r[case + "_sparse"], res[0][case + "_sparse"])  # same bits on every rank, like an all-reduce
-            assert torch.allclose(r[case + "_sparse"].double(), total, rtol=1e-6, atol=1e-6)
             assert torch.allclose(r[case + "_dense"].double(), total, rtol=1e-6, atol=1e-6)
-            assert torch.equal(r[case + "_owner"], res[0][case + "_owner"])    # owner-computed sums: bit-identical on every rank
-            assert torch.allclose(r[case + "_owner"].double(), total, rtol=1e-6, atol=1e-6)
-            assert torch.allclose(r[case + "_auto"].double(), total, rtol=1e-6, atol=1e-6)
+            assert torch.allclose(r[case + "_group"].double(), total, rtol=1e-6, atol=1e-6)
 
 
 # ---- slab-local L1 + SSIM with halo rows: host logic on CPU (gloo), torch expressions standing in for the CUDA kernels -----------
