@@ -140,7 +140,9 @@ __global__ void __launch_bounds__(256) exchange_spread_kernel(int P, int rows_pe
 		if (lane < RQ) {
 			float4* src = my_sum + (size_t)l * RQ + lane;
 			const float4 v = *src;
-			nz = !(v.x == 0.f && v.y == 0.f && v.z == 0.f && v.w == 0.f);
+			// on the bits, not `== 0`: red.add.f32 flushes a subnormal sum to -0.0, which must be cleared from `sum` and
+			// rewritten as +0.0 in `full` next step like any other value
+			nz = (__float_as_uint(v.x) | __float_as_uint(v.y) | __float_as_uint(v.z) | __float_as_uint(v.w)) != 0u;
 			if (nz) *src = make_float4(0.f, 0.f, 0.f, 0.f);
 			for (int p = 0; p < world; p++) reinterpret_cast<float4*>(tab.full[p])[idx * RQ + lane] = v;
 		}
