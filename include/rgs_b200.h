@@ -312,6 +312,51 @@ int32_t rgs_appearance_l1_forward(int32_t H0, int32_t W0, const float* image, co
 int32_t rgs_appearance_l1_backward(int32_t H0, int32_t W0, const float* image, const float* gt, const float* up4, const float* act, const float* w2,
                                    const float* w3, const float* b3, const float* upstream, float* d_image, float* d_up4, float* d_w2, float* d_b2,
                                    float* d_w3, float* d_b3, double* partials, float* d_x, void* cuda_stream);
+/* Row-sharded forms (multi-GPU; added functions, ABI 4).  A slab holds IMAGE rows [row_lo, row_hi), 0 <= row_lo <= row_hi <= H0;
+ * its crop rows are [c0, c1) = clamp([row_lo - top, row_hi - top), 0, H).  Every buffer is a window of whole rows, planar.  The
+ * whole-image functions above are these over [0, H0): the same kernels, tiles and CTAs, hence the same bits.
+ * Ownership partitions the rows of the maps the head exchanges (a slab may own none):
+ *   low-res row oy   the slab whose crop rows hold its upper tap (int)(s * oy) (the downsample's fp32 rule above)
+ *   up4 row u        the slab whose crop rows hold 2u
+ * Halos, from the x2 upsample's tap rule: sy = (H/2 - 1) / (H - 1) < 1/2, so crop row y taps up4 rows within [(y - 2) / 2,
+ * (y + 2) / 2]; the gather of up4 row u reads d_x rows [2u - 2, 2u + 2].  With the owned u's, d_x is needed on crop rows
+ * [c0 - 2, c1 + 2), d(conv2) on [c0 - 3, c1 + 3), the loss derivative (image, gt) on [c0 - 4, c1 + 4) and act on [c0 - 5, c1 + 5),
+ * each clipped to the crop, and each empty when c0 == c1.
+ *
+ * rgs_appearance_row_windows: windows[RGS_APPEARANCE_WINDOWS] = {c0, c1, oy_lo, oy_hi, u_lo, u_hi, act_lo, act_hi, dx_lo, dx_hi,
+ *   img_lo, img_hi}: the counted crop rows, the owned low-res and up4 rows, and the crop rows of act, d_x and of the image / gt
+ *   rows backward reads.  Host only.
+ * rgs_appearance_downsample_rows: down [3, oy_hi - oy_lo, w] = the owned low-res rows, each bit-identical to the whole map's.
+ *   image holds image rows [image_lo, image_lo + image_rows) of the render, inside the image and holding crop rows
+ *   [c0, min(c1 + 1, H)) (the taps reach at most one row below the slab).
+ * rgs_appearance_l1_forward_rows: image and gt are windows of the same rows [image_lo, image_lo + image_rows), holding crop rows
+ *   [c0, c1).  up4 is the whole head output.  act [16, act_hi - act_lo, W] receives A on crop rows [act_lo, act_hi).  loss_sum[0]
+ *   (fp64, not divided) = the sum of |M * crop - gt| over crop rows [c0, c1), in the whole call's order (fp32 per tile, fp64
+ *   over the tiles of each of RGS_APPEARANCE_CTAS CTAs, then over the CTAs); partials: RGS_APPEARANCE_CTAS doubles of scratch.
+ *   The loss of the whole image is (float)(sum over slabs of loss_sum / (3 H W)).
+ * rgs_appearance_l1_backward_rows: image and gt windows as in forward, holding crop rows [img_lo, img_hi); act is forward's.
+ *   d_image [3, row_hi - row_lo, W0], fully written: the slab's rows of the whole call's d_image (zero outside the crop),
+ *   bit-identical.  d_up4 [16, u_hi - u_lo, W/2] = the owned up4 rows of the whole call's d_up4, bit-identical: d_x is computed
+ *   completely on crop rows [dx_lo, dx_hi), which evaluates the loss derivative also at halo pixels whose loss a neighbour
+ *   counts.  grad_row [RGS_APPEARANCE_GRAD_FLOATS] (fp64, not cast): dW2 [16,16,3,3], db2 [16], dW3 [3,16,3,3], db3 [3] over
+ *   crop rows [c0, c1), summed per CTA over its tiles and then over the CTAs in order.  partials: RGS_APPEARANCE_CTAS x
+ *   RGS_APPEARANCE_GRAD_FLOATS doubles, d_x: 16 x (dx_hi - dx_lo) x W floats, both scratch.
+ * rgs_appearance_downsample_backward_rows: d_image [3, row_hi - row_lo, W0] += the taps of the whole d_down [3, h, w] that
+ *   land in rows [row_lo, row_hi), in the whole call's order: each element gets the whole call's bits.
+ * A slab without crop rows launches no kernel: loss_sum = 0, grad_row = 0, d_image = 0. */
+#define RGS_APPEARANCE_WINDOWS 12
+int32_t rgs_appearance_row_windows(int32_t H0, int32_t W0, int32_t row_lo, int32_t row_hi, int32_t* windows);
+int32_t rgs_appearance_downsample_rows(int32_t H0, int32_t W0, int32_t row_lo, int32_t row_hi, const float* image, int32_t image_lo, int32_t image_rows,
+                                       float* down, void* cuda_stream);
+int32_t rgs_appearance_downsample_backward_rows(int32_t H0, int32_t W0, int32_t row_lo, int32_t row_hi, const float* d_down, float* d_image,
+                                                void* cuda_stream);
+int32_t rgs_appearance_l1_forward_rows(int32_t H0, int32_t W0, int32_t row_lo, int32_t row_hi, const float* image, const float* gt, int32_t image_lo,
+                                       int32_t image_rows, const float* up4, const float* w2, const float* b2, const float* w3, const float* b3, float* act,
+                                       double* partials, double* loss_sum, void* cuda_stream);
+int32_t rgs_appearance_l1_backward_rows(int32_t H0, int32_t W0, int32_t row_lo, int32_t row_hi, const float* image, const float* gt, int32_t image_lo,
+                                        int32_t image_rows, const float* up4, const float* act, const float* w2, const float* w3, const float* b3,
+                                        const float* upstream, float* d_image, float* d_up4, double* grad_row, double* partials, float* d_x,
+                                        void* cuda_stream);
 
 /* ---- initial Gaussian scales: simple_knn's distCUDA2 (reference scene/gaussian_model.py:20, :315-316) ----
  * points [P,3] (device, fp32) -> mean_dist2 [P] (device): the mean of the squared Euclidean distances from point i to its 3 nearest

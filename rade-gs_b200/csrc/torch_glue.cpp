@@ -816,6 +816,112 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
 	return std::make_tuple(d_img, d_up4, d_w2, d_b2, d_w3, d_b3);
 }
 
+// Row-sharded forms (rgs_appearance_*_rows).  The image and gt windows hold image rows [image_lo, image_lo + rows) of an
+// H0-row image; the slab is image rows [row_lo, row_hi).
+
+// (c0, c1, oy_lo, oy_hi, u_lo, u_hi, act_lo, act_hi, dx_lo, dx_hi, img_lo, img_hi); host only
+std::vector<int64_t> AppearanceRowWindows(const int64_t H0, const int64_t W0, const int64_t row_lo, const int64_t row_hi) {
+	int32_t w[RGS_APPEARANCE_WINDOWS];
+	check(rgs_appearance_row_windows((int)H0, (int)W0, (int)row_lo, (int)row_hi, w));
+	return std::vector<int64_t>(w, w + RGS_APPEARANCE_WINDOWS);
+}
+
+struct AppearanceSlab {
+	int32_t H0, W0, row_lo, row_hi, image_lo, win[RGS_APPEARANCE_WINDOWS];
+};
+
+AppearanceSlab appearance_slab(const torch::Tensor& window, const int64_t image_lo, const int64_t H0, const int64_t row_lo, const int64_t row_hi) {
+	AppearanceSlab s;
+	s.H0 = (int32_t)H0; s.W0 = (int32_t)window.size(2); s.row_lo = (int32_t)row_lo; s.row_hi = (int32_t)row_hi; s.image_lo = (int32_t)image_lo;
+	check(rgs_appearance_row_windows(s.H0, s.W0, s.row_lo, s.row_hi, s.win));
+	return s;
+}
+
+// image window [3, rows, W0] -> the owned low-res rows [3, oy_hi - oy_lo, W0 / 32]
+torch::Tensor AppearanceDownsampleRows(const torch::Tensor& image, const int64_t image_lo, const int64_t H0, const int64_t row_lo, const int64_t row_hi) {
+	const torch::Tensor a = arg(image, "image window", torch::kFloat32, {3, -1, -1}, "[3, rows, W]");
+	const c10::cuda::CUDAGuard guard(a.device());
+	const AppearanceSlab s = appearance_slab(a, image_lo, H0, row_lo, row_hi);
+	torch::Tensor down = new_empty({3, s.win[3] - s.win[2], s.W0 / 32}, a.options());
+	check(rgs_appearance_downsample_rows(s.H0, s.W0, s.row_lo, s.row_hi, a.data_ptr<float>(), s.image_lo, (int32_t)a.size(1), down.data_ptr<float>(),
+	                                     at::cuda::getCurrentCUDAStream().stream()));
+	return down;
+}
+
+// d_image [3, row_hi - row_lo, W0] += the taps of d_down [3, H/32, W/32] in the slab's rows (in place)
+void AppearanceDownsampleBackwardRows(const torch::Tensor& d_down, torch::Tensor& d_image, const int64_t H0, const int64_t row_lo, const int64_t row_hi) {
+	arg(d_image, "d_image", torch::kFloat32, {3, row_hi - row_lo, -1}, "[3, row_hi - row_lo, W]", nullptr, REJECT);
+	const int32_t W0 = (int32_t)d_image.size(2);
+	const torch::Tensor g = arg(d_down, "d_down", torch::kFloat32, {3, H0 / 32, W0 / 32}, "[3, H/32, W/32]", &d_image);
+	const c10::cuda::CUDAGuard guard(d_image.device());
+	check(rgs_appearance_downsample_backward_rows((int32_t)H0, W0, (int32_t)row_lo, (int32_t)row_hi, g.data_ptr<float>(), d_image.data_ptr<float>(),
+	                                              at::cuda::getCurrentCUDAStream().stream()));
+}
+
+AppearanceArgs appearance_rows_args(const torch::Tensor& image, const torch::Tensor& gt, const torch::Tensor& up4, const torch::Tensor& w2,
+                                    const torch::Tensor& b2, const torch::Tensor& w3, const torch::Tensor& b3, const int64_t H0) {
+	AppearanceArgs a;
+	a.image = arg(image, "image window", torch::kFloat32, {3, -1, -1}, "[3, rows, W]");
+	a.H0 = (int)H0;
+	a.W0 = (int)image.size(2);
+	TORCH_CHECK(gt.sizes() == image.sizes(), "gt window must have the image window's shape");
+	a.gt = arg(gt, "gt window", torch::kFloat32, {}, "", &a.image);
+	const int64_t H = H0 / 32 * 32, W = a.W0 / 32 * 32;
+	a.up4 = arg(up4, "up4 output", torch::kFloat32, {}, "", &a.image);
+	TORCH_CHECK(a.up4.numel() == 16 * (H / 2) * (W / 2), "up4 output must be [1, 16, ", H / 2, ", ", W / 2, "], got ", up4.sizes());
+	a.w2 = arg(w2, "conv2 weight", torch::kFloat32, {16, 16, 3, 3}, "[16, 16, 3, 3]", &a.image);
+	a.b2 = arg(b2, "conv2 bias", torch::kFloat32, {16}, "[16]", &a.image);
+	a.w3 = arg(w3, "conv3 weight", torch::kFloat32, {3, 16, 3, 3}, "[3, 16, 3, 3]", &a.image);
+	a.b3 = arg(b3, "conv3 bias", torch::kFloat32, {3}, "[3]", &a.image);
+	return a;
+}
+
+// returns (loss_sum [1] float64, act [16, act_hi - act_lo, W])
+std::tuple<torch::Tensor, torch::Tensor> AppearanceL1ForwardRows(const torch::Tensor& image, const torch::Tensor& gt, const int64_t image_lo, const int64_t H0,
+                                                                 const int64_t row_lo, const int64_t row_hi, const torch::Tensor& up4, const torch::Tensor& w2,
+                                                                 const torch::Tensor& b2, const torch::Tensor& w3, const torch::Tensor& b3) {
+	const AppearanceArgs a = appearance_rows_args(image, gt, up4, w2, b2, w3, b3, H0);
+	const c10::cuda::CUDAGuard guard(a.image.device());
+	const AppearanceSlab s = appearance_slab(a.image, image_lo, H0, row_lo, row_hi);
+	const auto o = a.image.options();
+	torch::Tensor act = new_empty({16, s.win[7] - s.win[6], a.W0 / 32 * 32}, o);
+	torch::Tensor partials = new_empty({RGS_APPEARANCE_CTAS}, o.dtype(torch::kFloat64));
+	torch::Tensor loss_sum = new_empty({1}, o.dtype(torch::kFloat64));
+	check(rgs_appearance_l1_forward_rows(s.H0, s.W0, s.row_lo, s.row_hi, a.image.data_ptr<float>(), a.gt.data_ptr<float>(), s.image_lo, (int32_t)a.image.size(1),
+	                                     a.up4.data_ptr<float>(), a.w2.data_ptr<float>(), a.b2.data_ptr<float>(), a.w3.data_ptr<float>(), a.b3.data_ptr<float>(),
+	                                     act.data_ptr<float>(), partials.data_ptr<double>(), loss_sum.data_ptr<double>(), at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(loss_sum, act);
+}
+
+// returns (d_image [3, row_hi - row_lo, W0] (crop term only), d_up4 owned rows [16, u_hi - u_lo, W/2], grad_row [2755] float64)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> AppearanceL1BackwardRows(
+    const torch::Tensor& image, const torch::Tensor& gt, const int64_t image_lo, const int64_t H0, const int64_t row_lo, const int64_t row_hi,
+    const torch::Tensor& up4, const torch::Tensor& act, const torch::Tensor& w2, const torch::Tensor& b2, const torch::Tensor& w3, const torch::Tensor& b3,
+    const torch::Tensor& upstream) {
+	const AppearanceArgs a = appearance_rows_args(image, gt, up4, w2, b2, w3, b3, H0);
+	const c10::cuda::CUDAGuard guard(a.image.device());
+	const AppearanceSlab s = appearance_slab(a.image, image_lo, H0, row_lo, row_hi);
+	const int64_t W = a.W0 / 32 * 32;
+	const torch::Tensor ac = arg(act, "activations", torch::kFloat32, {16, s.win[7] - s.win[6], W}, "[16, act_hi - act_lo, W]", &a.image);
+	const float* up_ptr = nullptr;
+	torch::Tensor up;
+	if (upstream.defined() && upstream.numel() != 0) {
+		TORCH_CHECK(upstream.numel() == 1, "appearance loss backward: upstream gradient must be a scalar");
+		up = arg(upstream, "upstream gradient", torch::kFloat32, {}, "", &a.image);
+		up_ptr = up.data_ptr<float>();
+	}
+	const auto o = a.image.options();
+	torch::Tensor d_img = new_empty({3, row_hi - row_lo, a.W0}, o), d_up4 = new_empty({16, s.win[5] - s.win[4], W / 2}, o);
+	torch::Tensor grad_row = new_empty({RGS_APPEARANCE_GRAD_FLOATS}, o.dtype(torch::kFloat64));
+	torch::Tensor partials = new_empty({RGS_APPEARANCE_CTAS, RGS_APPEARANCE_GRAD_FLOATS}, o.dtype(torch::kFloat64));
+	torch::Tensor d_x = new_empty({16, s.win[9] - s.win[8], W}, o);
+	check(rgs_appearance_l1_backward_rows(s.H0, s.W0, s.row_lo, s.row_hi, a.image.data_ptr<float>(), a.gt.data_ptr<float>(), s.image_lo,
+	                                      (int32_t)a.image.size(1), a.up4.data_ptr<float>(), ac.data_ptr<float>(), a.w2.data_ptr<float>(), a.w3.data_ptr<float>(),
+	                                      a.b3.data_ptr<float>(), up_ptr, d_img.data_ptr<float>(), d_up4.data_ptr<float>(), grad_row.data_ptr<double>(),
+	                                      partials.data_ptr<double>(), d_x.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(d_img, d_up4, grad_row);
+}
+
 // ---- densify-and-prune and opacity reset (scene/gaussian_model.py:495-513, :662-741; rgs_densify_*, rgs_reset_opacity) ----------
 
 // a per-Gaussian input: float32 on `like`'s device with `width` floats per row over P rows
@@ -1698,6 +1804,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	sl.def("normal_consistency_rows", &NormalConsistencyRows, py::arg("rendered_normal"), py::arg("map_expected"), py::arg("map_median"),
 	       py::arg("from_depth"), py::arg("inv_fx"), py::arg("inv_fy"), py::arg("cx"), py::arg("cy"), py::arg("w_expected"), py::arg("w_median"), py::arg("H"),
 	       py::arg("row_lo"), py::arg("row_hi"));
+	sl.def("appearance_row_windows", &AppearanceRowWindows, py::arg("H0"), py::arg("W0"), py::arg("row_lo"), py::arg("row_hi"));
+	sl.def("appearance_downsample_rows", &AppearanceDownsampleRows, py::arg("image"), py::arg("image_lo"), py::arg("H0"), py::arg("row_lo"),
+	       py::arg("row_hi"));
+	sl.def("appearance_downsample_backward_rows", &AppearanceDownsampleBackwardRows, py::arg("d_down"), py::arg("d_image"), py::arg("H0"), py::arg("row_lo"),
+	       py::arg("row_hi"));
+	sl.def("appearance_l1_forward_rows", &AppearanceL1ForwardRows, py::arg("image"), py::arg("gt"), py::arg("image_lo"), py::arg("H0"), py::arg("row_lo"),
+	       py::arg("row_hi"), py::arg("up4"), py::arg("w2"), py::arg("b2"), py::arg("w3"), py::arg("b3"));
+	sl.def("appearance_l1_backward_rows", &AppearanceL1BackwardRows, py::arg("image"), py::arg("gt"), py::arg("image_lo"), py::arg("H0"), py::arg("row_lo"),
+	       py::arg("row_hi"), py::arg("up4"), py::arg("act"), py::arg("w2"), py::arg("b2"), py::arg("w3"), py::arg("b3"), py::arg("upstream"));
 	m.def("grad_stride",[](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });

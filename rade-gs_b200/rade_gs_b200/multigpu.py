@@ -448,8 +448,8 @@ def _cuda_normal_rows(normal_win, e_win, m_win, from_depth, inv_fx, inv_fy, cx, 
     return _C._slab.normal_consistency_rows(normal_win, e_win, m_win, from_depth, inv_fx, inv_fy, cx, cy, w_e, w_m, H, r0, r1)
 
 
-def _check_slab_rows(pixel_rows, all_pixel_rows, H, rank, world_size):
-    """Raise unless the slab rows suit the 2-row halo exchange.  With `all_pixel_rows` (every rank's rows, e.g.
+def _check_slab_rows(pixel_rows, all_pixel_rows, H, rank, world_size, halo=NORMAL_HALO, what="slab-local normal consistency"):
+    """Raise unless the slab rows suit the `halo`-row exchange.  With `all_pixel_rows` (every rank's rows, e.g.
     `[(min(b * 16, H), min(e * 16, H)) for b, e in rast.slabs]`) every rank checks the whole partition and all raise the same error
     before any collective.  Without it a rank sees only its own rows: a rank whose slab is too short raises, and its neighbours
     then wait in the halo exchange for rows that never come."""
@@ -464,9 +464,9 @@ def _check_slab_rows(pixel_rows, all_pixel_rows, H, rank, world_size):
         if rows[0][0] != 0 or rows[-1][1] != H or any(rows[i][1] != rows[i + 1][0] or rows[i][0] > rows[i][1] for i in range(len(rows) - 1)):
             raise ValueError(f"all_pixel_rows must tile the image's {H} rows in rank order, got {rows}")
     if world_size > 1:
-        short = [(b, e) for b, e in rows if e - b < NORMAL_HALO and e < H]
+        short = [(b, e) for b, e in rows if e - b < halo and e < H]
         if short:
-            raise ValueError("slab-local normal consistency needs every slab that does not end at the image's last row to hold at least 2 pixel "
+            raise ValueError(f"{what} needs every slab that does not end at the image's last row to hold at least {halo} pixel "
                              f"rows (a shorter slab breaks the neighbour halo exchange); slabs {short} do not")
     return r0, r1
 
@@ -533,3 +533,178 @@ def slab_point_normal_consistency_loss(normal: torch.Tensor, expected_coord: tor
     H = _image_height(normal, pixel_rows, image_height, world_size, group)
     return _slab_normal_loss(normal, expected_coord, median_coord, False, (0.0, 0.0, 0.0, 0.0), depth_ratio, H, pixel_rows, all_pixel_rows, rank,
                              world_size, group, kernels, 3)
+
+
+# ---- slab-local decoupled-appearance L1 (train.py:37-58) ---------------------------------------------------------------------
+APPEARANCE_HALO = 4   # image rows either side of a slab whose loss derivative its d_up4 rows need (include/rgs_b200.h)
+
+
+def _gather_rows(mine: torch.Tensor, ranges, n_rows: int, group) -> torch.Tensor:
+    """The whole [C, n_rows, ...] map from each rank's rows `ranges[r]` (`mine` holds this rank's): an all-gather of pure copies,
+    so every rank holds the bits their owners computed."""
+    if len(ranges) == 1:
+        return mine
+    hmax = max(e - b for b, e in ranges)
+    buf = mine.new_zeros(mine.shape[0], hmax, *mine.shape[2:])
+    buf[:, :mine.shape[1]] = mine
+    parts = [torch.empty_like(buf) for _ in ranges]
+    dist.all_gather(parts, buf, group=group)
+    out = mine.new_empty(mine.shape[0], n_rows, *mine.shape[2:])
+    for (b, e), p in zip(ranges, parts):
+        out[:, b:e] = p[:, :e - b]
+    return out
+
+
+def _sum_in_rank_order(mine: torch.Tensor, world: int, group) -> torch.Tensor:
+    """The fp64 per-rank values added in rank order (the same bits on every rank, whatever the collective's own order)."""
+    if world == 1:
+        return mine
+    parts = [torch.empty_like(mine) for _ in range(world)]
+    dist.all_gather(parts, mine, group=group)
+    total = parts[0]
+    for p in parts[1:]:
+        total = total + p
+    return total
+
+
+class _SlabAppearanceL1(torch.autograd.Function):
+    """train.py:37-58's `L1_loss_appearance` of the WHOLE image, evaluated slab by slab (include/rgs_b200.h's
+    `rgs_appearance_*_rows`).  Forward: 4 image rows to and from each neighbour, the owned low-resolution rows all-gathered, the
+    cuDNN head replicated on every rank, the tail on the slab, and the per-rank fp64 loss sums all-gathered and added in rank order.
+    Backward: the owned rows of d(up4) all-gathered, so that the head's backward, d(down) and the embedding gradient are the
+    single-GPU call's; the per-rank fp64 rows of conv2 / conv3's weight gradients added in rank order.  The image is never gathered.
+    `kernels` supplies the four row stages (the CUDA ones, or fp64 stand-ins in the CPU test)."""
+
+    @staticmethod
+    def forward(ctx, image, gt, emb, net, slab, kernels, *params):
+        H0, rows, rank, world, group = slab
+        from diff_gaussian_rasterization import _C
+        from .appearance import _head, _head_input
+        r0, r1 = rows[rank]
+        W0 = gt.shape[-1]
+        compact = image.shape[-2] != H0
+        H, W = H0 // 32 * 32, W0 // 32 * 32
+        wins = [_C._slab.appearance_row_windows(H0, W0, b, e) for b, e in rows]
+        lo, hi = max(0, r0 - APPEARANCE_HALO), min(H0, r1 + APPEARANCE_HALO)
+        win = image.new_zeros(3, hi - lo, W0)
+        a, b = r0 - lo, r1 - lo
+        if r1 > r0:
+            win[:, a:b] = image.detach() if compact else image.detach()[:, r0:r1]
+            k = min(APPEARANCE_HALO, r1 - r0)
+            # a slab that ends at the image's last row has no neighbour below (later ranks' slabs are empty there)
+            _exchange_rows(win, (a, a + k), (b - k, b) if r1 < H0 else (b, b), (0, a), (b, hi - lo), rank, world, group, add=False)
+        gt_win = gt.detach()[:, lo:hi].contiguous()
+        down = _gather_rows(kernels.downsample_rows(win, lo, H0, r0, r1), [(w[2], w[3]) for w in wins], H // 32, group)
+        with torch.enable_grad():
+            d_leaf = down.detach().requires_grad_(True)
+            e_leaf = emb.detach().requires_grad_(True)
+            up4 = _head(net, _head_input(d_leaf, e_leaf))
+        w2, b2, w3, b3 = (p.detach() for p in (net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias))
+        loss_sum, act = kernels.l1_forward_rows(win, gt_win, lo, H0, r0, r1, up4.detach(), w2, b2, w3, b3)
+        total = _sum_in_rank_order(loss_sum.clone(), world, group)
+        ctx.head = (up4, d_leaf, e_leaf, params[:-4])
+        ctx.meta = (H0, lo, r0, r1, compact, [(w[4], w[5]) for w in wins], world, group, kernels)
+        ctx.save_for_backward(win, gt_win, act, w2, b2, w3, b3)
+        return (total[0] / (3.0 * H * W)).to(gt.dtype)   # float32 on the GPU, as L1_loss_appearance returns it
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        win, gt_win, act, w2, b2, w3, b3 = ctx.saved_tensors
+        up4, d_leaf, e_leaf, head_params = ctx.head
+        H0, lo, r0, r1, compact, u_rows, world, group, kernels = ctx.meta
+        d_img, d_up4, grad_row = kernels.l1_backward_rows(win, gt_win, lo, H0, r0, r1, up4.detach(), act, w2, b2, w3, b3,
+                                                          grad_out.float().reshape(1))
+        d_up4 = _gather_rows(d_up4, u_rows, up4.shape[-2], group).reshape(up4.shape)
+        grads = torch.autograd.grad(up4, [d_leaf, e_leaf, *head_params], d_up4)
+        g = _sum_in_rank_order(grad_row.clone(), world, group).to(w2.dtype)
+        d_w2, d_b2, d_w3, d_b3 = g[:2304].view(w2.shape), g[2304:2320].view(b2.shape), g[2320:2752].view(w3.shape), g[2752:].view(b3.shape)
+        kernels.downsample_backward_rows(grads[0], d_img, H0, r0, r1)
+        if not compact:
+            full = d_img.new_zeros(3, H0, d_img.shape[-1])
+            full[:, r0:r1] = d_img
+            d_img = full
+        ctx.head = None
+        return (d_img, None, grads[1], None, None, None, *grads[2:], d_w2, d_b2, d_w3, d_b3)
+
+
+class _CudaAppearanceRows:
+    """The CUDA row stages (`_C._slab.appearance_*_rows`)."""
+
+    @staticmethod
+    def downsample_rows(win, lo, H0, r0, r1):
+        from diff_gaussian_rasterization import _C
+        return _C._slab.appearance_downsample_rows(win, lo, H0, r0, r1)
+
+    @staticmethod
+    def l1_forward_rows(win, gt_win, lo, H0, r0, r1, up4, w2, b2, w3, b3):
+        from diff_gaussian_rasterization import _C
+        return _C._slab.appearance_l1_forward_rows(win, gt_win, lo, H0, r0, r1, up4, w2, b2, w3, b3)
+
+    @staticmethod
+    def l1_backward_rows(win, gt_win, lo, H0, r0, r1, up4, act, w2, b2, w3, b3, upstream):
+        from diff_gaussian_rasterization import _C
+        return _C._slab.appearance_l1_backward_rows(win, gt_win, lo, H0, r0, r1, up4, act, w2, b2, w3, b3, upstream)
+
+    @staticmethod
+    def downsample_backward_rows(d_down, d_img, H0, r0, r1):
+        from diff_gaussian_rasterization import _C
+        _C._slab.appearance_downsample_backward_rows(d_down, d_img, H0, r0, r1)
+
+
+def slab_L1_loss_appearance(image: torch.Tensor, gt_image: torch.Tensor, gaussians, view_idx, pixel_rows: Tuple[int, int], all_pixel_rows=None,
+                            image_height: int | None = None, rank: int | None = None, world_size: int | None = None, group=None, kernels=None,
+                            return_transformed_image: bool = False) -> torch.Tensor:
+    """`appearance.L1_loss_appearance` (train.py:37-58, `--use_decoupled_appearance`) for a row-sharded render.  `image` is
+    `ShardedGaussianRasterizer`'s colour: compact ([3, slab rows, W]) or full-size with this rank's slab rows `pixel_rows` filled;
+    `gt_image` is the whole ground truth [3, H, W], as train.py holds it (it also gives the image height; `image_height`, when
+    given, must agree).  Returns the whole image's loss, the same value on every rank.  Its gradient w.r.t. `image` lies in this
+    rank's rows and is complete there; the network's parameter gradients and the embedding row's are the same bits on every rank.
+    Only conv2 / conv3's weight gradients and the loss are summed in another order than the single-GPU call's (fp64 per rank, then
+    over the ranks in rank order); at one rank every result is that call's, bit for bit.  Bit-identical head gradients across ranks
+    (and across calls) need `torch.backends.cudnn.deterministic = True`, as for the single-GPU call.
+
+    Every slab that does not end at the image's last row must hold at least 4 rows (the halo).  With `all_pixel_rows`, every rank's
+    row range, every rank refuses a bad partition before any collective; without it the ranks first all-gather their row ranges
+    (one small collective) and then all refuse a bad partition together.  The checks of a rank's own arguments (the network, the
+    image's shape, CUDA tensors) run before that gather: a rank whose own arguments are wrong raises alone, and without
+    `all_pixel_rows` its peers then wait in the gather.  `return_transformed_image` has no slab form."""
+    if return_transformed_image:
+        raise ValueError("slab_L1_loss_appearance has no transformed-image form: gather the image and call appearance.L1_loss_appearance")
+    from .appearance import _check_network
+    net = gaussians.appearance_network
+    _check_network(net)
+    if gt_image.requires_grad:
+        raise ValueError("slab_L1_loss_appearance differentiates w.r.t. the rendered image, not the ground truth")
+    if gt_image.dim() != 3 or gt_image.shape[0] != 3 or gt_image.shape[1] < 32 or gt_image.shape[2] < 32:
+        raise ValueError(f"slab_L1_loss_appearance needs a [3, H, W] ground truth with H, W >= 32, got {tuple(gt_image.shape)}")
+    H0, W0 = gt_image.shape[1:]
+    if image_height is not None and int(image_height) != H0:
+        raise ValueError(f"image_height {image_height} is not the ground truth's {H0} rows")
+    if world_size is None:
+        world_size = dist.get_world_size(group) if dist.is_initialized() else 1
+    if rank is None:
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+    what = "the slab-local appearance loss"
+    # without every rank's rows, the slab lengths are checked after the rows are gathered, so that all ranks raise together
+    r0, r1 = _check_slab_rows(pixel_rows, all_pixel_rows, H0, rank, world_size if all_pixel_rows is not None else 1, APPEARANCE_HALO, what)
+    if image.dim() != 3 or image.shape[0] != 3 or image.shape[2] != W0 or image.shape[1] not in (H0, r1 - r0):
+        raise ValueError(f"image must be [3, {H0} or {r1 - r0} rows, {W0}] (full-size or the slab's rows), got {tuple(image.shape)}")
+    if kernels is None and not (image.is_cuda and gt_image.is_cuda):
+        raise RuntimeError("slab_L1_loss_appearance needs CUDA tensors: there is no CPU path")
+    if all_pixel_rows is not None:
+        rows = [(int(b), int(e)) for b, e in all_pixel_rows]
+    elif world_size > 1:
+        mine = torch.tensor([r0, r1], dtype=torch.int64, device=image.device)
+        parts = [torch.empty_like(mine) for _ in range(world_size)]
+        dist.all_gather(parts, mine, group=group)
+        rows = [tuple(int(v) for v in p.tolist()) for p in parts]
+        _check_slab_rows(pixel_rows, rows, H0, rank, world_size, APPEARANCE_HALO, what)
+    else:
+        rows = [(r0, r1)]
+    head = [p for m in (net.conv1, net.up1, net.up2, net.up3, net.up4) for p in m.parameters()]
+    params = head + [net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias]
+    if len(params) != len(list(net.parameters())):
+        raise ValueError("appearance network: parameters outside conv1, up1..up4, conv2 and conv3 are not supported")
+    emb = gaussians.get_apperance_embedding(view_idx)
+    return _SlabAppearanceL1.apply(image, gt_image, emb, net, (H0, rows, rank, world_size, group), kernels or _CudaAppearanceRows, *params)
