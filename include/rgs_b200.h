@@ -111,6 +111,40 @@ typedef struct rgs_buffers {
 int64_t rgs_forward(const rgs_camera* cam, const rgs_gaussians* g, const rgs_forward_out* out,
                     const rgs_buffers* bufs, void* cuda_stream);
 
+/* ---- balanced row sharding: each frame's slabs cut from that frame's instance counts (DESIGN.md "Multi-GPU") ----
+ * Partition rule, integer-only, the same on every rank because preprocess and the tile counts are:
+ *   - I_y = instances (splat-tile pairs) in tile row y, over the whole image; grid_x tiles per row;
+ *   - row weight w_y = I_y + RGS_BALANCE_TILE_COST * grid_x: the blend kernels pay per instance and, per tile, a fixed cost
+ *     (CTA start, per-pixel set-up, the seven map writes, backward's per-pixel reads) worth RGS_BALANCE_TILE_COST instances;
+ *   - every slab holds at least one tile row (grid_y < world_size is RGS_E_INVALID);
+ *   - B* = the least possible largest slab weight over all such partitions into world_size contiguous slabs;
+ *   - cut greedily: ranks in order, each takes rows while its weight stays <= B* and enough rows remain for one per later
+ *     rank; the last rank takes the rest (its weight is <= B* too).
+ * row_cuts (host, world_size + 1 entries) receives the slab boundaries: rank r owns tile rows [row_cuts[r], row_cuts[r+1]).
+ * row_instances is a host array of grid_y counts.  Host-only, no GPU needed. */
+#define RGS_BALANCE_TILE_COST 2048
+int32_t rgs_balance_partition(int32_t grid_y, int32_t grid_x, int32_t world_size, const uint32_t* row_instances, int32_t* row_cuts);
+
+/* Maps callback of rgs_forward_balanced: the slab is known only after the frame's tile counts are read, so the caller allocates
+ * the forward maps then.  Receives the chosen tile rows [tile_row_begin, tile_row_end) and the maps' height (the slab's pixel rows
+ * with cam->compact_slab, else the image height); sets out's seven map pointers ([C, height, W] each; with full-size maps the rows
+ * outside the slab are the caller's to fill, as for rgs_forward).  Returns 0, or non-zero when it could not allocate. */
+typedef int32_t (*rgs_maps_fn)(void* user, int32_t tile_row_begin, int32_t tile_row_end, int32_t height, rgs_forward_out* out);
+
+/* rgs_forward for rank `rank` of `world_size` with the slab chosen from this frame:
+ *   preprocess over the whole image's tile rows -> tile counts -> per-row I_y and L_y (longest tile list of the row) -> ONE
+ *   host read (it replaces rgs_forward's read of num_rendered; still the only synchronisation) -> rgs_balance_partition ->
+ *   the tile ranges, chunk offsets, totals and per-splat tile counts restricted to this rank's slab -> `maps` -> binning,
+ *   sort and blend of the slab.
+ * Binning, sort, blend and the buffers left for backward are exactly those of rgs_forward with cam->tile_row_begin/end set to
+ * the chosen slab, so backward is rgs_backward_render / rgs_backward_render_exchange with those rows.  cam->tile_row_begin /
+ * tile_row_end are ignored.  out->radii is used as given, out's map pointers are set by `maps`.  row_cuts (host, world_size + 1)
+ * receives the whole partition; row_stats (host, 2 * grid_y, may be NULL) receives I_y then L_y.  Returns num_rendered of the
+ * slab or a negative rgs_status. */
+int64_t rgs_forward_balanced(const rgs_camera* cam, const rgs_gaussians* g, int32_t world_size, int32_t rank, rgs_forward_out* out,
+                             rgs_maps_fn maps, void* maps_user, const rgs_buffers* bufs, int32_t* row_cuts, uint32_t* row_stats,
+                             void* cuda_stream);
+
 /* ---- opacity integration at query points (SURVEY.md 8f-3) ----
  * Replaces CudaRasterizer::Rasterizer::integrate (rasterizer.h:68-108, rasterizer_impl.cu:573-844; binding
  * rasterize_points.cu:269-388).  All outputs are fully written by the call (untouched points get the reference's fill values

@@ -122,6 +122,22 @@ static ImgView carve_img(char* base, int grid_x, int grid_y, size_t N, bool coor
 	return v;
 }
 
+// The whole image's tile counts of a balanced forward before its slab is chosen: the scan's per-tile arrays, its difference grid
+// and the per-row statistics (3 words per tile row, rgs_balance.cu's row_stats_kernel).
+static ImgView carve_counts(char* base, int grid_x, int grid_y, uint32_t*& stats, size_t* total) {
+	const int tiles = grid_x * grid_y;
+	Carver c(base);
+	ImgView v{};
+	v.ranges = c.take<uint2>(tiles);
+	v.tile_count = c.take<uint32_t>(tiles);
+	v.totals = c.take<uint32_t>(2);
+	v.chunk_base = c.take<uint32_t>(tiles);
+	v.tile_diff = c.take<int>((size_t)(grid_x + 1) * (grid_y + 1));
+	stats = c.take<uint32_t>((size_t)3 * grid_y);
+	if (total) *total = c.size();
+	return v;
+}
+
 // Height of the [C,Hs,W] maps: the whole image, or with compact_slab only the pixel rows of tile rows [row_begin, row_end).
 static int slab_height(const rgs_camera* cam, int row_begin, int row_end) {
 	if (!cam->compact_slab) return cam->height;
@@ -191,6 +207,19 @@ static uint32_t* pinned_mailbox() {
 	return box;
 }
 
+// pinned per-thread mailbox of the balanced forward's per-row read-back, grown on demand
+static uint32_t* pinned_row_stats(size_t words) {
+	static thread_local uint32_t* box = nullptr;
+	static thread_local size_t capacity = 0;
+	if (words > capacity) {
+		if (box) cudaFreeHost(box);
+		capacity = 0;
+		if (cudaHostAlloc((void**)&box, words * sizeof(uint32_t), cudaHostAllocDefault) != cudaSuccess) return box = nullptr;
+		capacity = words;
+	}
+	return box;
+}
+
 }  // namespace rgs
 
 using namespace rgs;
@@ -213,44 +242,43 @@ int32_t rgs_stage_times(const char** names, double* total_ms, int64_t* launches,
 }
 int32_t rgs_grad_stride(int32_t require_coord, int32_t /*require_depth*/) { return grad_floats(require_coord != 0); }
 
-// preprocess -> tile counts -> (one host sync for the instance count) -> binning / sort: everything before blending.
-// Shared by rgs_forward and rgs_integrate.  Returns num_rendered or a negative status.
-static int64_t forward_to_binning(const rgs_camera* cam, const FwdParams& p, int* radii, const rgs_buffers* bufs, cudaStream_t s, GeomView& g,
-                                  BinView& b, ImgView& img) {
-	int rc;
-	const int P = p.P;
-	const size_t N = (size_t)p.W * p.Hs;
-	const int tiles = p.grid_x * p.grid_y;
+static int carve_geom_buffer(const FwdParams& p, const rgs_buffers* bufs, GeomView& g) {
+	size_t geom_bytes = 0;
+	carve_geom(nullptr, p.P, p.coord, &geom_bytes);
+	char* geom_ptr;
+	const int rc = grow(bufs->geom, bufs->geom_user, geom_bytes, geom_ptr, "geometry buffer");
+	if (rc == RGS_OK) g = carve_geom(geom_ptr, p.P, p.coord, nullptr);
+	return rc;
+}
 
+// image-side scratch (carved for maps of N pixels) and the geometry buffer
+static int carve_forward(const FwdParams& p, size_t N, const rgs_buffers* bufs, GeomView& g, ImgView& img) {
+	int rc;
+	char* img_ptr;
 	// image-side scratch first: needed even when there is nothing to draw (background fill)
 	size_t img_bytes = 0;
 	carve_img(nullptr, p.grid_x, p.grid_y, N, p.coord, p.depth, &img_bytes);
-	char* img_ptr;
 	if ((rc = grow(bufs->image, bufs->image_user, img_bytes, img_ptr, "image buffer")) != RGS_OK) return rc;
 	img = carve_img(img_ptr, p.grid_x, p.grid_y, N, p.coord, p.depth, nullptr);
+	return carve_geom_buffer(p, bufs, g);
+}
 
-	size_t geom_bytes = 0;
-	carve_geom(nullptr, P, p.coord, &geom_bytes);
-	char* geom_ptr;
-	if ((rc = grow(bufs->geom, bufs->geom_user, geom_bytes, geom_ptr, "geometry buffer")) != RGS_OK) return rc;
-	g = carve_geom(geom_ptr, P, p.coord, nullptr);
+// preprocess -> per-tile counts, ranges and totals of p's tile rows (P > 0)
+static int preprocess_and_scan(const rgs_camera* cam, const FwdParams& p, int* radii, GeomView g, ImgView img, cudaStream_t s) {
+	int rc;
+	RGS_CUDA_TRY(cudaMemsetAsync(img.tile_diff, 0, (size_t)(p.grid_x + 1) * (p.grid_y + 1) * sizeof(int), s));
+	{ StageScope sc(ST_PREPROCESS, s); launch_preprocess_forward(p, g, radii, img.tile_diff, s); }
+	if ((rc = debug_sync(cam, s, "preprocess")) != RGS_OK) return rc;
+	{ StageScope sc(ST_SCAN, s); launch_tile_scan(p, img, s); }
+	return RGS_OK;
+}
 
-	int64_t R = 0;
-	uint32_t max_list = 0;
-	if (P > 0) {
-		RGS_CUDA_TRY(cudaMemsetAsync(img.tile_diff, 0, (size_t)(p.grid_x + 1) * (p.grid_y + 1) * sizeof(int), s));
-		{ StageScope sc(ST_PREPROCESS, s); launch_preprocess_forward(p, g, radii, img.tile_diff, s); }
-		if ((rc = debug_sync(cam, s, "preprocess")) != RGS_OK) return rc;
-		{ StageScope sc(ST_SCAN, s); launch_tile_scan(p, img, s); }
-		// the one host sync of the forward pass: the instance count sizes the binning buffers and is returned to the
-		// caller (reference: blocking cudaMemcpy, rasterizer_impl.cu:354); the longest tile list picks the sort path
-		uint32_t* box = pinned_mailbox();
-		if (!box) return fail(RGS_E_CUDA, "cudaHostAlloc failed for the num_rendered mailbox");
-		RGS_CUDA_TRY(cudaMemcpyAsync(box, img.totals, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-		RGS_CUDA_TRY(cudaStreamSynchronize(s));
-		R = (int64_t)box[0];
-		max_list = box[1];
-	}
+// binning buffer for R instances -> scatter and per-tile sort of p's tile rows
+static int64_t bin_tiles(const rgs_camera* cam, const FwdParams& p, int* radii, const rgs_buffers* bufs, cudaStream_t s, GeomView g, BinView& b,
+                         ImgView img, int64_t R, uint32_t max_list) {
+	int rc;
+	const int P = p.P;
+	const int tiles = p.grid_x * p.grid_y;
 	size_t bin_bytes = 0;
 	carve_bin(nullptr, (size_t)R, tiles, &bin_bytes);
 	char* bin_ptr;
@@ -272,6 +300,29 @@ static int64_t forward_to_binning(const rgs_camera* cam, const FwdParams& p, int
 	return R;
 }
 
+// preprocess -> tile counts -> (one host sync for the instance count) -> binning / sort: everything before blending.
+// Shared by rgs_forward and rgs_integrate.  Returns num_rendered or a negative status.
+static int64_t forward_to_binning(const rgs_camera* cam, const FwdParams& p, int* radii, const rgs_buffers* bufs, cudaStream_t s, GeomView& g,
+                                  BinView& b, ImgView& img) {
+	int rc;
+	if ((rc = carve_forward(p, (size_t)p.W * p.Hs, bufs, g, img)) != RGS_OK) return rc;
+
+	int64_t R = 0;
+	uint32_t max_list = 0;
+	if (p.P > 0) {
+		if ((rc = preprocess_and_scan(cam, p, radii, g, img, s)) != RGS_OK) return rc;
+		// the one host sync of the forward pass: the instance count sizes the binning buffers and is returned to the
+		// caller (reference: blocking cudaMemcpy, rasterizer_impl.cu:354); the longest tile list picks the sort path
+		uint32_t* box = pinned_mailbox();
+		if (!box) return fail(RGS_E_CUDA, "cudaHostAlloc failed for the num_rendered mailbox");
+		RGS_CUDA_TRY(cudaMemcpyAsync(box, img.totals, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+		RGS_CUDA_TRY(cudaStreamSynchronize(s));
+		R = (int64_t)box[0];
+		max_list = box[1];
+	}
+	return bin_tiles(cam, p, radii, bufs, s, g, b, img, R, max_list);
+}
+
 int64_t rgs_forward(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_forward_out* out, const rgs_buffers* bufs, void* cuda_stream) {
 	FwdParams p;
 	int rc = make_params(cam, gs, p);
@@ -286,6 +337,80 @@ int64_t rgs_forward(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_fo
 	RenderOut ro{out->out_color, out->out_coord, out->out_mcoord, out->out_alpha, out->out_normal, out->out_depth, out->out_mdepth};
 	{ StageScope sc(ST_RENDER_FWD, s); launch_render_forward(p, g, b, img, ro, s); }
 	if ((rc = debug_sync(cam, s, "render")) != RGS_OK) return rc;
+	return R;
+}
+
+int64_t rgs_forward_balanced(const rgs_camera* cam, const rgs_gaussians* gs, int32_t world_size, int32_t rank, rgs_forward_out* out, rgs_maps_fn maps,
+                             void* maps_user, const rgs_buffers* bufs, int32_t* row_cuts, uint32_t* row_stats, void* cuda_stream) {
+	if (!cam) return fail(RGS_E_INVALID, "null camera / gaussians");
+	rgs_camera whole = *cam;
+	whole.tile_row_begin = 0;
+	whole.tile_row_end = -1;
+	FwdParams p;
+	int rc = make_params(&whole, gs, p);
+	if (rc != RGS_OK) return rc;
+	if (!out || !maps || !row_cuts || !bufs || !bufs->geom || !bufs->binning || !bufs->image)
+		return fail(RGS_E_INVALID, "null outputs / callbacks / row_cuts");
+	if (world_size <= 0 || rank < 0 || rank >= world_size) return fail(RGS_E_INVALID, "balanced forward: rank / world_size out of range");
+	cudaStream_t s = (cudaStream_t)cuda_stream;
+	const int gy = p.grid_y;
+	GeomView g;
+	if ((rc = carve_geom_buffer(p, bufs, g)) != RGS_OK) return rc;
+	// the whole image's tile counts live in the binning buffer until the slab is known: the image buffer is then carved for the
+	// slab's maps only, as a fixed-slab call carves it, and the binning buffer is grown for the slab's instances after the
+	// restriction has read them
+	size_t count_bytes = 0;
+	uint32_t* d_stats = nullptr;
+	carve_counts(nullptr, p.grid_x, gy, d_stats, &count_bytes);
+	char* count_ptr;
+	if ((rc = grow(bufs->binning, bufs->binning_user, count_bytes, count_ptr, "binning buffer")) != RGS_OK) return rc;
+	const ImgView counts = carve_counts(count_ptr, p.grid_x, gy, d_stats, nullptr);
+	std::vector<uint32_t> stats((size_t)3 * gy, 0u);  // I_y, L_y, 32-instance chunks per row
+	if (p.P > 0) {
+		if ((rc = preprocess_and_scan(&whole, p, out->radii, g, counts, s)) != RGS_OK) return rc;
+		{ StageScope sc(ST_SCAN, s); launch_row_stats(p, counts, d_stats, s); }
+		// the one host sync of the balanced forward: the per-row counts choose the slab, size its binning buffers and give num_rendered
+		uint32_t* box = pinned_row_stats(stats.size());
+		if (!box) return fail(RGS_E_CUDA, "cudaHostAlloc failed for the row-stats mailbox");
+		RGS_CUDA_TRY(cudaMemcpyAsync(box, d_stats, stats.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+		RGS_CUDA_TRY(cudaStreamSynchronize(s));
+		std::memcpy(stats.data(), box, stats.size() * sizeof(uint32_t));
+	}
+	if ((rc = rgs_balance_partition(gy, p.grid_x, world_size, stats.data(), row_cuts)) != RGS_OK) return rc;
+	if (row_stats) std::memcpy(row_stats, stats.data(), (size_t)2 * gy * sizeof(uint32_t));
+
+	rgs_camera slab = *cam;
+	slab.tile_row_begin = row_cuts[rank];
+	slab.tile_row_end = row_cuts[rank + 1];
+	FwdParams ps;
+	if ((rc = make_params(&slab, gs, ps)) != RGS_OK) return rc;
+	SlabShift sh{0u, 0u, 0u, 0u, 0u};
+	for (int y = 0; y < gy; y++) {
+		if (y < ps.row_begin) {
+			sh.range_off += stats[y];
+			sh.chunk_off += stats[2 * gy + y];
+		} else if (y < ps.row_end) {
+			sh.rendered += stats[y];
+			sh.longest = stats[gy + y] > sh.longest ? stats[gy + y] : sh.longest;
+			sh.chunk_total += stats[2 * gy + y];
+		}
+	}
+	size_t img_bytes = 0;
+	carve_img(nullptr, ps.grid_x, ps.grid_y, (size_t)ps.W * ps.Hs, ps.coord, ps.depth, &img_bytes);
+	char* img_ptr;
+	if ((rc = grow(bufs->image, bufs->image_user, img_bytes, img_ptr, "image buffer")) != RGS_OK) return rc;
+	const ImgView img = carve_img(img_ptr, ps.grid_x, ps.grid_y, (size_t)ps.W * ps.Hs, ps.coord, ps.depth, nullptr);
+	if (p.P > 0) {
+		StageScope sc(ST_SCAN, s);
+		launch_slab_restrict(ps, g, counts, img, out->radii, sh, s);
+	}
+	if (maps(maps_user, ps.row_begin, ps.row_end, ps.Hs, out) != 0) return fail(RGS_E_ALLOC, "maps callback failed");
+	BinView b;
+	const int64_t R = bin_tiles(&slab, ps, out->radii, bufs, s, g, b, img, (int64_t)sh.rendered, sh.longest);
+	if (R < 0) return R;
+	RenderOut ro{out->out_color, out->out_coord, out->out_mcoord, out->out_alpha, out->out_normal, out->out_depth, out->out_mdepth};
+	{ StageScope sc(ST_RENDER_FWD, s); launch_render_forward(ps, g, b, img, ro, s); }
+	if ((rc = debug_sync(&slab, s, "render")) != RGS_OK) return rc;
 	return R;
 }
 

@@ -263,6 +263,18 @@ constexpr int TILE_SORT_CAP = 8192;   // longest tile list the one-CTA shared-me
 void launch_tile_scan(const FwdParams& p, ImgView img, cudaStream_t s);
 void launch_tile_binning(const FwdParams& p, GeomView g, BinView b, ImgView img, const int* radii, int64_t R, uint32_t max_list, cudaStream_t s);
 
+// balanced row sharding (rgs_balance.cu): per-row instances / longest list / 32-instance chunks of a whole-image scan, then
+// that scan's state (`whole`) restricted to one slab, written into the slab's image buffer (`img`)
+void launch_row_stats(const FwdParams& p, ImgView img, uint32_t* stats, cudaStream_t s);
+struct SlabShift {
+	uint32_t range_off;    // instances in the rows above the slab
+	uint32_t chunk_off;    // 32-instance chunks in the rows above the slab
+	uint32_t chunk_total;  // 32-instance chunks in the slab
+	uint32_t rendered;     // instances in the slab
+	uint32_t longest;      // longest tile list in the slab
+};
+void launch_slab_restrict(const FwdParams& slab, GeomView g, ImgView whole, ImgView img, const int* radii, const SlabShift& sh, cudaStream_t s);
+
 struct RenderOut {
 	float *color, *coord, *mcoord, *alpha, *normal, *depth, *mdepth;
 };

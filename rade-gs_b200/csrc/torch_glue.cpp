@@ -230,6 +230,104 @@ FwdResult forward_impl(const torch::Tensor& background, const torch::Tensor& mea
 	                       binningBuffer, imgBuffer);
 }
 
+// ---- balanced row sharding: the slab is cut from the frame's own tile counts (rgs_forward_balanced) ----------------
+
+// the seven maps, allocated once the library has chosen the slab (its rgs_maps_fn)
+struct BalancedMaps {
+	torch::TensorOptions opts;
+	int W, grid_y;
+	bool compact;
+	torch::Tensor color, coord, mcoord, alpha, normal, depth, mdepth;
+
+	void make(int row_begin, int row_end, int height, bool zero) {
+		// full-size maps of a slab that is not the whole image: the rows outside it stay zero, as rasterize_gaussians_slab returns them
+		const bool fill = zero || (!compact && !(row_begin == 0 && row_end == grid_y));
+		auto img = [&](int ch) { return fill ? torch::zeros({ch, height, W}, opts) : new_empty({ch, height, W}, opts); };
+		color = img(3), coord = img(3), mcoord = img(3), alpha = img(1), normal = img(3), depth = img(1), mdepth = img(1);
+	}
+};
+
+int32_t balanced_maps_cb(void* user, int32_t row_begin, int32_t row_end, int32_t height, rgs_forward_out* out) {
+	auto* m = reinterpret_cast<BalancedMaps*>(user);
+	try {
+		m->make(row_begin, row_end, height, false);
+	} catch (const std::exception&) {
+		return 1;
+	}
+	out->out_color = m->color.data_ptr<float>();
+	out->out_coord = m->coord.data_ptr<float>();
+	out->out_mcoord = m->mcoord.data_ptr<float>();
+	out->out_alpha = m->alpha.data_ptr<float>();
+	out->out_normal = m->normal.data_ptr<float>();
+	out->out_depth = m->depth.data_ptr<float>();
+	out->out_mdepth = m->mdepth.data_ptr<float>();
+	return 0;
+}
+
+// rasterize_gaussians_slab's 12-tuple for the slab the frame's tile counts give rank `rank` of `world_size`, then the partition
+// (world_size + 1 tile-row cuts) and the per-row statistics [2, grid_y] (instances, longest tile list) on the host
+py::tuple RasterizeBalanced(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
+                            const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
+                            const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                            const float kernel_size, const int image_height, const int image_width, const torch::Tensor& sh, const int degree,
+                            const torch::Tensor& campos, const bool prefiltered, const bool require_coord, const bool require_depth, const bool debug,
+                            const int world_size, const int rank, const bool compact) {
+	if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
+		AT_ERROR("means3D must have dimensions (num_points, 3)");
+	}
+	const auto guard = cuda_guard(means3D);
+	const int P = means3D.size(0);
+	const int H = image_height, W = image_width;
+	const int grid_x = (W + 15) / 16, grid_y = (H + 15) / 16;
+	TORCH_CHECK(world_size > 0 && rank >= 0 && rank < world_size, "rank ", rank, " is not a rank of ", world_size);
+	TORCH_CHECK(H > 0 && W > 0, "image size must be positive");
+	BalancedMaps m{means3D.options().dtype(torch::kFloat32), W, grid_y, compact};
+	torch::Tensor radii = P == 0 ? torch::zeros({P}, means3D.options().dtype(torch::kInt32)) : new_empty({P}, means3D.options().dtype(torch::kInt32));
+	torch::Tensor geomBuffer = bytes(means3D), binningBuffer = bytes(means3D), imgBuffer = bytes(means3D);
+	std::vector<int32_t> cuts(world_size + 1);
+	torch::Tensor stats = torch::zeros({2, grid_y}, torch::dtype(torch::kInt64));
+	std::vector<uint32_t> row_stats((size_t)2 * grid_y, 0u);
+	int rendered = 0;
+	if (P == 0) {  // nothing to render: the partition of empty rows and all-zero maps, as rasterize_gaussians_slab returns them
+		check(rgs_balance_partition(grid_y, grid_x, world_size, row_stats.data(), cuts.data()));
+		const int r0 = cuts[rank], r1 = cuts[rank + 1];
+		m.make(r0, r1, compact ? std::max(0, std::min(r1 * 16, H) - r0 * 16) : H, true);
+	} else {
+		CamHolder ch;
+		fill_camera(ch, means3D, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, kernel_size, scale_modifier, H, W, degree, sh_coeffs(sh),
+		            prefiltered, require_coord, require_depth, debug, 0, -1, compact);
+		GaussHolder gh;
+		fill_gaussians(gh, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp);
+		rgs_forward_out fo{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, radii.data_ptr<int>()};
+		rgs_buffers bufs{resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer};
+		const int64_t rc = rgs_forward_balanced(&ch.cam, &gh.g, world_size, rank, &fo, balanced_maps_cb, &m, &bufs, cuts.data(), row_stats.data(),
+		                                        at::cuda::getCurrentCUDAStream().stream());
+		check(rc);
+		rendered = (int)rc;
+		auto acc = stats.accessor<int64_t, 2>();
+		for (int y = 0; y < grid_y; y++) {
+			acc[0][y] = row_stats[y];
+			acc[1][y] = row_stats[grid_y + y];
+		}
+	}
+	py::list py_cuts;
+	for (int32_t c : cuts) py_cuts.append(c);
+	return py::make_tuple(rendered, m.color, m.coord, m.mcoord, m.alpha, m.normal, m.depth, m.mdepth, radii, geomBuffer, binningBuffer, imgBuffer, py_cuts,
+	                      stats);
+}
+
+// the library's partition of `row_instances` (one count per tile row) over `world_size` ranks: world_size + 1 tile-row cuts
+std::vector<int32_t> BalancePartition(const std::vector<int64_t>& row_instances, const int grid_x, const int world_size) {
+	std::vector<uint32_t> rows(row_instances.size());
+	for (size_t y = 0; y < rows.size(); y++) {
+		TORCH_CHECK(row_instances[y] >= 0 && row_instances[y] <= (int64_t)UINT32_MAX, "row instance counts must fit in 32 bits");
+		rows[y] = (uint32_t)row_instances[y];
+	}
+	std::vector<int32_t> cuts(std::max(world_size, 0) + 1);
+	check(rgs_balance_partition((int32_t)rows.size(), grid_x, world_size, rows.data(), cuts.data()));
+	return cuts;
+}
+
 // ---- the reference's four symbols ------------------------------------------------------------------------------
 
 FwdResult RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
@@ -1804,6 +1902,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	sl.def("normal_consistency_rows", &NormalConsistencyRows, py::arg("rendered_normal"), py::arg("map_expected"), py::arg("map_median"),
 	       py::arg("from_depth"), py::arg("inv_fx"), py::arg("inv_fy"), py::arg("cx"), py::arg("cy"), py::arg("w_expected"), py::arg("w_median"), py::arg("H"),
 	       py::arg("row_lo"), py::arg("row_hi"));
+	sl.def("rasterize_balanced", &RasterizeBalanced, py::arg("background"), py::arg("means3D"), py::arg("colors"), py::arg("opacity"), py::arg("scales"),
+	       py::arg("rotations"), py::arg("scale_modifier"), py::arg("cov3D_precomp"), py::arg("viewmatrix"), py::arg("projmatrix"), py::arg("tan_fovx"),
+	       py::arg("tan_fovy"), py::arg("kernel_size"), py::arg("image_height"), py::arg("image_width"), py::arg("sh"), py::arg("degree"), py::arg("campos"),
+	       py::arg("prefiltered"), py::arg("require_coord"), py::arg("require_depth"), py::arg("debug"), py::arg("world_size"), py::arg("rank"),
+	       py::arg("compact") = false);
+	sl.def("balance_partition", &BalancePartition, py::arg("row_instances"), py::arg("grid_x"), py::arg("world_size"));
+	sl.attr("BALANCE_TILE_COST") = RGS_BALANCE_TILE_COST;
 	sl.def("appearance_row_windows", &AppearanceRowWindows, py::arg("H0"), py::arg("W0"), py::arg("row_lo"), py::arg("row_hi"));
 	sl.def("appearance_downsample_rows", &AppearanceDownsampleRows, py::arg("image"), py::arg("image_lo"), py::arg("H0"), py::arg("row_lo"),
 	       py::arg("row_hi"));

@@ -189,11 +189,20 @@ class _ShardedRasterize(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, slab, group, exchange=None,
-                compact=False):
+                compact=False, balance=None):
         from diff_gaussian_rasterization import _C, _forward_args
         s = raster_settings
         args = _forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh)
-        num_rendered, color, coord, mcoord, alpha, normal, depth, mdepth, radii, geom, binning, img = _C.rasterize_gaussians_slab(*args, *slab, compact)
+        if balance is not None:   # (rank, world_size, plan): the slab is cut from this frame's tile counts and reported in `plan`
+            rank, world_size, plan = balance
+            out = _C._slab.rasterize_balanced(*args, world_size, rank, compact)
+            cuts, plan["row_stats"] = out[12], out[13]
+            plan["slabs"] = [(cuts[r], cuts[r + 1]) for r in range(world_size)]
+            slab = plan["slabs"][rank]
+            out = out[:12]
+        else:
+            out = _C.rasterize_gaussians_slab(*args, *slab, compact)
+        num_rendered, color, coord, mcoord, alpha, normal, depth, mdepth, radii, geom, binning, img = out
         ctx.s, ctx.slab, ctx.compact, ctx.group, ctx.num_rendered, ctx.exchange = s, slab, compact, group, num_rendered, exchange
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, normal, radii, sh, geom, binning, img, alpha, opacities)
         return color, radii, coord, mcoord, depth, mdepth, alpha, normal
@@ -217,7 +226,7 @@ class _ShardedRasterize(torch.autograd.Function):
         acc = (ctx.exchange.backward_render(_C, *stage1_args) if ctx.exchange is not None
                else allreduce_sum_(_C.rasterize_gaussians_backward_render(*stage1_args), ctx.group))
         g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot = stage2(acc)
-        return g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, None, None, None, None, None
+        return g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, None, None, None, None, None, None
 
 
 class _GatherSlabs(torch.autograd.Function):
@@ -253,11 +262,19 @@ class ShardedGaussianRasterizer(torch.nn.Module):
     Each rank returns full-size maps of which only its slab rows are filled (the rest is zero) or, with ``compact=True``, maps
     that hold only the slab's pixel rows ([C, rows, W]); callers that need the whole image gather the slabs (`gather_image`).  Gradients returned on every rank are the full,
     already-reduced parameter gradients.
+
+    ``balance=True`` cuts the slabs anew in every forward call from that frame's instances per tile row (include/rgs_b200.h's
+    partition rule; every rank derives the same partition without communicating).  After a forward, `slabs`, `slab`,
+    `pixel_rows()` and `all_pixel_rows()` describe that frame, `row_stats` holds its [2, tile rows] instances and longest tile
+    list per row, and `gather_image` uses its partition; the backward of a frame uses the slab chosen at its forward.  Every slab
+    holds at least one tile row, so the image needs at least `world_size` tile rows.  Cannot be combined with ``row_weights``.
     """
 
     def __init__(self, raster_settings, rank: int | None = None, world_size: int | None = None, group=None, row_weights=None,
-                 exchange: GradExchange | None = None, compact: bool = False):
+                 exchange: GradExchange | None = None, compact: bool = False, balance: bool = False):
         super().__init__()
+        if balance and row_weights is not None:
+            raise ValueError("balance=True cuts the slabs from each frame's tile counts: it cannot be combined with row_weights")
         self.compact = compact     # True: the returned maps are [C, slab rows, W] (per-rank image memory and fill scale with 1/ranks)
         self.raster_settings = raster_settings
         self.group = group
@@ -267,18 +284,34 @@ class ShardedGaussianRasterizer(torch.nn.Module):
         if rank is None:
             rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.rank, self.world_size = rank, world_size
-        self.slabs = partition_tile_rows(tile_rows(raster_settings.image_height), world_size, row_weights)
+        self.balance = bool(balance)
+        grid_y = tile_rows(raster_settings.image_height)
+        if self.balance and grid_y < world_size:
+            raise ValueError(f"balance=True gives every rank at least one tile row: {grid_y} tile rows cannot serve {world_size} ranks")
+        self.slabs = partition_tile_rows(grid_y, world_size, row_weights)   # with balance: until the first forward
         self.slab = self.slabs[rank]
+        self.row_stats = None
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None):
         from diff_gaussian_rasterization import _inputs
         shs, colors_precomp, scales, rotations, cov3D_precomp = _inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        return _ShardedRasterize.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                       self.raster_settings, self.slab, self.group, self.exchange, self.compact)
+        plan = {}
+        out = _ShardedRasterize.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
+                                      self.raster_settings, self.slab, self.group, self.exchange, self.compact,
+                                      (self.rank, self.world_size, plan) if self.balance else None)
+        if self.balance:
+            self.slabs, self.row_stats = plan["slabs"], plan["row_stats"]
+            self.slab = self.slabs[self.rank]
+        return out
 
     def pixel_rows(self) -> Tuple[int, int]:
         H = self.raster_settings.image_height
         return min(self.slab[0] * TILE, H), min(self.slab[1] * TILE, H)
+
+    def all_pixel_rows(self) -> List[Tuple[int, int]]:
+        """Every rank's pixel rows, in rank order: the `all_pixel_rows` argument of the slab losses."""
+        H = self.raster_settings.image_height
+        return [(min(b * TILE, H), min(e * TILE, H)) for b, e in self.slabs]
 
     def gather_image(self, img: torch.Tensor) -> torch.Tensor:
         """The whole [C,H,W] map from the ranks' slabs (all-gather of the slab rows; rows outside a rank's slab are zero locally).
@@ -288,7 +321,7 @@ class ShardedGaussianRasterizer(torch.nn.Module):
         rasterizer's backward reads only the rows of its own slab, so nothing is counted twice.
         """
         H = self.raster_settings.image_height
-        rows = [(min(b * TILE, H), min(e * TILE, H)) for b, e in self.slabs]
+        rows = self.all_pixel_rows()
         if self.compact:   # [C, slab rows, W] -> place into a full-size map first (the gather copies slab rows only)
             full = img.new_zeros(img.shape[0], H, img.shape[2])
             r0, r1 = rows[self.rank]
@@ -371,18 +404,27 @@ def _cuda_slab_bwd(img, gt, state, w_ssim, w_l1, r0, r1):
     return _C.ssim_l1_backward(img, gt, state[0], w_ssim, w_l1, torch.empty(0), r0, r1)
 
 
+def _check_ssim_rows(pixel_rows, H, world_size):
+    """Raise unless this rank's rows suit slab_l1_ssim_loss's 5-row halo exchange (its docstring states the rule)."""
+    r0, r1 = int(pixel_rows[0]), int(pixel_rows[1])
+    if world_size > 1 and r1 - r0 < HALO and not r0 < r1 == H:
+        raise ValueError("slab-local SSIM needs at least 5 pixel rows on every slab that does not end at the image's last row (a shorter "
+                         "slab breaks the neighbour halo exchange)")
+
+
 def slab_l1_ssim_loss(image: torch.Tensor, gt: torch.Tensor, lambda_dssim: float, pixel_rows: Tuple[int, int], rank: int | None = None,
                       world_size: int | None = None, group=None, kernels=None) -> torch.Tensor:
     """train.py:163's `(1 - l) * l1_loss(image, gt) + l * (1 - ssim(image, gt))` for a row-sharded render: `image` [3,H,W] holds this
     rank's slab rows `pixel_rows` (`ShardedGaussianRasterizer.pixel_rows()`), `gt` the ground truth (at least those rows +- 5).
     Returns the full-image loss (the same value on every rank); its gradient w.r.t. `image` is non-zero in this rank's rows only and
-    already contains the neighbours' contributions.  Slabs must be at least 5 rows tall (they are multiples of 16)."""
+    already contains the neighbours' contributions.  Every slab that does not end at the image's last row must be at least 5 rows
+    tall; a non-empty slab that ends there may be shorter (the halo its neighbour above needs ends at the image's edge too), as the
+    last tile row of an image whose height is not a multiple of 16 is."""
     if world_size is None:
         world_size = dist.get_world_size(group) if dist.is_initialized() else 1
     if rank is None:
         rank = dist.get_rank(group) if dist.is_initialized() else 0
-    if world_size > 1 and pixel_rows[1] - pixel_rows[0] < HALO:
-        raise ValueError("slab-local SSIM needs slabs of at least 5 pixel rows on every rank (a shorter slab breaks the neighbour halo exchange)")
+    _check_ssim_rows(pixel_rows, image.shape[-2], world_size)
     fwd, bwd = kernels if kernels is not None else (_cuda_slab_fwd, _cuda_slab_bwd)
     return _SlabSsimL1.apply(image, gt, float(lambda_dssim), (int(pixel_rows[0]), int(pixel_rows[1])), rank, world_size, group, fwd, bwd)
 
