@@ -317,8 +317,8 @@ int32_t rgs_normal_consistency_rows(int32_t H, int32_t W, int32_t row_lo, int32_
 
 /* ---- decoupled-appearance L1 loss (train.py:37-58 with GOF's AppearanceNetwork, scene/appearance_network.py) ----
  * The image is planar fp32 [3, H0, W0], H0, W0 >= 32.  The crop is H = H0 / 32 * 32 rows by W = W0 / 32 * 32 columns at
- * top = H0 / 2 - H / 2, left = W0 / 2 - W / 2.  The network's head (conv1, up1..up4) is the caller's; these functions run the
- * rest.  up4 is the head's output [16, H/2, W/2].  w2 [16,16,3,3], b2 [16], w3 [3,16,3,3], b3 [3] are conv2 and conv3.  All
+ * top = H0 / 2 - H / 2, left = W0 / 2 - W / 2.  The network's head (conv1, up1..up4) is rgs_appearance_head_* below; these
+ * functions run the rest.  up4 is the head's output [16, H/2, W/2].  w2 [16,16,3,3], b2 [16], w3 [3,16,3,3], b3 [3] are conv2 and conv3.  All
  * arithmetic is fp32 (FFMA, no tensor cores); sums are fixed-order, so every output is bit-reproducible from run to run.
  *
  * rgs_appearance_downsample: down [3, H/32, W/32] = bilinear, align_corners=True, of the crop.  Source index = s * dst in fp32
@@ -391,6 +391,37 @@ int32_t rgs_appearance_l1_backward_rows(int32_t H0, int32_t W0, int32_t row_lo, 
                                         int32_t image_rows, const float* up4, const float* act, const float* w2, const float* w3, const float* b3,
                                         const float* upstream, float* d_image, float* d_up4, double* grad_row, double* partials, float* d_x,
                                         void* cuda_stream);
+/* The network's head (added functions, ABI 4): conv1 (67 -> 256) + ReLU, then up1..up4, each PixelShuffle(2) (torch's rule
+ * out[c][2y+i][2x+j] = in[4c+2i+j][y][x]), a 3x3 convolution (64 -> 128, 32 -> 64, 16 -> 32, 8 -> 16) and a ReLU, every
+ * convolution with zero padding at its own map's border.  h = H/32, w = W/32 >= 1 (h w <= 2^18).  conv1's input is down
+ * [3, h, w] (rgs_appearance_downsample's output) followed by the 64-float embedding row on every pixel, zero in the padding ring
+ * as in the concatenated input; neither it nor any shuffled map is materialised.  The ten parameters have torch's layouts:
+ * w1 [256,67,3,3], b1 [256], wu1 [128,64,3,3], bu1 [128], wu2 [64,32,3,3], bu2 [64], wu3 [32,16,3,3], bu3 [32], wu4 [16,8,3,3],
+ * bu4 [16].  All arithmetic is fp32 FFMA (no tensor cores, no TF32), every sum has a fixed order and there are no float atomics:
+ * every output is bit-reproducible from run to run, whatever torch's cuDNN and TF32 settings.
+ *
+ * rgs_appearance_head_forward: act [RGS_APPEARANCE_HEAD_ACT_PER_HW h w] receives the post-ReLU outputs of conv1 [256, h, w],
+ *   up1 [128, 2h, 2w], up2 [64, 4h, 4w] and up3 [32, 8h, 8w], back to back; up4 [16, 16h, 16w] the head's output.
+ * rgs_appearance_head_backward: from d_up4 [16, 16h, 16w] (rgs_appearance_l1_backward's) and forward's act and up4: each layer's
+ *   ReLU mask (output > 0), the data gradient (the flipped-weight convolution, then the inverse shuffle) and the weight and
+ *   bias gradients.  d_down [3, h, w] is conv1's input gradient on the image channels (for rgs_appearance_downsample_backward);
+ *   d_emb [64] is its sum over every pixel on channels 3..66: fp32 over pixels t, t + 256, ... for each of 256 partial sums,
+ *   which are added in order in fp64, one cast.  d_w*, d_b* have the parameters' layouts: each layer's map is cut into tiles of
+ *   4 x 32 pixels (up4: 8 x 32) and the tiles, in row-major order, into bands; within a band each weight's and each bias's sum
+ *   runs in fp32 over the tiles in order, within a tile over rows g, g + G, ... for each of G pixel groups (G = 1 for conv1..up2,
+ *   2 for up3, 8 for up4) and over the columns in order, the groups added in group order; the bands are added in band order in
+ *   fp64, one cast.  scratch: rgs_appearance_head_scratch_bytes.
+ * rgs_appearance_head_scratch_bytes: the backward's scratch for an h x w head input (host only): the fp64 band rows (at most
+ *   16 MB) plus 3072 h w floats, 37.6 MB at h, w = 37, 50 (1600 x 1200). */
+#define RGS_APPEARANCE_HEAD_ACT_PER_HW 3840
+int32_t rgs_appearance_head_scratch_bytes(int32_t h, int32_t w, size_t* bytes);
+int32_t rgs_appearance_head_forward(int32_t h, int32_t w, const float* down, const float* emb, const float* w1, const float* b1, const float* wu1,
+                                    const float* bu1, const float* wu2, const float* bu2, const float* wu3, const float* bu3, const float* wu4,
+                                    const float* bu4, float* act, float* up4, void* cuda_stream);
+int32_t rgs_appearance_head_backward(int32_t h, int32_t w, const float* down, const float* emb, const float* w1, const float* wu1, const float* wu2,
+                                     const float* wu3, const float* wu4, const float* act, const float* up4, const float* d_up4, float* d_down,
+                                     float* d_emb, float* d_w1, float* d_b1, float* d_wu1, float* d_bu1, float* d_wu2, float* d_bu2, float* d_wu3,
+                                     float* d_bu3, float* d_wu4, float* d_bu4, void* scratch, void* cuda_stream);
 
 /* ---- initial Gaussian scales: simple_knn's distCUDA2 (reference scene/gaussian_model.py:20, :315-316) ----
  * points [P,3] (device, fp32) -> mean_dist2 [P] (device): the mean of the squared Euclidean distances from point i to its 3 nearest

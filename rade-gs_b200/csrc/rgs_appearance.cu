@@ -1,6 +1,6 @@
 // rgs_appearance.cu -- train.py:37-58 (L1_loss_appearance with GOF's AppearanceNetwork, scene/appearance_network.py), the
-// parts that run at the crop's resolution or touch the image.  The network's low-resolution head (conv1, up1..up4) stays on
-// cuDNN; everything else is here, in FP32 FFMA, without floating-point atomics:
+// parts that run at the crop's resolution or touch the image.  The network's low-resolution head (conv1, up1..up4) is in
+// rgs_appearance_head.cu; everything else is here, in FP32 FFMA, without floating-point atomics:
 //
 //   downsample          center crop (a multiple of 32 per axis) -> bilinear, align_corners=True, to H/32 x W/32
 //   downsample_backward adds each low-resolution sample's <= 4 taps into d_image; taps of different samples are disjoint

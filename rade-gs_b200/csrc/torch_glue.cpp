@@ -1020,6 +1020,75 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> AppearanceL1BackwardRows
 	return std::make_tuple(d_img, d_up4, grad_row);
 }
 
+// The network's head (rgs_appearance_head_*): down [3, h, w], the embedding row [64] and the ten head parameters in the
+// module's order (conv1.weight, conv1.bias, up1.conv.weight, ..., up4.conv.bias).
+struct AppearanceHeadArgs {
+	torch::Tensor down, emb;
+	std::vector<torch::Tensor> p;
+	int h, w;
+};
+
+AppearanceHeadArgs appearance_head_args(const torch::Tensor& down, const torch::Tensor& emb, const std::vector<torch::Tensor>& params) {
+	static const char* names[10] = {"conv1 weight", "conv1 bias", "up1 weight", "up1 bias", "up2 weight", "up2 bias", "up3 weight", "up3 bias", "up4 weight", "up4 bias"};
+	static const int64_t cin[5] = {67, 64, 32, 16, 8}, cout[5] = {256, 128, 64, 32, 16};
+	AppearanceHeadArgs a;
+	a.down = arg(down, "down", torch::kFloat32, {3, -1, -1}, "[3, h, w]");
+	a.h = (int)a.down.size(1);
+	a.w = (int)a.down.size(2);
+	a.emb = arg(emb, "embedding row", torch::kFloat32, {64}, "[64]", &a.down);
+	TORCH_CHECK(params.size() == 10, "appearance head: 10 parameters (conv1, up1..up4 weights and biases), got ", params.size());
+	for (int i = 0; i < 10; i++) {
+		const int l = i / 2;
+		if (i % 2 == 0) {
+			const std::string shape = "[" + std::to_string(cout[l]) + ", " + std::to_string(cin[l]) + ", 3, 3]";
+			a.p.push_back(arg(params[i], names[i], torch::kFloat32, {cout[l], cin[l], 3, 3}, shape.c_str(), &a.down));
+		} else {
+			const std::string shape = "[" + std::to_string(cout[l]) + "]";
+			a.p.push_back(arg(params[i], names[i], torch::kFloat32, {cout[l]}, shape.c_str(), &a.down));
+		}
+	}
+	return a;
+}
+
+const float* fp(const torch::Tensor& t) { return t.data_ptr<float>(); }
+
+// returns (act [3840 h w], up4 [1, 16, 16h, 16w])
+std::tuple<torch::Tensor, torch::Tensor> AppearanceHeadForward(const torch::Tensor& down, const torch::Tensor& emb, const std::vector<torch::Tensor>& params) {
+	const AppearanceHeadArgs a = appearance_head_args(down, emb, params);
+	const c10::cuda::CUDAGuard guard(a.down.device());
+	const auto o = a.down.options();
+	torch::Tensor act = new_empty({(int64_t)RGS_APPEARANCE_HEAD_ACT_PER_HW * a.h * a.w}, o), up4 = new_empty({1, 16, 16 * a.h, 16 * a.w}, o);
+	const auto& p = a.p;
+	check(rgs_appearance_head_forward(a.h, a.w, fp(a.down), fp(a.emb), fp(p[0]), fp(p[1]), fp(p[2]), fp(p[3]), fp(p[4]), fp(p[5]), fp(p[6]), fp(p[7]),
+	                                  fp(p[8]), fp(p[9]), act.data_ptr<float>(), up4.data_ptr<float>(), at::cuda::getCurrentCUDAStream().stream()));
+	return std::make_tuple(act, up4);
+}
+
+// returns [d_down [3, h, w], d_emb [64], the ten parameter gradients]
+std::vector<torch::Tensor> AppearanceHeadBackward(const torch::Tensor& down, const torch::Tensor& emb, const std::vector<torch::Tensor>& params,
+                                                  const torch::Tensor& act, const torch::Tensor& up4, const torch::Tensor& d_up4) {
+	const AppearanceHeadArgs a = appearance_head_args(down, emb, params);
+	const c10::cuda::CUDAGuard guard(a.down.device());
+	const int64_t h = a.h, w = a.w;
+	const torch::Tensor ac = arg(act, "head activations", torch::kFloat32, {RGS_APPEARANCE_HEAD_ACT_PER_HW * h * w}, "[3840 h w]", &a.down);
+	const torch::Tensor u = arg(up4, "up4 output", torch::kFloat32, {1, 16, 16 * h, 16 * w}, "[1, 16, 16h, 16w]", &a.down);
+	const torch::Tensor du = arg(d_up4, "d_up4", torch::kFloat32, {}, "", &a.down);
+	TORCH_CHECK(du.numel() == u.numel(), "d_up4 must have up4's ", u.numel(), " elements, got ", d_up4.sizes());
+	size_t bytes = 0;
+	check(rgs_appearance_head_scratch_bytes(a.h, a.w, &bytes));
+	const auto o = a.down.options();
+	torch::Tensor scratch = new_empty({(int64_t)bytes}, o.dtype(torch::kByte));
+	std::vector<torch::Tensor> out{new_empty({3, h, w}, o), new_empty({64}, o)};
+	for (const torch::Tensor& t : a.p) out.push_back(new_empty(t.sizes(), o));
+	float* g[12];
+	for (int i = 0; i < 12; i++) g[i] = out[i].data_ptr<float>();
+	const auto& p = a.p;
+	check(rgs_appearance_head_backward(a.h, a.w, fp(a.down), fp(a.emb), fp(p[0]), fp(p[2]), fp(p[4]), fp(p[6]), fp(p[8]), fp(ac), fp(u), fp(du), g[0], g[1],
+	                                   g[2], g[3], g[4], g[5], g[6], g[7], g[8], g[9], g[10], g[11], scratch.data_ptr(),
+	                                   at::cuda::getCurrentCUDAStream().stream()));
+	return out;
+}
+
 // ---- densify-and-prune and opacity reset (scene/gaussian_model.py:495-513, :662-741; rgs_densify_*, rgs_reset_opacity) ----------
 
 // a per-Gaussian input: float32 on `like`'s device with `width` floats per row over P rows
@@ -1918,6 +1987,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	       py::arg("row_hi"), py::arg("up4"), py::arg("w2"), py::arg("b2"), py::arg("w3"), py::arg("b3"));
 	sl.def("appearance_l1_backward_rows", &AppearanceL1BackwardRows, py::arg("image"), py::arg("gt"), py::arg("image_lo"), py::arg("H0"), py::arg("row_lo"),
 	       py::arg("row_hi"), py::arg("up4"), py::arg("act"), py::arg("w2"), py::arg("b2"), py::arg("w3"), py::arg("b3"), py::arg("upstream"));
+	// the decoupled-appearance network's head: a private submodule behind rade_gs_b200.appearance and multigpu
+	py::module_ ah = m.def_submodule("_appearance_head", "conv1 and up1..up4 of the appearance network behind rade_gs_b200.appearance");
+	ah.def("forward", &AppearanceHeadForward, py::arg("down"), py::arg("emb"), py::arg("params"));
+	ah.def("backward", &AppearanceHeadBackward, py::arg("down"), py::arg("emb"), py::arg("params"), py::arg("act"), py::arg("up4"), py::arg("d_up4"));
 	m.def("grad_stride",[](bool require_coord, bool require_depth) { return rgs_grad_stride(require_coord, require_depth); });
 	m.def("set_poison", [](int byte) { g_poison = byte; });
 	m.def("launch_count", []() { return rgs_launch_count(); });

@@ -5,9 +5,10 @@ the reference's function (train.py:37-58, from Gaussian Opacity Fields): center-
 it by 32, append the view's appearance embedding, run ``gaussians.appearance_network`` (scene/appearance_network.py) and take
 the L1 of ``mapping * crop`` against the ground truth's crop.
 
-The network's low-resolution head (conv1, relu, up1..up4) runs as the module's own layers on cuDNN.  The crop and downsample,
-the x2 upsample, conv2 + ReLU, conv3 + sigmoid and the loss run in csrc/rgs_appearance.cu, in FP32 without tensor cores, and
-their backward sums in a fixed order: two calls give identical bits, where torch's bilinear backward accumulates with atomics.
+The whole network and the loss run in the project's kernels, in FP32 without tensor cores: the crop and downsample, the x2
+upsample, conv2 + ReLU, conv3 + sigmoid and the loss in csrc/rgs_appearance.cu, the low-resolution head (conv1, relu, up1..up4)
+in csrc/rgs_appearance_head.cu.  Every backward sum has a fixed order and there are no float atomics: two calls give identical
+bits, whatever torch's cuDNN and TF32 settings, where torch's bilinear backward accumulates with atomics.
 Gradients reach the module's parameters, the embedding table row ``view_idx`` and the image, as autograd would deliver them.
 No CPU path: CUDA tensors only.
 """
@@ -21,18 +22,34 @@ from diff_gaussian_rasterization import _C
 __all__ = ["L1_loss_appearance"]
 
 
-def _head(net, x):
-    x = net.relu(net.conv1(x))
-    return net.up4(net.up3(net.up2(net.up1(x))))
+# GOF's head (scene/appearance_network.py): conv1, then up1..up4's convolutions after each PixelShuffle(2)
+_HEAD_LAYERS = (("conv1", 67, 256), ("up1", 64, 128), ("up2", 32, 64), ("up3", 16, 32), ("up4", 8, 16))
+
+
+def _head_convs(net):
+    return [(name, getattr(net, name, None) if name == "conv1" else getattr(getattr(net, name, None), "conv", None), cin, cout)
+            for name, cin, cout in _HEAD_LAYERS]
+
+
+def _head_params(net):
+    """conv1.weight, conv1.bias, up1.conv.weight, ..., up4.conv.bias: the module's parameter order."""
+    return [p for _, conv, _, _ in _head_convs(net) for p in (conv.weight, conv.bias)]
 
 
 def _check_network(net):
-    for name, cin, cout in (("conv2", 16, 16), ("conv3", 16, 3)):
-        conv = getattr(net, name, None)
+    tail = [(name, getattr(net, name, None), cin, cout) for name, cin, cout in (("conv2", 16, 16), ("conv3", 16, 3))]
+    for name, conv, cin, cout in tail + _head_convs(net):
         w = getattr(conv, "weight", None)
         if w is None or tuple(w.shape) != (cout, cin, 3, 3) or getattr(conv, "bias", None) is None:
             raise ValueError(f"appearance network: {name} must be a {cin} -> {cout} 3x3 convolution with bias, got "
                              f"{None if w is None else tuple(w.shape)}")
+
+
+def _embedding(gaussians, view_idx):
+    emb = gaussians.get_apperance_embedding(view_idx)
+    if tuple(emb.shape) != (64,):
+        raise ValueError(f"appearance embedding: the view's row must hold 64 values, got {tuple(emb.shape)}")
+    return emb
 
 
 def _check_images(image, gt):
@@ -46,6 +63,12 @@ def _check_images(image, gt):
         raise RuntimeError("L1_loss_appearance needs CUDA tensors: there is no CPU path")
 
 
+def _head(net, x):
+    """The head as the module's own layers (for row stages without a fused head, multigpu's CPU stand-ins)."""
+    x = net.relu(net.conv1(x))
+    return net.up4(net.up3(net.up2(net.up1(x))))
+
+
 def _head_input(down, emb):
     h, w = down.shape[1:]
     return torch.cat([down, emb[:, None, None].expand(emb.shape[0], h, w)], dim=0)[None]
@@ -55,27 +78,21 @@ class _AppearanceL1(torch.autograd.Function):
     @staticmethod
     def forward(ctx, image, gt, emb, net, *params):
         image, gt = image.contiguous(), gt.contiguous()
-        down = _C.appearance_downsample(image)
-        with torch.enable_grad():
-            d_leaf = down.detach().requires_grad_(True)
-            e_leaf = emb.detach().requires_grad_(True)
-            up4 = _head(net, _head_input(d_leaf, e_leaf))
+        down, emb = _C.appearance_downsample(image), emb.detach()
+        head = [p.detach() for p in params[:-4]]
+        head_act, up4 = _C._appearance_head.forward(down, emb, head)
         w2, b2, w3, b3 = net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias
-        loss, act, _ = _C.appearance_l1_forward(image, gt, up4.detach(), w2.detach(), b2.detach(), w3.detach(), b3.detach(), True, False)
-        ctx.head = (up4, d_leaf, e_leaf, params[:-4])
-        ctx.save_for_backward(image, gt, act, w2.detach(), b2.detach(), w3.detach(), b3.detach())
+        loss, act, _ = _C.appearance_l1_forward(image, gt, up4, w2.detach(), b2.detach(), w3.detach(), b3.detach(), True, False)
+        ctx.save_for_backward(image, gt, act, w2.detach(), b2.detach(), w3.detach(), b3.detach(), down, emb, head_act, up4, *head)
         return loss
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
-        image, gt, act, w2, b2, w3, b3 = ctx.saved_tensors
-        up4, d_leaf, e_leaf, head_params = ctx.head
-        d_img, d_up4, d_w2, d_b2, d_w3, d_b3 = _C.appearance_l1_backward(image, gt, up4.detach(), act, w2, b2, w3, b3,
-                                                                         grad_out.float().reshape(1))
-        grads = torch.autograd.grad(up4, [d_leaf, e_leaf, *head_params], d_up4)
+        image, gt, act, w2, b2, w3, b3, down, emb, head_act, up4, *head = ctx.saved_tensors
+        d_img, d_up4, d_w2, d_b2, d_w3, d_b3 = _C.appearance_l1_backward(image, gt, up4, act, w2, b2, w3, b3, grad_out.float().reshape(1))
+        grads = _C._appearance_head.backward(down, emb, head, head_act, up4, d_up4)
         _C.appearance_downsample_backward(grads[0], d_img)
-        ctx.head = None
         return (d_img, None, grads[1], None, *grads[2:], d_w2, d_b2, d_w3, d_b3)
 
 
@@ -84,16 +101,15 @@ def L1_loss_appearance(image: torch.Tensor, gt_image: torch.Tensor, gaussians, v
     the reference's transformed image (``mapping * crop`` resized back to the image size; forward only)."""
     net = gaussians.appearance_network
     _check_network(net)
+    emb = _embedding(gaussians, view_idx)
     _check_images(image, gt_image)
-    emb = gaussians.get_apperance_embedding(view_idx)
     if not return_transformed_image:
-        head = [p for m in (net.conv1, net.up1, net.up2, net.up3, net.up4) for p in m.parameters()]
-        params = head + [net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias]
+        params = _head_params(net) + [net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias]
         if len(params) != len(list(net.parameters())):
             raise ValueError("appearance network: parameters outside conv1, up1..up4, conv2 and conv3 are not supported")
         return _AppearanceL1.apply(image, gt_image, emb, net, *params)
     with torch.no_grad():
         image, gt_image = image.contiguous(), gt_image.contiguous()
-        up4 = _head(net, _head_input(_C.appearance_downsample(image), emb))
+        _, up4 = _C._appearance_head.forward(_C.appearance_downsample(image), emb, _head_params(net))
         _, _, t = _C.appearance_l1_forward(image, gt_image, up4, net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias, False, True)
         return F.interpolate(t[None], size=tuple(image.shape[1:]), mode="bilinear", align_corners=True)[0]

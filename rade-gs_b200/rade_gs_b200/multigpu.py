@@ -612,10 +612,10 @@ def _sum_in_rank_order(mine: torch.Tensor, world: int, group) -> torch.Tensor:
 class _SlabAppearanceL1(torch.autograd.Function):
     """train.py:37-58's `L1_loss_appearance` of the WHOLE image, evaluated slab by slab (include/rgs_b200.h's
     `rgs_appearance_*_rows`).  Forward: 4 image rows to and from each neighbour, the owned low-resolution rows all-gathered, the
-    cuDNN head replicated on every rank, the tail on the slab, and the per-rank fp64 loss sums all-gathered and added in rank order.
+    head replicated on every rank (the fused head kernels when `kernels` has them, else the module's layers), the tail on the slab, and the per-rank fp64 loss sums all-gathered and added in rank order.
     Backward: the owned rows of d(up4) all-gathered, so that the head's backward, d(down) and the embedding gradient are the
     single-GPU call's; the per-rank fp64 rows of conv2 / conv3's weight gradients added in rank order.  The image is never gathered.
-    `kernels` supplies the four row stages (the CUDA ones, or fp64 stand-ins in the CPU test)."""
+    `kernels` supplies the four row stages and the head (the CUDA ones), or the row stages alone (fp64 stand-ins in the CPU test)."""
 
     @staticmethod
     def forward(ctx, image, gt, emb, net, slab, kernels, *params):
@@ -637,14 +637,19 @@ class _SlabAppearanceL1(torch.autograd.Function):
             _exchange_rows(win, (a, a + k), (b - k, b) if r1 < H0 else (b, b), (0, a), (b, hi - lo), rank, world, group, add=False)
         gt_win = gt.detach()[:, lo:hi].contiguous()
         down = _gather_rows(kernels.downsample_rows(win, lo, H0, r0, r1), [(w[2], w[3]) for w in wins], H // 32, group)
-        with torch.enable_grad():
-            d_leaf = down.detach().requires_grad_(True)
-            e_leaf = emb.detach().requires_grad_(True)
-            up4 = _head(net, _head_input(d_leaf, e_leaf))
+        if hasattr(kernels, "head_forward"):   # the fused head (csrc/rgs_appearance_head.cu)
+            e, head = emb.detach(), [p.detach() for p in params[:-4]]
+            head_act, up4 = kernels.head_forward(down, e, head)
+            ctx.head = (up4, down, e, head, head_act)
+        else:                                  # the module's layers, for row stages that bring no head
+            with torch.enable_grad():
+                d_leaf = down.detach().requires_grad_(True)
+                e_leaf = emb.detach().requires_grad_(True)
+                up4 = _head(net, _head_input(d_leaf, e_leaf))
+            ctx.head = (up4, d_leaf, e_leaf, params[:-4], None)
         w2, b2, w3, b3 = (p.detach() for p in (net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias))
         loss_sum, act = kernels.l1_forward_rows(win, gt_win, lo, H0, r0, r1, up4.detach(), w2, b2, w3, b3)
         total = _sum_in_rank_order(loss_sum.clone(), world, group)
-        ctx.head = (up4, d_leaf, e_leaf, params[:-4])
         ctx.meta = (H0, lo, r0, r1, compact, [(w[4], w[5]) for w in wins], world, group, kernels)
         ctx.save_for_backward(win, gt_win, act, w2, b2, w3, b3)
         return (total[0] / (3.0 * H * W)).to(gt.dtype)   # float32 on the GPU, as L1_loss_appearance returns it
@@ -653,12 +658,15 @@ class _SlabAppearanceL1(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
         win, gt_win, act, w2, b2, w3, b3 = ctx.saved_tensors
-        up4, d_leaf, e_leaf, head_params = ctx.head
+        up4, down, emb, head_params, head_act = ctx.head
         H0, lo, r0, r1, compact, u_rows, world, group, kernels = ctx.meta
         d_img, d_up4, grad_row = kernels.l1_backward_rows(win, gt_win, lo, H0, r0, r1, up4.detach(), act, w2, b2, w3, b3,
                                                           grad_out.float().reshape(1))
         d_up4 = _gather_rows(d_up4, u_rows, up4.shape[-2], group).reshape(up4.shape)
-        grads = torch.autograd.grad(up4, [d_leaf, e_leaf, *head_params], d_up4)
+        if head_act is not None:
+            grads = kernels.head_backward(down, emb, head_params, head_act, up4, d_up4)
+        else:
+            grads = torch.autograd.grad(up4, [down, emb, *head_params], d_up4)
         g = _sum_in_rank_order(grad_row.clone(), world, group).to(w2.dtype)
         d_w2, d_b2, d_w3, d_b3 = g[:2304].view(w2.shape), g[2304:2320].view(b2.shape), g[2320:2752].view(w3.shape), g[2752:].view(b3.shape)
         kernels.downsample_backward_rows(grads[0], d_img, H0, r0, r1)
@@ -671,7 +679,7 @@ class _SlabAppearanceL1(torch.autograd.Function):
 
 
 class _CudaAppearanceRows:
-    """The CUDA row stages (`_C._slab.appearance_*_rows`)."""
+    """The CUDA row stages (`_C._slab.appearance_*_rows`) and the fused head (`_C._appearance_head`)."""
 
     @staticmethod
     def downsample_rows(win, lo, H0, r0, r1):
@@ -693,6 +701,16 @@ class _CudaAppearanceRows:
         from diff_gaussian_rasterization import _C
         _C._slab.appearance_downsample_backward_rows(d_down, d_img, H0, r0, r1)
 
+    @staticmethod
+    def head_forward(down, emb, head_params):
+        from diff_gaussian_rasterization import _C
+        return _C._appearance_head.forward(down, emb, head_params)
+
+    @staticmethod
+    def head_backward(down, emb, head_params, head_act, up4, d_up4):
+        from diff_gaussian_rasterization import _C
+        return _C._appearance_head.backward(down, emb, head_params, head_act, up4, d_up4)
+
 
 def slab_L1_loss_appearance(image: torch.Tensor, gt_image: torch.Tensor, gaussians, view_idx, pixel_rows: Tuple[int, int], all_pixel_rows=None,
                             image_height: int | None = None, rank: int | None = None, world_size: int | None = None, group=None, kernels=None,
@@ -703,19 +721,22 @@ def slab_L1_loss_appearance(image: torch.Tensor, gt_image: torch.Tensor, gaussia
     given, must agree).  Returns the whole image's loss, the same value on every rank.  Its gradient w.r.t. `image` lies in this
     rank's rows and is complete there; the network's parameter gradients and the embedding row's are the same bits on every rank.
     Only conv2 / conv3's weight gradients and the loss are summed in another order than the single-GPU call's (fp64 per rank, then
-    over the ranks in rank order); at one rank every result is that call's, bit for bit.  Bit-identical head gradients across ranks
-    (and across calls) need `torch.backends.cudnn.deterministic = True`, as for the single-GPU call.
+    over the ranks in rank order); at one rank every result is that call's, bit for bit.  With the built-in CUDA stages
+    (`kernels=None`) the head runs in the project's kernels on every rank, so its gradients are the same bits on every rank and
+    in every call, whatever torch's cuDNN and TF32 settings.  A `kernels` object without `head_forward` / `head_backward` runs the
+    head as the module's own layers instead (the CPU test's fp64 stand-ins), and that guarantee does not hold for it.
 
     Every slab that does not end at the image's last row must hold at least 4 rows (the halo).  With `all_pixel_rows`, every rank's
     row range, every rank refuses a bad partition before any collective; without it the ranks first all-gather their row ranges
     (one small collective) and then all refuse a bad partition together.  The checks of a rank's own arguments (the network, the
-    image's shape, CUDA tensors) run before that gather: a rank whose own arguments are wrong raises alone, and without
+    image's shape, the embedding row, CUDA tensors) run before that gather: a rank whose own arguments are wrong raises alone, and without
     `all_pixel_rows` its peers then wait in the gather.  `return_transformed_image` has no slab form."""
     if return_transformed_image:
         raise ValueError("slab_L1_loss_appearance has no transformed-image form: gather the image and call appearance.L1_loss_appearance")
-    from .appearance import _check_network
+    from .appearance import _check_network, _embedding, _head_params
     net = gaussians.appearance_network
     _check_network(net)
+    emb = _embedding(gaussians, view_idx)
     if gt_image.requires_grad:
         raise ValueError("slab_L1_loss_appearance differentiates w.r.t. the rendered image, not the ground truth")
     if gt_image.dim() != 3 or gt_image.shape[0] != 3 or gt_image.shape[1] < 32 or gt_image.shape[2] < 32:
@@ -744,9 +765,7 @@ def slab_L1_loss_appearance(image: torch.Tensor, gt_image: torch.Tensor, gaussia
         _check_slab_rows(pixel_rows, rows, H0, rank, world_size, APPEARANCE_HALO, what)
     else:
         rows = [(r0, r1)]
-    head = [p for m in (net.conv1, net.up1, net.up2, net.up3, net.up4) for p in m.parameters()]
-    params = head + [net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias]
+    params = _head_params(net) + [net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias]
     if len(params) != len(list(net.parameters())):
         raise ValueError("appearance network: parameters outside conv1, up1..up4, conv2 and conv3 are not supported")
-    emb = gaussians.get_apperance_embedding(view_idx)
     return _SlabAppearanceL1.apply(image, gt_image, emb, net, (H0, rows, rank, world_size, group), kernels or _CudaAppearanceRows, *params)
