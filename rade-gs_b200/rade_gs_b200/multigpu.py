@@ -62,6 +62,15 @@ def partition_tile_rows(grid_y: int, world_size: int, weights: Sequence[float] |
     return [(cuts[i], max(cuts[i], cuts[i + 1])) for i in range(world_size)]
 
 
+def _rank_world(rank, world_size, group):
+    """(rank, world size) in `group`: an explicit argument wins; without an initialised process group this is rank 0 of 1."""
+    if world_size is None:
+        world_size = dist.get_world_size(group) if dist.is_initialized() else 1
+    if rank is None:
+        rank = dist.get_rank(group) if dist.is_initialized() else 0
+    return rank, world_size
+
+
 def allreduce_sum_(t: torch.Tensor, group=None) -> torch.Tensor:
     """In-place sum over ranks; a no-op outside an initialised process group (single-GPU path)."""
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
@@ -99,8 +108,7 @@ class GradExchange:
 
     def __init__(self, capacity_rows: int, row_floats: int, device, group=None, mode: str | None = None):
         self.group, self.device = group, torch.device(device)
-        self.world = dist.get_world_size(group) if dist.is_initialized() else 1
-        self.rank = dist.get_rank(group) if dist.is_initialized() else 0
+        self.rank, self.world = _rank_world(None, None, group)
         mode = mode or os.environ.get("RGS_GRAD_EXCHANGE", "peer")
         if mode not in ("peer", "dense"):
             raise ValueError(f"gradient exchange mode must be 'peer' or 'dense', got {mode!r}")
@@ -229,6 +237,47 @@ class _ShardedRasterize(torch.autograd.Function):
         return g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, None, None, None, None, None, None
 
 
+def _gather_rows(mine: torch.Tensor, ranges, n_rows: int, group) -> torch.Tensor:
+    """The whole [C, n_rows, ...] map from each rank's rows `ranges[r]` (`mine` holds this rank's): an all-gather of pure copies,
+    so every rank holds the bits their owners computed."""
+    if len(ranges) == 1:
+        return mine
+    hmax = max(e - b for b, e in ranges)
+    buf = mine.new_zeros(mine.shape[0], hmax, *mine.shape[2:])
+    buf[:, :mine.shape[1]] = mine
+    parts = [torch.empty_like(buf) for _ in ranges]
+    dist.all_gather(parts, buf, group=group)
+    out = mine.new_empty(mine.shape[0], n_rows, *mine.shape[2:])
+    for (b, e), p in zip(ranges, parts):
+        out[:, b:e] = p[:, :e - b]
+    return out
+
+
+class _SlabLayout:
+    """How a rank's maps hold its pixel rows [r0, r1) of an H-row image: compact maps ([C, r1 - r0, W]) hold only those rows,
+    full-size ones ([C, H, W]) all rows with the slab's filled.  The two coincide when the slab is the whole image."""
+
+    def __init__(self, t, H, r0, r1):   # the layout of map `t`
+        self.H, self.r0, self.r1, self.compact = H, r0, r1, t.shape[-2] != H
+
+    @staticmethod
+    def check(maps, H, r0, r1, W, together=None):
+        """Raise unless every map of `maps` [(name, tensor, channels)] is [channels, H or r1 - r0 rows, W], all in one layout."""
+        for name, t, c in maps:
+            if t.dim() != 3 or t.shape[0] != c or t.shape[-1] != W or t.shape[-2] not in (H, r1 - r0):
+                raise ValueError(f"{name} must be [{c}, {H} or {r1 - r0} rows, {W}] (full-size or the slab's rows), got {tuple(t.shape)}")
+        if len({t.shape[-2] for _, t, _ in maps}) != 1:
+            raise ValueError(f"{together} must all be full-size or all hold the slab's rows")
+
+    def own(self, t):   # the slab's rows of map `t`, detached
+        return t.detach() if self.compact else t.detach()[:, self.r0:self.r1]
+
+    def full(self, rows):   # the slab's rows [C, r1 - r0, W] in a full-size map, zero elsewhere
+        out = rows.new_zeros(rows.shape[0], self.H, rows.shape[-1])
+        out[:, self.r0:self.r1] = rows
+        return out
+
+
 class _GatherSlabs(torch.autograd.Function):
     """All-gather of the ranks' slab rows into the whole map (pure copies: the gathered map holds exactly the bits each
     rank rendered); identity backward (every rank holds the same full-image loss, and a rank's backward reads only the rows
@@ -236,20 +285,9 @@ class _GatherSlabs(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, img, group, pixel_rows, rank):
-        world = len(pixel_rows)
-        if not (dist.is_available() and dist.is_initialized()) or world == 1:
+        if not (dist.is_available() and dist.is_initialized()) or len(pixel_rows) == 1:
             return img.detach().clone()
-        C, H, W = img.shape
-        hmax = max(e - b for b, e in pixel_rows)
-        b, e = pixel_rows[rank]
-        mine = img.new_zeros(C, hmax, W)
-        mine[:, : e - b] = img.detach()[:, b:e]
-        parts = [torch.empty_like(mine) for _ in range(world)]
-        dist.all_gather(parts, mine, group=group)
-        out = torch.empty_like(img)
-        for r, (rb, re) in enumerate(pixel_rows):
-            out[:, rb:re] = parts[r][:, : re - rb]
-        return out
+        return _gather_rows(img.detach()[:, slice(*pixel_rows[rank])], pixel_rows, img.shape[1], group)
 
     @staticmethod
     def backward(ctx, grad_out):
@@ -279,11 +317,7 @@ class ShardedGaussianRasterizer(torch.nn.Module):
         self.raster_settings = raster_settings
         self.group = group
         self.exchange = exchange   # a GradExchange created once by the caller (collective); None: one dense all-reduce per backward
-        if world_size is None:
-            world_size = dist.get_world_size(group) if dist.is_initialized() else 1
-        if rank is None:
-            rank = dist.get_rank(group) if dist.is_initialized() else 0
-        self.rank, self.world_size = rank, world_size
+        self.rank, self.world_size = rank, world_size = _rank_world(rank, world_size, group)
         self.balance = bool(balance)
         grid_y = tile_rows(raster_settings.image_height)
         if self.balance and grid_y < world_size:
@@ -320,13 +354,9 @@ class ShardedGaussianRasterizer(torch.nn.Module):
         normal consistency) can be evaluated redundantly per rank; its gradient flows back unchanged and the sharded
         rasterizer's backward reads only the rows of its own slab, so nothing is counted twice.
         """
-        H = self.raster_settings.image_height
         rows = self.all_pixel_rows()
         if self.compact:   # [C, slab rows, W] -> place into a full-size map first (the gather copies slab rows only)
-            full = img.new_zeros(img.shape[0], H, img.shape[2])
-            r0, r1 = rows[self.rank]
-            full[:, r0:r1] = img
-            img = full
+            img = _SlabLayout(img, self.raster_settings.image_height, *rows[self.rank]).full(img)
         return _GatherSlabs.apply(img, self.group, rows, self.rank)
 
 
@@ -357,6 +387,30 @@ def _exchange_rows(t: torch.Tensor, send_up, send_down, recv_up, recv_down, rank
             t[:, r0:r1] = buf
 
 
+def _exchange_halo(t: torch.Tensor, lo: int, r0: int, r1: int, H: int, halo: int, rank: int, world: int, group, backward: bool = False):
+    """The `halo`-row exchange of the rank owning pixel rows [r0, r1) of an H-row image, on `t` holding image rows [lo, lo + t.shape[1]).
+    Forward: the slab's first and last min(halo, r1 - r0) rows go up and down (not down when the slab ends at the image's last row:
+    the ranks after it hold empty slabs), and the neighbours' rows fill [max(0, r0 - halo), r0) and [r1, min(H, r1 + halo)).
+    Backward: the reverse, rows outside [r0, r1) go to their owners and are added into the slab's edge rows.  An empty slab exchanges nothing."""
+    if r1 <= r0:
+        return
+    k = min(halo, r1 - r0)
+    edges = ((r0, r0 + k), (r1 - k, r1) if r1 < H else (r1, r1))
+    halos = ((max(0, r0 - halo), r0), (r1, min(H, r1 + halo)))
+    send, recv = (halos, edges) if backward else (edges, halos)
+    _exchange_rows(t, *((b - lo, e - lo) for b, e in send + recv), rank, world, group, add=backward)
+
+
+def _halo_window(maps, layout: _SlabLayout, halo: int, rank: int, world: int, group):
+    """(window, lo): `maps`' rows [lo = max(0, r0 - halo), min(H, r1 + halo)) stacked along channels, the halo rows exchanged."""
+    lo = max(0, layout.r0 - halo)
+    win = maps[0].new_zeros(sum(m.shape[0] for m in maps), min(layout.H, layout.r1 + halo) - lo, maps[0].shape[-1])
+    for part, m in zip(win.split([m.shape[0] for m in maps]), maps):
+        part[:, layout.r0 - lo:layout.r1 - lo] = layout.own(m)
+    _exchange_halo(win, lo, layout.r0, layout.r1, layout.H, halo, rank, world, group)
+    return win, lo
+
+
 class _SlabSsimL1(torch.autograd.Function):
     """(1 - l) * L1 + l * (1 - SSIM) of the WHOLE image (train.py:163), evaluated slab by slab: a rank counts the SSIM-map and L1
     rows of its own slab; the 11x11 window reaches 5 rows into the neighbours' slabs, so 5 halo rows travel to each neighbour in
@@ -371,7 +425,7 @@ class _SlabSsimL1(torch.autograd.Function):
         H = image.shape[-2]
         img = image.detach().clone()
         # my first / last 5 rows are the neighbours' halos; theirs are mine
-        _exchange_rows(img, (r0, min(r0 + HALO, r1)), (max(r1 - HALO, r0), r1), (max(r0 - HALO, 0), r0), (r1, min(r1 + HALO, H)), rank, world, group, add=False)
+        _exchange_halo(img, 0, r0, r1, H, HALO, rank, world, group)
         sums, state = fwd(img, gt, r0, r1, ctx.needs_input_grad[0])
         sums = sums.clone()
         if world > 1:
@@ -387,10 +441,8 @@ class _SlabSsimL1(torch.autograd.Function):
         lam, n, r0, r1, rank, world, group, bwd, H = ctx.meta
         d = bwd(img, gt, state, -lam / n, (1.0 - lam) / n, r0, r1)
         # rows [r0-5, r0) and [r1, r1+5) hold what MY slab's SSIM values contribute to the neighbours' pixels: send them home
-        _exchange_rows(d, (max(r0 - HALO, 0), r0), (r1, min(r1 + HALO, H)), (r0, min(r0 + HALO, r1)), (max(r1 - HALO, r0), r1), rank, world, group, add=True)
-        out = torch.zeros_like(d)
-        out[:, r0:r1] = d[:, r0:r1]
-        return out * grad_out, None, None, None, None, None, None, None, None
+        _exchange_halo(d, 0, r0, r1, H, HALO, rank, world, group, backward=True)
+        return _SlabLayout(d, H, r0, r1).full(d[:, r0:r1]) * grad_out, None, None, None, None, None, None, None, None
 
 
 def _cuda_slab_fwd(img, gt, r0, r1, need_grad):
@@ -405,11 +457,11 @@ def _cuda_slab_bwd(img, gt, state, w_ssim, w_l1, r0, r1):
 
 
 def _check_ssim_rows(pixel_rows, H, world_size):
-    """Raise unless this rank's rows suit slab_l1_ssim_loss's 5-row halo exchange (its docstring states the rule)."""
-    r0, r1 = int(pixel_rows[0]), int(pixel_rows[1])
-    if world_size > 1 and r1 - r0 < HALO and not r0 < r1 == H:
-        raise ValueError("slab-local SSIM needs at least 5 pixel rows on every slab that does not end at the image's last row (a shorter "
-                         "slab breaks the neighbour halo exchange)")
+    """Raise unless this rank's rows suit slab_l1_ssim_loss's 5-row halo exchange: `_check_slab_rows`, and no empty slab at > 1 rank."""
+    r0, r1 = _check_slab_rows(pixel_rows, None, H, 0, world_size, HALO, "slab-local SSIM")
+    if world_size > 1 and r0 == r1:
+        raise ValueError(f"slab-local SSIM needs at least 5 pixel rows on every slab but a non-empty last one; slab [{r0}, {r1}) is empty")
+    return r0, r1
 
 
 def slab_l1_ssim_loss(image: torch.Tensor, gt: torch.Tensor, lambda_dssim: float, pixel_rows: Tuple[int, int], rank: int | None = None,
@@ -420,13 +472,10 @@ def slab_l1_ssim_loss(image: torch.Tensor, gt: torch.Tensor, lambda_dssim: float
     already contains the neighbours' contributions.  Every slab that does not end at the image's last row must be at least 5 rows
     tall; a non-empty slab that ends there may be shorter (the halo its neighbour above needs ends at the image's edge too), as the
     last tile row of an image whose height is not a multiple of 16 is."""
-    if world_size is None:
-        world_size = dist.get_world_size(group) if dist.is_initialized() else 1
-    if rank is None:
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
-    _check_ssim_rows(pixel_rows, image.shape[-2], world_size)
+    rank, world_size = _rank_world(rank, world_size, group)
+    rows = _check_ssim_rows(pixel_rows, image.shape[-2], world_size)
     fwd, bwd = kernels if kernels is not None else (_cuda_slab_fwd, _cuda_slab_bwd)
-    return _SlabSsimL1.apply(image, gt, float(lambda_dssim), (int(pixel_rows[0]), int(pixel_rows[1])), rank, world_size, group, fwd, bwd)
+    return _SlabSsimL1.apply(image, gt, float(lambda_dssim), rows, rank, world_size, group, fwd, bwd)
 
 
 # ---- slab-local normal consistency (train.py:141-156) ------------------------------------------------------------------------
@@ -446,19 +495,12 @@ class _SlabNormalConsistency(torch.autograd.Function):
         r0, r1 = rows
         W = normal.shape[-1]
         C = map_e.shape[0]
-        compact = normal.shape[-2] != H   # else full-size (the two coincide when one slab is the whole image)
-        own = (lambda t: t.detach()) if compact else (lambda t: t.detach()[:, r0:r1])
-        m_lo, m_hi = max(0, r0 - NORMAL_HALO), min(H, r1 + NORMAL_HALO)
+        layout = _SlabLayout(normal, H, r0, r1)
         n_lo, n_hi = max(0, r0 - 1), min(H, r1 + 1)
         w_e, w_m = (1.0 - depth_ratio) / (H * W), depth_ratio / (H * W)
         if r1 > r0:
             # both maps and the normal in one row window, so that one exchange carries all their halo rows
-            win = normal.new_zeros(2 * C + 3, m_hi - m_lo, W)
-            a, b = r0 - m_lo, r1 - m_lo
-            win[:C, a:b], win[C:2 * C, a:b], win[2 * C:, a:b] = own(map_e), own(map_m), own(normal)
-            k = min(NORMAL_HALO, r1 - r0)
-            # a slab that ends at the image's last row has no neighbour below (later ranks' slabs are empty there)
-            _exchange_rows(win, (a, a + k), (b - k, b) if r1 < H else (b, b), (0, a), (b, m_hi - m_lo), rank, world, group, add=False)
+            win, m_lo = _halo_window([map_e, map_m, normal], layout, NORMAL_HALO, rank, world, group)
             loss, dn, de, dm = kernel(win[2 * C:, n_lo - m_lo:n_hi - m_lo].contiguous(), win[:C].contiguous(), win[C:2 * C].contiguous(), from_depth,
                                       *cam, w_e, w_m, H, r0, r1)
             loss = loss.clone()
@@ -468,21 +510,13 @@ class _SlabNormalConsistency(torch.autograd.Function):
         if world > 1:
             dist.all_reduce(loss, group=group)
         ctx.save_for_backward(dn, de, dm)
-        ctx.meta = (compact, H, r0, r1)
+        ctx.layout = layout
         return loss[0].float()
 
     @staticmethod
     def backward(ctx, grad_out):
-        compact, H, r0, r1 = ctx.meta
-
-        def place(d):
-            if compact:
-                return d * grad_out
-            out = d.new_zeros(d.shape[0], H, d.shape[2])
-            out[:, r0:r1] = d * grad_out
-            return out
-
-        return (*(place(d) for d in ctx.saved_tensors), None, None, None, None, None, None, None, None, None)
+        lay = ctx.layout
+        return (*(d * grad_out if lay.compact else lay.full(d * grad_out) for d in ctx.saved_tensors), None, None, None, None, None, None, None, None, None)
 
 
 def _cuda_normal_rows(normal_win, e_win, m_win, from_depth, inv_fx, inv_fy, cx, cy, w_e, w_m, H, r0, r1):
@@ -513,32 +547,34 @@ def _check_slab_rows(pixel_rows, all_pixel_rows, H, rank, world_size, halo=NORMA
     return r0, r1
 
 
+def _gather_and_check_slab_rows(pixel_rows, H, rank, world_size, group, halo, what, device):
+    """Every rank's pixel rows, for a caller that was not given them: at more than one rank all-gathered (one small collective), then
+    checked as a whole partition by `_check_slab_rows` on every rank, so that all ranks refuse a bad one together."""
+    if world_size == 1:
+        return [(int(pixel_rows[0]), int(pixel_rows[1]))]
+    parts = [torch.empty(2, dtype=torch.int64, device=device) for _ in range(world_size)]
+    dist.all_gather(parts, torch.tensor([int(pixel_rows[0]), int(pixel_rows[1])], dtype=torch.int64, device=device), group=group)
+    rows = [tuple(p.tolist()) for p in parts]
+    _check_slab_rows(pixel_rows, rows, H, rank, world_size, halo, what)
+    return rows
+
+
 def _slab_normal_loss(normal, map_e, map_m, from_depth, cam, depth_ratio, H, pixel_rows, all_pixel_rows, rank, world_size, group, kernels,
                       map_channels):
-    if world_size is None:
-        world_size = dist.get_world_size(group) if dist.is_initialized() else 1
-    if rank is None:
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
     r0, r1 = _check_slab_rows(pixel_rows, all_pixel_rows, H, rank, world_size)
     if kernels is None and not (normal.is_cuda and map_e.is_cuda and map_m.is_cuda):
         raise RuntimeError("slab-local normal consistency needs CUDA tensors: there is no CPU path")
-    W = normal.shape[-1]
-    for name, t, c in (("normal", normal, 3), ("expected map", map_e, map_channels), ("median map", map_m, map_channels)):
-        if t.dim() != 3 or t.shape[0] != c or t.shape[-1] != W or t.shape[-2] not in (H, r1 - r0):
-            raise ValueError(f"{name} must be [{c}, {H} or {r1 - r0} rows, {W}] (full-size or the slab's rows), got {tuple(t.shape)}")
-    if len({normal.shape[-2], map_e.shape[-2], map_m.shape[-2]}) != 1:
-        raise ValueError("the normal and both maps must all be full-size or all hold the slab's rows")
+    _SlabLayout.check([("normal", normal, 3), ("expected map", map_e, map_channels), ("median map", map_m, map_channels)], H, r0, r1,
+                      normal.shape[-1], "the normal and both maps")
     kernel = kernels if kernels is not None else _cuda_normal_rows
     return _SlabNormalConsistency.apply(normal, map_e, map_m, from_depth, cam, float(depth_ratio), H, (r0, r1), rank, world_size, group, kernel)
 
 
-def _image_height(t, pixel_rows, image_height, world_size, group):
+def _image_height(t, pixel_rows, image_height, world_size):
     """The image's row count: `image_height`, else that of full-size maps.  Maps with the slab's row count are taken for compact
     ones when there are several ranks, and then the height cannot be read from them."""
     if image_height is not None:
         return int(image_height)
-    if world_size is None:
-        world_size = dist.get_world_size(group) if dist.is_initialized() else 1
     if world_size > 1 and t.shape[-2] == pixel_rows[1] - pixel_rows[0]:
         raise ValueError("maps that hold only the slab's rows need image_height")
     return int(t.shape[-2])
@@ -557,7 +593,8 @@ def slab_depth_normal_consistency_loss(view, normal: torch.Tensor, expected_dept
     raises and its neighbours block in the halo exchange."""
     if image_height is None:
         image_height = getattr(view, "image_height", None)
-    H = _image_height(normal, pixel_rows, image_height, world_size, group)
+    rank, world_size = _rank_world(rank, world_size, group)
+    H = _image_height(normal, pixel_rows, image_height, world_size)
     W = normal.shape[-1]
     fx = W / (2 * math.tan(view.FoVx / 2.))
     fy = H / (2 * math.tan(view.FoVy / 2.))
@@ -572,29 +609,14 @@ def slab_point_normal_consistency_loss(normal: torch.Tensor, expected_coord: tor
                                        world_size: int | None = None, group=None, kernels=None) -> torch.Tensor:
     """`losses.point_normal_consistency_loss` (train.py:141-156 with require_coord) for a row-sharded render; the maps as in
     `slab_depth_normal_consistency_loss`, and so is `all_pixel_rows`.  Compact maps need `image_height`."""
-    H = _image_height(normal, pixel_rows, image_height, world_size, group)
+    rank, world_size = _rank_world(rank, world_size, group)
+    H = _image_height(normal, pixel_rows, image_height, world_size)
     return _slab_normal_loss(normal, expected_coord, median_coord, False, (0.0, 0.0, 0.0, 0.0), depth_ratio, H, pixel_rows, all_pixel_rows, rank,
                              world_size, group, kernels, 3)
 
 
 # ---- slab-local decoupled-appearance L1 (train.py:37-58) ---------------------------------------------------------------------
 APPEARANCE_HALO = 4   # image rows either side of a slab whose loss derivative its d_up4 rows need (include/rgs_b200.h)
-
-
-def _gather_rows(mine: torch.Tensor, ranges, n_rows: int, group) -> torch.Tensor:
-    """The whole [C, n_rows, ...] map from each rank's rows `ranges[r]` (`mine` holds this rank's): an all-gather of pure copies,
-    so every rank holds the bits their owners computed."""
-    if len(ranges) == 1:
-        return mine
-    hmax = max(e - b for b, e in ranges)
-    buf = mine.new_zeros(mine.shape[0], hmax, *mine.shape[2:])
-    buf[:, :mine.shape[1]] = mine
-    parts = [torch.empty_like(buf) for _ in ranges]
-    dist.all_gather(parts, buf, group=group)
-    out = mine.new_empty(mine.shape[0], n_rows, *mine.shape[2:])
-    for (b, e), p in zip(ranges, parts):
-        out[:, b:e] = p[:, :e - b]
-    return out
 
 
 def _sum_in_rank_order(mine: torch.Tensor, world: int, group) -> torch.Tensor:
@@ -624,18 +646,11 @@ class _SlabAppearanceL1(torch.autograd.Function):
         from .appearance import _head, _head_input
         r0, r1 = rows[rank]
         W0 = gt.shape[-1]
-        compact = image.shape[-2] != H0
+        layout = _SlabLayout(image, H0, r0, r1)
         H, W = H0 // 32 * 32, W0 // 32 * 32
         wins = [_C._slab.appearance_row_windows(H0, W0, b, e) for b, e in rows]
-        lo, hi = max(0, r0 - APPEARANCE_HALO), min(H0, r1 + APPEARANCE_HALO)
-        win = image.new_zeros(3, hi - lo, W0)
-        a, b = r0 - lo, r1 - lo
-        if r1 > r0:
-            win[:, a:b] = image.detach() if compact else image.detach()[:, r0:r1]
-            k = min(APPEARANCE_HALO, r1 - r0)
-            # a slab that ends at the image's last row has no neighbour below (later ranks' slabs are empty there)
-            _exchange_rows(win, (a, a + k), (b - k, b) if r1 < H0 else (b, b), (0, a), (b, hi - lo), rank, world, group, add=False)
-        gt_win = gt.detach()[:, lo:hi].contiguous()
+        win, lo = _halo_window([image], layout, APPEARANCE_HALO, rank, world, group)
+        gt_win = gt.detach()[:, lo:lo + win.shape[1]].contiguous()
         down = _gather_rows(kernels.downsample_rows(win, lo, H0, r0, r1), [(w[2], w[3]) for w in wins], H // 32, group)
         if hasattr(kernels, "head_forward"):   # the fused head (csrc/rgs_appearance_head.cu)
             e, head = emb.detach(), [p.detach() for p in params[:-4]]
@@ -650,7 +665,7 @@ class _SlabAppearanceL1(torch.autograd.Function):
         w2, b2, w3, b3 = (p.detach() for p in (net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias))
         loss_sum, act = kernels.l1_forward_rows(win, gt_win, lo, H0, r0, r1, up4.detach(), w2, b2, w3, b3)
         total = _sum_in_rank_order(loss_sum.clone(), world, group)
-        ctx.meta = (H0, lo, r0, r1, compact, [(w[4], w[5]) for w in wins], world, group, kernels)
+        ctx.meta = (H0, lo, r0, r1, layout, [(w[4], w[5]) for w in wins], world, group, kernels)
         ctx.save_for_backward(win, gt_win, act, w2, b2, w3, b3)
         return (total[0] / (3.0 * H * W)).to(gt.dtype)   # float32 on the GPU, as L1_loss_appearance returns it
 
@@ -659,7 +674,7 @@ class _SlabAppearanceL1(torch.autograd.Function):
     def backward(ctx, grad_out):
         win, gt_win, act, w2, b2, w3, b3 = ctx.saved_tensors
         up4, down, emb, head_params, head_act = ctx.head
-        H0, lo, r0, r1, compact, u_rows, world, group, kernels = ctx.meta
+        H0, lo, r0, r1, layout, u_rows, world, group, kernels = ctx.meta
         d_img, d_up4, grad_row = kernels.l1_backward_rows(win, gt_win, lo, H0, r0, r1, up4.detach(), act, w2, b2, w3, b3,
                                                           grad_out.float().reshape(1))
         d_up4 = _gather_rows(d_up4, u_rows, up4.shape[-2], group).reshape(up4.shape)
@@ -670,12 +685,8 @@ class _SlabAppearanceL1(torch.autograd.Function):
         g = _sum_in_rank_order(grad_row.clone(), world, group).to(w2.dtype)
         d_w2, d_b2, d_w3, d_b3 = g[:2304].view(w2.shape), g[2304:2320].view(b2.shape), g[2320:2752].view(w3.shape), g[2752:].view(b3.shape)
         kernels.downsample_backward_rows(grads[0], d_img, H0, r0, r1)
-        if not compact:
-            full = d_img.new_zeros(3, H0, d_img.shape[-1])
-            full[:, r0:r1] = d_img
-            d_img = full
         ctx.head = None
-        return (d_img, None, grads[1], None, None, None, *grads[2:], d_w2, d_b2, d_w3, d_b3)
+        return (d_img if layout.compact else layout.full(d_img), None, grads[1], None, None, None, *grads[2:], d_w2, d_b2, d_w3, d_b3)
 
 
 class _CudaAppearanceRows:
@@ -744,27 +755,15 @@ def slab_L1_loss_appearance(image: torch.Tensor, gt_image: torch.Tensor, gaussia
     H0, W0 = gt_image.shape[1:]
     if image_height is not None and int(image_height) != H0:
         raise ValueError(f"image_height {image_height} is not the ground truth's {H0} rows")
-    if world_size is None:
-        world_size = dist.get_world_size(group) if dist.is_initialized() else 1
-    if rank is None:
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
+    rank, world_size = _rank_world(rank, world_size, group)
     what = "the slab-local appearance loss"
     # without every rank's rows, the slab lengths are checked after the rows are gathered, so that all ranks raise together
     r0, r1 = _check_slab_rows(pixel_rows, all_pixel_rows, H0, rank, world_size if all_pixel_rows is not None else 1, APPEARANCE_HALO, what)
-    if image.dim() != 3 or image.shape[0] != 3 or image.shape[2] != W0 or image.shape[1] not in (H0, r1 - r0):
-        raise ValueError(f"image must be [3, {H0} or {r1 - r0} rows, {W0}] (full-size or the slab's rows), got {tuple(image.shape)}")
+    _SlabLayout.check([("image", image, 3)], H0, r0, r1, W0)
     if kernels is None and not (image.is_cuda and gt_image.is_cuda):
         raise RuntimeError("slab_L1_loss_appearance needs CUDA tensors: there is no CPU path")
-    if all_pixel_rows is not None:
-        rows = [(int(b), int(e)) for b, e in all_pixel_rows]
-    elif world_size > 1:
-        mine = torch.tensor([r0, r1], dtype=torch.int64, device=image.device)
-        parts = [torch.empty_like(mine) for _ in range(world_size)]
-        dist.all_gather(parts, mine, group=group)
-        rows = [tuple(int(v) for v in p.tolist()) for p in parts]
-        _check_slab_rows(pixel_rows, rows, H0, rank, world_size, APPEARANCE_HALO, what)
-    else:
-        rows = [(r0, r1)]
+    rows = ([(int(b), int(e)) for b, e in all_pixel_rows] if all_pixel_rows is not None
+            else _gather_and_check_slab_rows(pixel_rows, H0, rank, world_size, group, APPEARANCE_HALO, what, image.device))
     params = _head_params(net) + [net.conv2.weight, net.conv2.bias, net.conv3.weight, net.conv3.bias]
     if len(params) != len(list(net.parameters())):
         raise ValueError("appearance network: parameters outside conv1, up1..up4, conv2 and conv3 are not supported")

@@ -193,6 +193,8 @@ def test_ssim_row_check_still_refuses_short_inner_and_empty_last_slabs():
         multigpu._check_ssim_rows((96, 98), 100, 3)      # short, not at the image's last row
     with pytest.raises(ValueError, match="5 pixel rows"):
         multigpu._check_ssim_rows((98, 98), 98, 3)       # empty
+    with pytest.raises(ValueError, match="not rows of a 100-row image"):
+        multigpu._check_ssim_rows((96, 104), 100, 3)     # past the image's last row: refused before the halo exchange
     multigpu._check_ssim_rows((96, 98), 98, 3)
 
 
