@@ -251,16 +251,15 @@ static int carve_geom_buffer(const FwdParams& p, const rgs_buffers* bufs, GeomVi
 	return rc;
 }
 
-// image-side scratch (carved for maps of N pixels) and the geometry buffer
-static int carve_forward(const FwdParams& p, size_t N, const rgs_buffers* bufs, GeomView& g, ImgView& img) {
-	int rc;
-	char* img_ptr;
-	// image-side scratch first: needed even when there is nothing to draw (background fill)
+// image-side scratch, carved for p's maps ([C, Hs, W])
+static int carve_img_buffer(const FwdParams& p, const rgs_buffers* bufs, ImgView& img) {
+	const size_t N = (size_t)p.W * p.Hs;
 	size_t img_bytes = 0;
 	carve_img(nullptr, p.grid_x, p.grid_y, N, p.coord, p.depth, &img_bytes);
-	if ((rc = grow(bufs->image, bufs->image_user, img_bytes, img_ptr, "image buffer")) != RGS_OK) return rc;
-	img = carve_img(img_ptr, p.grid_x, p.grid_y, N, p.coord, p.depth, nullptr);
-	return carve_geom_buffer(p, bufs, g);
+	char* img_ptr;
+	const int rc = grow(bufs->image, bufs->image_user, img_bytes, img_ptr, "image buffer");
+	if (rc == RGS_OK) img = carve_img(img_ptr, p.grid_x, p.grid_y, N, p.coord, p.depth, nullptr);
+	return rc;
 }
 
 // preprocess -> per-tile counts, ranges and totals of p's tile rows (P > 0)
@@ -305,7 +304,8 @@ static int64_t bin_tiles(const rgs_camera* cam, const FwdParams& p, int* radii, 
 static int64_t forward_to_binning(const rgs_camera* cam, const FwdParams& p, int* radii, const rgs_buffers* bufs, cudaStream_t s, GeomView& g,
                                   BinView& b, ImgView& img) {
 	int rc;
-	if ((rc = carve_forward(p, (size_t)p.W * p.Hs, bufs, g, img)) != RGS_OK) return rc;
+	// image-side scratch first: needed even when there is nothing to draw (background fill)
+	if ((rc = carve_img_buffer(p, bufs, img)) != RGS_OK || (rc = carve_geom_buffer(p, bufs, g)) != RGS_OK) return rc;
 
 	int64_t R = 0;
 	uint32_t max_list = 0;
@@ -395,11 +395,8 @@ int64_t rgs_forward_balanced(const rgs_camera* cam, const rgs_gaussians* gs, int
 			sh.chunk_total += stats[2 * gy + y];
 		}
 	}
-	size_t img_bytes = 0;
-	carve_img(nullptr, ps.grid_x, ps.grid_y, (size_t)ps.W * ps.Hs, ps.coord, ps.depth, &img_bytes);
-	char* img_ptr;
-	if ((rc = grow(bufs->image, bufs->image_user, img_bytes, img_ptr, "image buffer")) != RGS_OK) return rc;
-	const ImgView img = carve_img(img_ptr, ps.grid_x, ps.grid_y, (size_t)ps.W * ps.Hs, ps.coord, ps.depth, nullptr);
+	ImgView img;
+	if ((rc = carve_img_buffer(ps, bufs, img)) != RGS_OK) return rc;
 	if (p.P > 0) {
 		StageScope sc(ST_SCAN, s);
 		launch_slab_restrict(ps, g, counts, img, out->radii, sh, s);
@@ -486,43 +483,43 @@ static int backward_views(const rgs_camera* cam, const rgs_gaussians* gs, const 
 	return RGS_OK;
 }
 
-int32_t rgs_backward_render(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_backward_in* in, float* grad_accum, void* cuda_stream) {
-	FwdParams p;
-	GeomView g;
+// Stage 1 into the accumulator rows `acc` (`missing`: the error when there are none), zero-filled first with `zero_first`.  Leaves
+// p and g for the caller's next step.
+static int backward_render(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_backward_in* in, float* acc, const char* missing,
+                           bool zero_first, cudaStream_t s, FwdParams& p, GeomView& g) {
 	BinView b;
 	ImgView img;
 	int rc = backward_views(cam, gs, in, p, g, b, img);
-	if (rc != RGS_OK) return rc;
-	if (p.P == 0) return RGS_OK;
-	if (!grad_accum) return fail(RGS_E_INVALID, "null gradient accumulator");
-	cudaStream_t s = (cudaStream_t)cuda_stream;
+	if (rc != RGS_OK || p.P == 0) return rc;
+	if (!acc) return fail(RGS_E_INVALID, missing);
 	RenderGradIn gin{in->dL_dout_color, in->dL_dout_coord, in->dL_dout_mcoord, in->dL_dout_depth, in->dL_dout_mdepth,
 	                 in->dL_dout_alpha, in->dL_dout_normal, in->out_alpha, in->out_normal};
-	{ StageScope sc(ST_RENDER_BWD, s); launch_render_backward(p, g, b, img, gin, grad_accum, s); }
+	{ StageScope sc(ST_RENDER_BWD, s); launch_render_backward(p, g, b, img, gin, acc, s, zero_first); }
 	return debug_sync(cam, s, "backward render");
+}
+
+int32_t rgs_backward_render(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_backward_in* in, float* grad_accum, void* cuda_stream) {
+	FwdParams p;
+	GeomView g;
+	return backward_render(cam, gs, in, grad_accum, "null gradient accumulator", true, (cudaStream_t)cuda_stream, p, g);
 }
 
 int32_t rgs_backward_render_exchange(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_backward_in* in, rgs_exchange* ex, void* cuda_stream) {
 	FwdParams p;
 	GeomView g;
-	BinView b;
-	ImgView img;
-	int rc = backward_views(cam, gs, in, p, g, b, img);
-	if (rc != RGS_OK) return rc;
-	if (p.P == 0) return RGS_OK;
-	float* acc = rgs_exchange_accumulator(ex);
-	if (!acc) return fail(RGS_E_INVALID, "null exchange");
 	cudaStream_t s = (cudaStream_t)cuda_stream;
-	RenderGradIn gin{in->dL_dout_color, in->dL_dout_coord, in->dL_dout_mcoord, in->dL_dout_depth, in->dL_dout_mdepth,
-	                 in->dL_dout_alpha, in->dL_dout_normal, in->out_alpha, in->out_normal};
-	{ StageScope sc(ST_RENDER_BWD, s); launch_render_backward(p, g, b, img, gin, acc, s, /*zero_first=*/false); }
-	if ((rc = debug_sync(cam, s, "backward render")) != RGS_OK) return rc;
+	int rc = backward_render(cam, gs, in, rgs_exchange_accumulator(ex), "null exchange", false, s, p, g);
+	if (rc != RGS_OK || p.P == 0) return rc;
 	{
 		StageScope sc(ST_EXCHANGE, s);
 		rc = rgs_exchange_rows(ex, p.P, g.tiles_touched, in->radii, cuda_stream);
 	}
 	if (rc != RGS_OK) return rc;
 	return debug_sync(cam, s, "gradient exchange");
+}
+
+static ParamGradOut param_grads(const rgs_backward_out* o) {
+	return {o->dL_dmeans2D, o->dL_dcolors, o->dL_dopacity, o->dL_dmeans3D, o->dL_dcov3D, o->dL_dsh, o->dL_dscales, o->dL_drotations, o->dL_dsh_rest};
 }
 
 static int32_t backward_preprocess_impl(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_backward_in* in, const float* grad_accum,
@@ -536,7 +533,7 @@ static int32_t backward_preprocess_impl(const rgs_camera* cam, const rgs_gaussia
 	if (p.P == 0) return RGS_OK;
 	if (!grad_accum || !out) return fail(RGS_E_INVALID, "null gradient accumulator / outputs");
 	cudaStream_t s = (cudaStream_t)cuda_stream;
-	ParamGradOut po{out->dL_dmeans2D, out->dL_dcolors, out->dL_dopacity, out->dL_dmeans3D, out->dL_dcov3D, out->dL_dsh, out->dL_dscales, out->dL_drotations, out->dL_dsh_rest};
+	const ParamGradOut po = param_grads(out);
 	if ((p.shs_rest != nullptr) != (po.d_sh_rest != nullptr) && po.d_sh != nullptr)
 		return fail(RGS_E_INVALID, "dL_dsh_rest must be given exactly when shs_rest is");
 	{ StageScope sc(ST_PREPROCESS_BWD, s); launch_preprocess_backward(p, g, in->radii, grad_accum, po, s, prefilled); }
@@ -585,7 +582,7 @@ int32_t rgs_backward(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_b
 		FwdParams p;
 		int rc0 = make_params(cam, gs, p);
 		if (rc0 != RGS_OK) return rc0;
-		ParamGradOut po{out->dL_dmeans2D, out->dL_dcolors, out->dL_dopacity, out->dL_dmeans3D, out->dL_dcov3D, out->dL_dsh, out->dL_dscales, out->dL_drotations, out->dL_dsh_rest};
+		const ParamGradOut po = param_grads(out);
 		if (cudaEventRecord(ss->fork, s) == cudaSuccess && cudaStreamWaitEvent(ss->stream, ss->fork, 0) == cudaSuccess) {
 			launch_backward_zero_fill(p, po, ss->stream);
 			prefilled = cudaEventRecord(ss->join, ss->stream) == cudaSuccess;

@@ -101,77 +101,10 @@ void check(int64_t rc) {
 }
 
 // The rasterizer has no CPU fallback: refuse host tensors, then run on the device of means3D.
-c10::cuda::CUDAGuard cuda_guard(const torch::Tensor& means3D, const torch::Tensor* points3D = nullptr) {
+c10::Device rasterizer_device(const torch::Tensor& means3D, const torch::Tensor* points3D = nullptr) {
 	TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor: no CPU path");
 	TORCH_CHECK(!points3D || points3D->is_cuda(), "points3D must be a CUDA tensor: no CPU path");
-	return c10::cuda::CUDAGuard(means3D.device());
-}
-
-struct CamHolder {
-	torch::Tensor bg, view, proj, campos;
-	rgs_camera cam;
-};
-
-void fill_camera(CamHolder& h, const torch::Tensor& like, const torch::Tensor& background, const torch::Tensor& viewmatrix,
-                 const torch::Tensor& projmatrix, const torch::Tensor& campos, float tan_fovx, float tan_fovy, float kernel_size,
-                 float scale_modifier, int H, int W, int degree, int M, bool prefiltered, bool require_coord, bool require_depth, bool debug,
-                 int row_begin, int row_end, bool compact = false) {
-	h.bg = as_input(background, like, "background");
-	h.view = as_input(viewmatrix, like, "viewmatrix");
-	h.proj = as_input(projmatrix, like, "projmatrix");
-	h.campos = as_input(campos, like, "campos");
-	rgs_camera& c = h.cam;
-	c.width = W;
-	c.height = H;
-	c.tan_fovx = tan_fovx;
-	c.tan_fovy = tan_fovy;
-	c.kernel_size = kernel_size;
-	c.scale_modifier = scale_modifier;
-	c.viewmatrix = h.view.data_ptr<float>();
-	c.projmatrix = h.proj.data_ptr<float>();
-	c.cam_pos = h.campos.data_ptr<float>();
-	c.background = h.bg.data_ptr<float>();
-	c.sh_degree = degree;
-	c.sh_coeffs = M;
-	c.require_coord = require_coord;
-	c.require_depth = require_depth;
-	c.prefiltered = prefiltered;
-	c.debug = debug;
-	c.tile_row_begin = row_begin;
-	c.tile_row_end = row_end;
-	c.compact_slab = compact ? 1 : 0;
-}
-
-struct GaussHolder {
-	torch::Tensor means, opac, sh, sh_rest, colors, scales, rots, cov;
-	rgs_gaussians g;
-};
-
-void fill_gaussians(GaussHolder& h, const torch::Tensor& means3D, const torch::Tensor& opacity, const torch::Tensor& sh, const torch::Tensor& colors,
-                    const torch::Tensor& scales, const torch::Tensor& rotations, const torch::Tensor& cov3D_precomp,
-                    const torch::Tensor& sh_rest = torch::Tensor()) {
-	h.means = as_input(means3D, means3D, "means3D");
-	h.opac = as_input(opacity, means3D, "opacity");
-	h.sh = as_input(sh, means3D, "sh");
-	h.colors = as_input(colors, means3D, "colors_precomp");
-	h.scales = as_input(scales, means3D, "scales");
-	h.rots = as_input(rotations, means3D, "rotations");
-	h.cov = as_input(cov3D_precomp, means3D, "cov3D_precomp");
-	h.g.P = (int)means3D.size(0);
-	h.g.means3D = opt_ptr(h.means);
-	h.g.opacities = opt_ptr(h.opac);
-	h.g.shs = opt_ptr(h.sh);
-	h.g.colors_precomp = opt_ptr(h.colors);
-	h.g.scales = opt_ptr(h.scales);
-	h.g.rotations = opt_ptr(h.rots);
-	h.g.cov3D_precomp = opt_ptr(h.cov);
-	h.g.shs_rest = nullptr;
-	if (sh_rest.defined() && sh_rest.numel() != 0) {  // split layout: `sh` is [P,1,3], sh_rest [P,M-1,3]
-		TORCH_CHECK(sh.dim() == 3 && sh.size(1) == 1 && sh_rest.dim() == 3 && sh_rest.size(0) == sh.size(0) && sh_rest.size(2) == 3,
-		            "split SH layout needs shs_dc [P,1,3] and shs_rest [P,M-1,3]");
-		h.sh_rest = as_input(sh_rest, means3D, "shs_rest");
-		h.g.shs_rest = h.sh_rest.data_ptr<float>();
-	}
+	return means3D.device();
 }
 
 // number of SH coefficients per Gaussian for either layout
@@ -182,138 +115,176 @@ int sh_coeffs(const torch::Tensor& sh, const torch::Tensor& sh_rest = torch::Ten
 	return M;
 }
 
+// One rasterizer call's camera and Gaussians as the C ABI takes them, built from the reference's arguments, with the tensors behind
+// their pointers.  Building it checks means3D (and integrate's query points) and switches to the device of means3D for the call.
+// With `sh_rest` (split-SH symbols) the SH coefficients come split into `sh` [P,1,3] and `sh_rest` [P,M-1,3].
+struct Frame {
+	c10::cuda::CUDAGuard guard;
+	torch::Tensor bg, view, proj, pos, means, opac, shs, shs_rest, cols, scale, rot, cov;
+	rgs_camera cam;
+	rgs_gaussians g;
+
+	static c10::Device checked_device(const torch::Tensor& means3D, const torch::Tensor* points3D) {
+		if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
+			AT_ERROR("means3D must have dimensions (num_points, 3)");
+		}
+		if (points3D && (points3D->ndimension() != 2 || points3D->size(1) != 3)) {
+			AT_ERROR("points3D must have dimensions (num_points, 3)");
+		}
+		return rasterizer_device(means3D, points3D);
+	}
+
+	Frame(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
+	      const torch::Tensor& scales, const torch::Tensor& rotations, float scale_modifier, const torch::Tensor& cov3D_precomp,
+	      const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, float tan_fovx, float tan_fovy, float kernel_size, int H, int W,
+	      const torch::Tensor& sh, int degree, const torch::Tensor& campos, bool prefiltered, bool require_coord, bool require_depth, bool debug,
+	      int row_begin, int row_end, bool compact, const torch::Tensor& sh_rest = torch::Tensor(), const torch::Tensor* points3D = nullptr)
+	    : guard(checked_device(means3D, points3D)) {
+		bg = as_input(background, means3D, "background");
+		view = as_input(viewmatrix, means3D, "viewmatrix");
+		proj = as_input(projmatrix, means3D, "projmatrix");
+		pos = as_input(campos, means3D, "campos");
+		cam = rgs_camera{W, H, tan_fovx, tan_fovy, kernel_size, scale_modifier, view.data_ptr<float>(), proj.data_ptr<float>(), pos.data_ptr<float>(),
+		                 bg.data_ptr<float>(), degree, sh_coeffs(sh, sh_rest), require_coord, require_depth, prefiltered, debug, row_begin, row_end,
+		                 compact};
+		means = as_input(means3D, means3D, "means3D");
+		opac = as_input(opacity, means3D, "opacity");
+		shs = as_input(sh, means3D, "sh");
+		cols = as_input(colors, means3D, "colors_precomp");
+		scale = as_input(scales, means3D, "scales");
+		rot = as_input(rotations, means3D, "rotations");
+		cov = as_input(cov3D_precomp, means3D, "cov3D_precomp");
+		g = rgs_gaussians{(int)means3D.size(0), opt_ptr(means), opt_ptr(opac), opt_ptr(shs), opt_ptr(cols), opt_ptr(scale), opt_ptr(rot), opt_ptr(cov), nullptr};
+		if (sh_rest.defined() && sh_rest.numel() != 0) {
+			TORCH_CHECK(sh.dim() == 3 && sh.size(1) == 1 && sh_rest.dim() == 3 && sh_rest.size(0) == sh.size(0) && sh_rest.size(2) == 3,
+			            "split SH layout needs shs_dc [P,1,3] and shs_rest [P,M-1,3]");
+			shs_rest = as_input(sh_rest, means3D, "shs_rest");
+			g.shs_rest = shs_rest.data_ptr<float>();
+		}
+	}
+};
+
+// Pixel rows of tile rows [row_begin, row_end) in an H-row image: the height of compact slab maps, as slab_height in rgs_api.cu
+// gives it for compact_slab.
+int compact_rows(int H, int row_begin, int row_end) { return std::max(0, std::min(row_end * 16, H) - row_begin * 16); }
+
+// The seven maps of a forward: [C, H, W], or with `compact` only the slab's pixel rows.  They are zero-filled when nothing is drawn,
+// and so are full-size maps of a slab that is not the whole image, whose rows outside the slab the library does not write.
+struct Maps {
+	torch::TensorOptions opts;
+	int H, W;
+	bool compact;
+	torch::Tensor color, coord, mcoord, alpha, normal, depth, mdepth;
+
+	int height(int row_begin, int row_end) const { return compact ? compact_rows(H, row_begin, row_end) : H; }
+
+	void make(int row_begin, int row_end, bool zero) {  // tile rows [row_begin, row_end); row_end < 0: to the last
+		const int grid_y = (H + 15) / 16;
+		if (row_end < 0) row_end = grid_y;
+		const bool fill = zero || (!compact && !(row_begin == 0 && row_end == grid_y));
+		const int h = height(row_begin, row_end);
+		auto img = [&](int ch) { return fill ? torch::zeros({ch, h, W}, opts) : new_empty({ch, h, W}, opts); };
+		color = img(3), depth = img(1), mdepth = img(1), coord = img(3), mcoord = img(3), alpha = img(1), normal = img(3);
+	}
+
+	void point(rgs_forward_out& out) const {
+		out.out_color = color.data_ptr<float>();
+		out.out_coord = coord.data_ptr<float>();
+		out.out_mcoord = mcoord.data_ptr<float>();
+		out.out_alpha = alpha.data_ptr<float>();
+		out.out_normal = normal.data_ptr<float>();
+		out.out_depth = depth.data_ptr<float>();
+		out.out_mdepth = mdepth.data_ptr<float>();
+	}
+};
+
+// rgs_forward_balanced's maps callback: the maps of the slab the library chose
+int32_t balanced_maps_cb(void* user, int32_t row_begin, int32_t row_end, int32_t height, rgs_forward_out* out) {
+	auto* m = reinterpret_cast<Maps*>(user);
+	if (height != m->height(row_begin, row_end)) return 1;
+	try {
+		m->make(row_begin, row_end, false);
+	} catch (const std::exception&) {
+		return 1;
+	}
+	m->point(*out);
+	return 0;
+}
+
+// A balanced forward's rank of `world_size`, and what it returns beyond the slab's outputs: the partition (world_size + 1 tile-row
+// cuts) and the per-row statistics [2, grid_y] (instances, longest tile list) on the host.
+struct Balance {
+	int world_size, rank;
+	std::vector<int32_t> cuts;
+	torch::Tensor stats;
+};
+
 using FwdResult = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
                              torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
 
+// The forward of tile rows [row_begin, row_end) (the whole image: 0, -1), or with `balance` of the slab the frame's own tile
+// counts give its rank.
 FwdResult forward_impl(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
                        const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
                        const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
                        const float kernel_size, const int image_height, const int image_width, const torch::Tensor& sh, const int degree,
                        const torch::Tensor& campos, const bool prefiltered, const bool require_coord, const bool require_depth, const bool debug,
-                       int row_begin, int row_end, const torch::Tensor& sh_rest = torch::Tensor(), bool compact = false) {
-	if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
-		AT_ERROR("means3D must have dimensions (num_points, 3)");
-	}
-	const auto guard = cuda_guard(means3D);
-	const int P = means3D.size(0);
-	const int H = image_height, W = image_width;
-	auto int_opts = means3D.options().dtype(torch::kInt32);
-	auto float_opts = means3D.options().dtype(torch::kFloat32);
-	const int grid_y = (H + 15) / 16;
-	const bool whole = (row_begin == 0 && (row_end < 0 || row_end == grid_y));
-	// compact: the maps hold the slab's pixel rows only ([ch, Hs, W]) and are fully written by the kernels
-	const int r1 = row_end < 0 ? grid_y : row_end;
-	const int Hm = compact ? std::max(0, std::min(r1 * 16, H) - row_begin * 16) : H;
-	const bool fill = (P == 0) || (!whole && !compact);  // P == 0: the reference returns all-zero maps (rasterize_points.cu:90)
-	auto img = [&](int ch) { return fill ? torch::zeros({ch, Hm, W}, float_opts) : new_empty({ch, Hm, W}, float_opts); };
-	torch::Tensor out_color = img(3), out_depth = img(1), out_mdepth = img(1), out_coord = img(3), out_mcoord = img(3), out_alpha = img(1),
-	              out_normal = img(3);
-	torch::Tensor radii = P == 0 ? torch::zeros({P}, int_opts) : new_empty({P}, int_opts);
+                       int row_begin, int row_end, const torch::Tensor& sh_rest = torch::Tensor(), bool compact = false, Balance* balance = nullptr) {
+	const Frame f(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	              kernel_size, image_height, image_width, sh, degree, campos, prefiltered, require_coord, require_depth, debug, row_begin, row_end, compact,
+	              sh_rest);
+	const int P = f.g.P, H = image_height, W = image_width;
+	Maps m{means3D.options().dtype(torch::kFloat32), H, W, compact};
+	if (!balance) m.make(row_begin, row_end, P == 0);  // P == 0: the reference returns all-zero maps (rasterize_points.cu:90)
+	torch::Tensor radii = P == 0 ? torch::zeros({P}, means3D.options().dtype(torch::kInt32)) : new_empty({P}, means3D.options().dtype(torch::kInt32));
 	torch::Tensor geomBuffer = bytes(means3D), binningBuffer = bytes(means3D), imgBuffer = bytes(means3D);
-
-	int rendered = 0;
-	if (P != 0) {
-		const int M = sh_coeffs(sh, sh_rest);
-		CamHolder ch;
-		fill_camera(ch, means3D, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, kernel_size, scale_modifier, H, W, degree, M,
-		            prefiltered, require_coord, require_depth, debug, row_begin, row_end, compact);
-		GaussHolder gh;
-		fill_gaussians(gh, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp, sh_rest);
-		rgs_forward_out fo{out_color.data_ptr<float>(), out_coord.data_ptr<float>(), out_mcoord.data_ptr<float>(), out_alpha.data_ptr<float>(),
-		                   out_normal.data_ptr<float>(), out_depth.data_ptr<float>(), out_mdepth.data_ptr<float>(), radii.data_ptr<int>()};
-		rgs_buffers bufs{resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer};
-		const int64_t rc = rgs_forward(&ch.cam, &gh.g, &fo, &bufs, at::cuda::getCurrentCUDAStream().stream());
-		check(rc);
-		rendered = (int)rc;
+	rgs_buffers bufs{resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer};
+	rgs_forward_out fo{};
+	fo.radii = radii.data_ptr<int>();
+	const cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
+	int64_t rc = 0;
+	if (!balance) {
+		m.point(fo);
+		if (P != 0) check(rc = rgs_forward(&f.cam, &f.g, &fo, &bufs, stream));
+	} else {
+		const int grid_x = (W + 15) / 16, grid_y = (H + 15) / 16;
+		TORCH_CHECK(balance->world_size > 0 && balance->rank >= 0 && balance->rank < balance->world_size, "rank ", balance->rank, " is not a rank of ",
+		            balance->world_size);
+		TORCH_CHECK(H > 0 && W > 0, "image size must be positive");
+		balance->cuts.resize(balance->world_size + 1);
+		balance->stats = torch::zeros({2, grid_y}, torch::dtype(torch::kInt64));
+		std::vector<uint32_t> row_stats((size_t)2 * grid_y, 0u);
+		if (P == 0) {  // nothing to render: the partition of empty rows and all-zero maps, as rasterize_gaussians_slab returns them
+			check(rgs_balance_partition(grid_y, grid_x, balance->world_size, row_stats.data(), balance->cuts.data()));
+			m.make(balance->cuts[balance->rank], balance->cuts[balance->rank + 1], true);
+		} else {
+			check(rc = rgs_forward_balanced(&f.cam, &f.g, balance->world_size, balance->rank, &fo, balanced_maps_cb, &m, &bufs, balance->cuts.data(),
+			                                row_stats.data(), stream));
+			auto acc = balance->stats.accessor<int64_t, 2>();
+			for (int y = 0; y < grid_y; y++) {
+				acc[0][y] = row_stats[y];
+				acc[1][y] = row_stats[grid_y + y];
+			}
+		}
 	}
-	return std::make_tuple(rendered, out_color, out_coord, out_mcoord, out_alpha, out_normal, out_depth, out_mdepth, radii, geomBuffer,
-	                       binningBuffer, imgBuffer);
+	return std::make_tuple((int)rc, m.color, m.coord, m.mcoord, m.alpha, m.normal, m.depth, m.mdepth, radii, geomBuffer, binningBuffer, imgBuffer);
 }
 
-// ---- balanced row sharding: the slab is cut from the frame's own tile counts (rgs_forward_balanced) ----------------
-
-// the seven maps, allocated once the library has chosen the slab (its rgs_maps_fn)
-struct BalancedMaps {
-	torch::TensorOptions opts;
-	int W, grid_y;
-	bool compact;
-	torch::Tensor color, coord, mcoord, alpha, normal, depth, mdepth;
-
-	void make(int row_begin, int row_end, int height, bool zero) {
-		// full-size maps of a slab that is not the whole image: the rows outside it stay zero, as rasterize_gaussians_slab returns them
-		const bool fill = zero || (!compact && !(row_begin == 0 && row_end == grid_y));
-		auto img = [&](int ch) { return fill ? torch::zeros({ch, height, W}, opts) : new_empty({ch, height, W}, opts); };
-		color = img(3), coord = img(3), mcoord = img(3), alpha = img(1), normal = img(3), depth = img(1), mdepth = img(1);
-	}
-};
-
-int32_t balanced_maps_cb(void* user, int32_t row_begin, int32_t row_end, int32_t height, rgs_forward_out* out) {
-	auto* m = reinterpret_cast<BalancedMaps*>(user);
-	try {
-		m->make(row_begin, row_end, height, false);
-	} catch (const std::exception&) {
-		return 1;
-	}
-	out->out_color = m->color.data_ptr<float>();
-	out->out_coord = m->coord.data_ptr<float>();
-	out->out_mcoord = m->mcoord.data_ptr<float>();
-	out->out_alpha = m->alpha.data_ptr<float>();
-	out->out_normal = m->normal.data_ptr<float>();
-	out->out_depth = m->depth.data_ptr<float>();
-	out->out_mdepth = m->mdepth.data_ptr<float>();
-	return 0;
-}
-
-// rasterize_gaussians_slab's 12-tuple for the slab the frame's tile counts give rank `rank` of `world_size`, then the partition
-// (world_size + 1 tile-row cuts) and the per-row statistics [2, grid_y] (instances, longest tile list) on the host
+// rasterize_gaussians_slab's 12-tuple for the slab the frame's tile counts give rank `rank` of `world_size`, then the partition and
+// the per-row statistics
 py::tuple RasterizeBalanced(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
                             const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
                             const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
                             const float kernel_size, const int image_height, const int image_width, const torch::Tensor& sh, const int degree,
                             const torch::Tensor& campos, const bool prefiltered, const bool require_coord, const bool require_depth, const bool debug,
                             const int world_size, const int rank, const bool compact) {
-	if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
-		AT_ERROR("means3D must have dimensions (num_points, 3)");
-	}
-	const auto guard = cuda_guard(means3D);
-	const int P = means3D.size(0);
-	const int H = image_height, W = image_width;
-	const int grid_x = (W + 15) / 16, grid_y = (H + 15) / 16;
-	TORCH_CHECK(world_size > 0 && rank >= 0 && rank < world_size, "rank ", rank, " is not a rank of ", world_size);
-	TORCH_CHECK(H > 0 && W > 0, "image size must be positive");
-	BalancedMaps m{means3D.options().dtype(torch::kFloat32), W, grid_y, compact};
-	torch::Tensor radii = P == 0 ? torch::zeros({P}, means3D.options().dtype(torch::kInt32)) : new_empty({P}, means3D.options().dtype(torch::kInt32));
-	torch::Tensor geomBuffer = bytes(means3D), binningBuffer = bytes(means3D), imgBuffer = bytes(means3D);
-	std::vector<int32_t> cuts(world_size + 1);
-	torch::Tensor stats = torch::zeros({2, grid_y}, torch::dtype(torch::kInt64));
-	std::vector<uint32_t> row_stats((size_t)2 * grid_y, 0u);
-	int rendered = 0;
-	if (P == 0) {  // nothing to render: the partition of empty rows and all-zero maps, as rasterize_gaussians_slab returns them
-		check(rgs_balance_partition(grid_y, grid_x, world_size, row_stats.data(), cuts.data()));
-		const int r0 = cuts[rank], r1 = cuts[rank + 1];
-		m.make(r0, r1, compact ? std::max(0, std::min(r1 * 16, H) - r0 * 16) : H, true);
-	} else {
-		CamHolder ch;
-		fill_camera(ch, means3D, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, kernel_size, scale_modifier, H, W, degree, sh_coeffs(sh),
-		            prefiltered, require_coord, require_depth, debug, 0, -1, compact);
-		GaussHolder gh;
-		fill_gaussians(gh, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp);
-		rgs_forward_out fo{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, radii.data_ptr<int>()};
-		rgs_buffers bufs{resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer};
-		const int64_t rc = rgs_forward_balanced(&ch.cam, &gh.g, world_size, rank, &fo, balanced_maps_cb, &m, &bufs, cuts.data(), row_stats.data(),
-		                                        at::cuda::getCurrentCUDAStream().stream());
-		check(rc);
-		rendered = (int)rc;
-		auto acc = stats.accessor<int64_t, 2>();
-		for (int y = 0; y < grid_y; y++) {
-			acc[0][y] = row_stats[y];
-			acc[1][y] = row_stats[grid_y + y];
-		}
-	}
-	py::list py_cuts;
-	for (int32_t c : cuts) py_cuts.append(c);
-	return py::make_tuple(rendered, m.color, m.coord, m.mcoord, m.alpha, m.normal, m.depth, m.mdepth, radii, geomBuffer, binningBuffer, imgBuffer, py_cuts,
-	                      stats);
+	Balance b{world_size, rank};
+	const FwdResult out = forward_impl(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+	                                   tan_fovx, tan_fovy, kernel_size, image_height, image_width, sh, degree, campos, prefiltered, require_coord,
+	                                   require_depth, debug, 0, -1, torch::Tensor(), compact, &b);
+	py::list cuts;
+	for (int32_t c : b.cuts) cuts.append(c);
+	return std::apply([&](const auto&... o) { return py::make_tuple(o..., cuts, b.stats); }, out);
 }
 
 // the library's partition of `row_instances` (one count per tile row) over `world_size` ranks: world_size + 1 tile-row cuts
@@ -341,59 +312,46 @@ FwdResult RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::T
 	                    tan_fovy, kernel_size, image_height, image_width, sh, degree, campos, prefiltered, require_coord, require_depth, debug, 0, -1);
 }
 
-struct BackwardCtx {
-	CamHolder ch;
-	GaussHolder gh;
-	torch::Tensor g_color, g_coord, g_mcoord, g_depth, g_mdepth, g_alpha, g_normal, normalmap, alphas, radii, geom, binning, image;
-	rgs_backward_in in;
-};
+// The inputs of the backward stages: the frame and rgs_backward_in.  The whole backward and stage 1 pass `maps`: the upstream
+// gradients of the seven maps (color, coord, mcoord, depth, mdepth, alpha, normal), then the forward's normal and alpha maps.  Their
+// height is read off the colour gradient like the reference does (rasterize_points.cu:171-172), except for compact slab maps, which
+// need the image height.  Stage 2 reads no maps nor the binning and image buffers: it passes no maps and the image size.
+struct Backward {
+	Frame f;
+	torch::Tensor maps[9], radii, geom, binning, image;
+	rgs_backward_in in{};
 
-void fill_backward(BackwardCtx& c, const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii,
-                   const torch::Tensor& colors, const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
-                   const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
-                   const float tan_fovy, const float kernel_size, const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_coord,
-                   const torch::Tensor& dL_dout_mcoord, const torch::Tensor& dL_dout_depth, const torch::Tensor& dL_dout_mdepth,
-                   const torch::Tensor& dL_dout_alpha, const torch::Tensor& dL_dout_normal, const torch::Tensor& normalmap, const torch::Tensor& sh,
-                   const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer,
-                   const torch::Tensor& imageBuffer, const torch::Tensor& alphas, const bool require_coord, const bool require_depth,
-                   const bool debug, int row_begin, int row_end, const torch::Tensor& sh_rest = torch::Tensor(), bool compact = false,
-                   int image_height = -1) {
-	// the image height is read off the gradient map like the reference does (rasterize_points.cu:171-172), except for compact slab maps
-	const int H = (compact && image_height > 0) ? image_height : dL_dout_color.size(1), W = dL_dout_color.size(2);
-	TORCH_CHECK(!compact || image_height > 0, "compact slab maps need the full image height");
-	const int M = sh_coeffs(sh, sh_rest);
-	fill_camera(c.ch, means3D, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, kernel_size, scale_modifier, H, W, degree, M, false,
-	            require_coord, require_depth, debug, row_begin, row_end, compact);
-	torch::Tensor no_opacity = torch::empty({0});  // backward does not receive the opacities (rasterize_points.h:43-76)
-	fill_gaussians(c.gh, means3D, no_opacity, sh, colors, scales, rotations, cov3D_precomp, sh_rest);
-	c.g_color = as_input(dL_dout_color, means3D, "dL_dout_color");
-	c.g_coord = as_input(dL_dout_coord, means3D, "dL_dout_coord");
-	c.g_mcoord = as_input(dL_dout_mcoord, means3D, "dL_dout_mcoord");
-	c.g_depth = as_input(dL_dout_depth, means3D, "dL_dout_depth");
-	c.g_mdepth = as_input(dL_dout_mdepth, means3D, "dL_dout_mdepth");
-	c.g_alpha = as_input(dL_dout_alpha, means3D, "dL_dout_alpha");
-	c.g_normal = as_input(dL_dout_normal, means3D, "dL_dout_normal");
-	c.normalmap = as_input(normalmap, means3D, "normalmap");
-	c.alphas = as_input(alphas, means3D, "alphas");
-	c.radii = radii.contiguous();
-	c.geom = geomBuffer.contiguous();
-	c.binning = binningBuffer.contiguous();
-	c.image = imageBuffer.contiguous();
-	c.in.dL_dout_color = c.g_color.data_ptr<float>();
-	c.in.dL_dout_coord = c.g_coord.data_ptr<float>();
-	c.in.dL_dout_mcoord = c.g_mcoord.data_ptr<float>();
-	c.in.dL_dout_depth = c.g_depth.data_ptr<float>();
-	c.in.dL_dout_mdepth = c.g_mdepth.data_ptr<float>();
-	c.in.dL_dout_alpha = c.g_alpha.data_ptr<float>();
-	c.in.dL_dout_normal = c.g_normal.data_ptr<float>();
-	c.in.out_alpha = c.alphas.data_ptr<float>();
-	c.in.out_normal = c.normalmap.data_ptr<float>();
-	c.in.radii = c.radii.data_ptr<int>();
-	c.in.geom_buffer = reinterpret_cast<const char*>(c.geom.data_ptr());
-	c.in.binning_buffer = reinterpret_cast<const char*>(c.binning.data_ptr());
-	c.in.image_buffer = reinterpret_cast<const char*>(c.image.data_ptr());
-	c.in.num_rendered = R;
-}
+	Backward(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii_, const torch::Tensor& colors,
+	         const torch::Tensor& opacity, const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
+	         const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+	         const float tan_fovy, const float kernel_size, std::initializer_list<torch::Tensor> maps_, const torch::Tensor& sh, const int degree,
+	         const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer,
+	         const torch::Tensor& imageBuffer, const bool require_coord, const bool require_depth, const bool debug, int row_begin, int row_end,
+	         bool compact, int image_height, int image_width, const torch::Tensor& sh_rest = torch::Tensor())
+	    : f(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	        kernel_size, maps_.size() == 0 || (compact && image_height > 0) ? image_height : maps_.begin()[0].size(1),
+	        maps_.size() == 0 ? image_width : maps_.begin()[0].size(2), sh, degree, campos, false, require_coord, require_depth, debug, row_begin,
+	        row_end, compact, sh_rest) {
+		TORCH_CHECK(!compact || image_height > 0, "compact slab maps need the full image height");
+		static const char* const names[9] = {"dL_dout_color", "dL_dout_coord", "dL_dout_mcoord", "dL_dout_depth", "dL_dout_mdepth",
+		                                     "dL_dout_alpha", "dL_dout_normal", "normalmap", "alphas"};
+		const float** ptrs[9] = {&in.dL_dout_color, &in.dL_dout_coord, &in.dL_dout_mcoord, &in.dL_dout_depth, &in.dL_dout_mdepth,
+		                         &in.dL_dout_alpha, &in.dL_dout_normal, &in.out_normal, &in.out_alpha};
+		for (size_t i = 0; i < maps_.size(); i++) {
+			maps[i] = as_input(maps_.begin()[i], means3D, names[i]);
+			*ptrs[i] = maps[i].data_ptr<float>();
+		}
+		radii = radii_.contiguous();
+		geom = geomBuffer.contiguous();
+		binning = binningBuffer.contiguous();
+		image = imageBuffer.contiguous();
+		in.radii = radii.data_ptr<int>();
+		in.geom_buffer = reinterpret_cast<const char*>(geom.data_ptr());
+		in.binning_buffer = reinterpret_cast<const char*>(binning.data_ptr());
+		in.image_buffer = reinterpret_cast<const char*>(image.data_ptr());
+		in.num_rendered = R;
+	}
+};
 
 using BwdResult = std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
 
@@ -436,19 +394,17 @@ GradTensors backward_impl(const torch::Tensor& background, const torch::Tensor& 
                           const torch::Tensor& sh, const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
                           const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const torch::Tensor& alphas, const bool require_coord,
                           const bool require_depth, const bool debug, const torch::Tensor& sh_rest) {
-	const auto guard = cuda_guard(means3D);
+	// backward does not receive the opacities (rasterize_points.h:43-76)
+	const Backward b(background, means3D, radii, colors, torch::empty({0}), scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+	                 tan_fovx, tan_fovy, kernel_size,
+	                 {dL_dout_color, dL_dout_coord, dL_dout_mcoord, dL_dout_depth, dL_dout_mdepth, dL_dout_alpha, dL_dout_normal, normalmap, alphas}, sh,
+	                 degree, campos, geomBuffer, R, binningBuffer, imageBuffer, require_coord, require_depth, debug, 0, -1, false, -1, -1, sh_rest);
 	TORCH_CHECK(!sh_rest.defined() || sh_rest.numel() != 0, "split SH layout needs a non-empty shs_rest");
-	const int P = means3D.size(0);
 	GradTensors gt;
-	alloc_grads(gt, means3D, P, sh_coeffs(sh, sh_rest), sh_rest.defined());
-	if (P != 0) {
-		BackwardCtx c;
-		fill_backward(c, background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx,
-		              tan_fovy, kernel_size, dL_dout_color, dL_dout_coord, dL_dout_mcoord, dL_dout_depth, dL_dout_mdepth, dL_dout_alpha,
-		              dL_dout_normal, normalmap, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, alphas, require_coord, require_depth,
-		              debug, 0, -1, sh_rest);
+	alloc_grads(gt, means3D, b.f.g.P, b.f.cam.sh_coeffs, sh_rest.defined());
+	if (b.f.g.P != 0) {
 		torch::Tensor scratch = bytes(means3D);
-		check(rgs_backward(&c.ch.cam, &c.gh.g, &c.in, &gt.out, resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
+		check(rgs_backward(&b.f.cam, &b.f.g, &b.in, &gt.out, resize_cb, &scratch, at::cuda::getCurrentCUDAStream().stream()));
 	}
 	return gt;
 }
@@ -475,7 +431,7 @@ torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, tor
 	const int P = means3D.size(0);
 	torch::Tensor present = torch::full({P}, false, means3D.options().dtype(at::kBool));
 	if (P != 0) {
-		const auto guard = cuda_guard(means3D);
+		const c10::cuda::CUDAGuard guard(rasterizer_device(means3D));
 		torch::Tensor m = means3D.contiguous(), v = viewmatrix.contiguous(), pr = projmatrix.contiguous();
 		check(rgs_mark_visible(P, m.data_ptr<float>(), v.data_ptr<float>(), pr.data_ptr<float>(), reinterpret_cast<uint8_t*>(present.data_ptr<bool>()),
 		                       at::cuda::getCurrentCUDAStream().stream()));
@@ -493,14 +449,9 @@ IntegrateGaussiansToPointsCUDA(const torch::Tensor& background, const torch::Ten
                                const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy, const float kernel_size,
                                const torch::Tensor& subpixel_offset, const int image_height, const int image_width, const torch::Tensor& sh,
                                const int degree, const torch::Tensor& campos, const bool prefiltered, const bool debug) {
-	if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
-		AT_ERROR("means3D must have dimensions (num_points, 3)");
-	}
-	if (points3D.ndimension() != 2 || points3D.size(1) != 3) {
-		AT_ERROR("points3D must have dimensions (num_points, 3)");
-	}
-	const auto guard = cuda_guard(means3D, &points3D);
-	const int PN = points3D.size(0), P = means3D.size(0), H = image_height, W = image_width;
+	const Frame f(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	              kernel_size, image_height, image_width, sh, degree, campos, prefiltered, false, true, debug, 0, -1, false, torch::Tensor(), &points3D);
+	const int PN = points3D.size(0), P = f.g.P, H = image_height, W = image_width;
 	auto int_opts = means3D.options().dtype(torch::kInt32);
 	auto float_opts = means3D.options().dtype(torch::kFloat32);
 	const bool run = P != 0 && PN != 0;  // rasterize_points.cu:341: otherwise the fill values below are returned
@@ -513,17 +464,12 @@ IntegrateGaussiansToPointsCUDA(const torch::Tensor& background, const torch::Ten
 	torch::Tensor geomBuffer = bytes(means3D), binningBuffer = bytes(means3D), imgBuffer = bytes(means3D), pointBuffer = bytes(means3D);
 	int rendered = 0;
 	if (run) {
-		CamHolder ch;
-		fill_camera(ch, means3D, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, kernel_size, scale_modifier, H, W, degree,
-		            sh_coeffs(sh), prefiltered, false, true, debug, 0, -1);
-		GaussHolder gh;
-		fill_gaussians(gh, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp);
 		torch::Tensor pts = as_input(points3D, means3D, "points3D");
 		rgs_integrate_io io{PN, pts.data_ptr<float>(), out_color.data_ptr<float>(), out_alpha_integrated.data_ptr<float>(),
 		                    out_color_integrated.data_ptr<float>(), out_coordinate2d.data_ptr<float>(), out_sdf.data_ptr<float>(), radii.data_ptr<int>()};
 		rgs_buffers bufs{resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer};
 		int32_t overflowed = 0;
-		const int64_t rc = rgs_integrate(&ch.cam, &gh.g, &io, &bufs, resize_cb, &pointBuffer, &overflowed,  // always read: 4 bytes on a call that synchronises anyway
+		const int64_t rc = rgs_integrate(&f.cam, &f.g, &io, &bufs, resize_cb, &pointBuffer, &overflowed,  // always read: 4 bytes on a call that synchronises anyway
 		                                 at::cuda::getCurrentCUDAStream().stream());
 		check(rc);
 		rendered = (int)rc;
@@ -548,19 +494,18 @@ torch::Tensor backward_render_impl(rgs_exchange* ex, const torch::Tensor& backgr
                                    const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer,
                                    const torch::Tensor& imageBuffer, const torch::Tensor& alphas, const bool require_coord, const bool require_depth,
                                    const bool debug, const int tile_row_begin, const int tile_row_end, const bool compact, const int image_height) {
-	const auto guard = cuda_guard(means3D);
-	const int P = means3D.size(0);
+	const Backward b(background, means3D, radii, colors, torch::empty({0}), scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+	                 tan_fovx, tan_fovy, kernel_size,
+	                 {dL_dout_color, dL_dout_coord, dL_dout_mcoord, dL_dout_depth, dL_dout_mdepth, dL_dout_alpha, dL_dout_normal, normalmap, alphas}, sh,
+	                 degree, campos, geomBuffer, R, binningBuffer, imageBuffer, require_coord, require_depth, debug, tile_row_begin, tile_row_end,
+	                 compact, image_height, -1);
+	const int P = b.f.g.P;
 	const int GS = rgs_grad_stride(require_coord, require_depth);
 	torch::Tensor acc = ex ? torch::Tensor() : P == 0 ? torch::zeros({P, GS}, means3D.options()) : new_empty({P, GS}, means3D.options());
 	if (P != 0) {
-		BackwardCtx c;
-		fill_backward(c, background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx,
-		              tan_fovy, kernel_size, dL_dout_color, dL_dout_coord, dL_dout_mcoord, dL_dout_depth, dL_dout_mdepth, dL_dout_alpha,
-		              dL_dout_normal, normalmap, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, alphas, require_coord, require_depth,
-		              debug, tile_row_begin, tile_row_end, torch::Tensor(), compact, image_height);
 		const cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
-		check(ex ? rgs_backward_render_exchange(&c.ch.cam, &c.gh.g, &c.in, ex, stream)
-		         : rgs_backward_render(&c.ch.cam, &c.gh.g, &c.in, acc.data_ptr<float>(), stream));
+		check(ex ? rgs_backward_render_exchange(&b.f.cam, &b.f.g, &b.in, ex, stream)
+		         : rgs_backward_render(&b.f.cam, &b.f.g, &b.in, acc.data_ptr<float>(), stream));
 	}
 	return ex ? torch::from_blob(const_cast<float*>(rgs_exchange_result(ex)), {P, GS}, means3D.options().dtype(torch::kFloat32)) : acc;
 }
@@ -624,6 +569,7 @@ int ExchangeStatus(const int64_t ex) {
 
 void ExchangeDestroy(const int64_t ex) { rgs_exchange_destroy(reinterpret_cast<rgs_exchange*>(ex)); }
 
+
 // stage 2: accumulator (after the cross-rank sum) -> the reference's 8-tuple of parameter gradients
 BwdResult BackwardPreprocessCUDA(const torch::Tensor& grad_accum, const torch::Tensor& background, const torch::Tensor& means3D,
                                  const torch::Tensor& radii, const torch::Tensor& colors, const torch::Tensor& opacity, const torch::Tensor& scales,
@@ -632,26 +578,14 @@ BwdResult BackwardPreprocessCUDA(const torch::Tensor& grad_accum, const torch::T
                                  const float kernel_size, const int image_height, const int image_width, const torch::Tensor& sh, const int degree,
                                  const torch::Tensor& campos, const torch::Tensor& geomBuffer, const bool require_coord, const bool require_depth,
                                  const bool debug) {
-	const auto guard = cuda_guard(means3D);
-	const int P = means3D.size(0);
-	const int M = sh_coeffs(sh);
+	const Backward b(background, means3D, radii, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx,
+	                 tan_fovy, kernel_size, {}, sh, degree, campos, geomBuffer, 0, geomBuffer, geomBuffer, require_coord, require_depth, debug, 0, -1,
+	                 false, image_height, image_width);
 	GradTensors gt;
-	alloc_grads(gt, means3D, P, M);
-	if (P != 0) {
-		CamHolder ch;
-		fill_camera(ch, means3D, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, kernel_size, scale_modifier, image_height,
-		            image_width, degree, M, false, require_coord, require_depth, debug, 0, -1);
-		GaussHolder gh;
-		fill_gaussians(gh, means3D, opacity, sh, colors, scales, rotations, cov3D_precomp);
+	alloc_grads(gt, means3D, b.f.g.P, b.f.cam.sh_coeffs);
+	if (b.f.g.P != 0) {
 		torch::Tensor acc = as_input(grad_accum, means3D, "grad_accum");
-		torch::Tensor geom = geomBuffer.contiguous(), rad = radii.contiguous();
-		rgs_backward_in in;
-		memset(&in, 0, sizeof(in));
-		in.radii = rad.data_ptr<int>();
-		in.geom_buffer = reinterpret_cast<const char*>(geom.data_ptr());
-		in.image_buffer = in.geom_buffer;    // not read by stage 2
-		in.binning_buffer = in.geom_buffer;  // not read by stage 2
-		check(rgs_backward_preprocess(&ch.cam, &gh.g, &in, acc.data_ptr<float>(), &gt.out, at::cuda::getCurrentCUDAStream().stream()));
+		check(rgs_backward_preprocess(&b.f.cam, &b.f.g, &b.in, acc.data_ptr<float>(), &gt.out, at::cuda::getCurrentCUDAStream().stream()));
 	}
 	return gt.reference_tuple();
 }

@@ -24,6 +24,7 @@ from typing import NamedTuple
 
 import torch
 import torch.nn as nn
+from rade_gs_b200.rawapi import backward_args, forward_args
 
 try:
     from . import _C
@@ -72,27 +73,6 @@ def _call_with_dump(fn, args, debug: bool, dump_name: str, what: str):
         raise
 
 
-def _forward_args(s: GaussianRasterizationSettings, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh, sh_rest=None):
-    # order of RasterizeGaussiansCUDA (reference: rasterize_points.h:18-41); the split-SH symbol takes `sh_rest` after `sh`
-    return (
-        s.bg, means3D, colors_precomp, opacities, scales, rotations, s.scale_modifier, cov3Ds_precomp,
-        s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.kernel_size, s.image_height, s.image_width,
-        *((sh,) if sh_rest is None else (sh, sh_rest)), s.sh_degree, s.campos, s.prefiltered, s.require_coord, s.require_depth, s.debug,
-    )
-
-
-def _backward_args(s: GaussianRasterizationSettings, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp, grads, normal, sh,
-                   geom_buf, num_rendered, binning_buf, img_buf, alpha, sh_rest=None):
-    # order of RasterizeGaussiansBackwardCUDA (reference: rasterize_points.h:43-76); `grads` are the gradients of the maps in the
-    # order color, coord, mcoord, depth, mdepth, alpha, normal; the split-SH symbol takes `sh_rest` after `sh`
-    return (
-        s.bg, means3D, radii, colors_precomp, scales, rotations, s.scale_modifier, cov3Ds_precomp,
-        s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.kernel_size, *grads, normal,
-        *((sh,) if sh_rest is None else (sh, sh_rest)), s.sh_degree, s.campos, geom_buf, num_rendered, binning_buf, img_buf, alpha,
-        s.require_coord, s.require_depth, s.debug,
-    )
-
-
 class _RasterizeGaussians(torch.autograd.Function):
     """The reference's autograd function, plus one input: a non-empty ``sh_rest`` keeps the SH coefficients in the model's two
     tensors (``sh`` = ``_features_dc`` [P,1,3], ``sh_rest`` = ``_features_rest`` [P,M-1,3]; reference
@@ -103,7 +83,7 @@ class _RasterizeGaussians(torch.autograd.Function):
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, sh_rest):
         s = raster_settings
         rest = sh_rest if sh_rest.numel() else None
-        args = _forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh, rest)
+        args = forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh, rest)
         fn = _C.rasterize_gaussians if rest is None else _C.rasterize_gaussians_split_sh
         (num_rendered, color, coord, mcoord, alpha, normal, depth, mdepth, radii,
          geom_buf, binning_buf, img_buf) = _call_with_dump(fn, args, s.debug, "snapshot_fw.dump", "forward")
@@ -119,9 +99,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, normal, radii, sh,
          geom_buf, binning_buf, img_buf, alpha, sh_rest) = ctx.saved_tensors
         rest = sh_rest if sh_rest.numel() else None
-        args = _backward_args(s, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp,
-                              (grad_color, grad_coord, grad_mcoord, grad_depth, grad_mdepth, grad_alpha, grad_normal), normal, sh,
-                              geom_buf, ctx.num_rendered, binning_buf, img_buf, alpha, rest)
+        args = backward_args(s, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp,
+                             (grad_color, grad_coord, grad_mcoord, grad_depth, grad_mdepth, grad_alpha, grad_normal), normal, sh,
+                             geom_buf, ctx.num_rendered, binning_buf, img_buf, alpha, rest)
         fn = _C.rasterize_gaussians_backward if rest is None else _C.rasterize_gaussians_backward_split_sh
         # the split-SH symbol returns the gradient of sh_rest after that of sh
         (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, *g_sh_rest, g_scales, g_rotations) = _call_with_dump(

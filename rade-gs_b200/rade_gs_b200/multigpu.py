@@ -20,6 +20,8 @@ from typing import List, Sequence, Tuple
 import torch
 import torch.distributed as dist
 
+from .rawapi import backward_args, forward_args, preprocess_args
+
 TILE = 16
 
 
@@ -198,9 +200,9 @@ class _ShardedRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, slab, group, exchange=None,
                 compact=False, balance=None):
-        from diff_gaussian_rasterization import _C, _forward_args
+        from diff_gaussian_rasterization import _C
         s = raster_settings
-        args = _forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh)
+        args = forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh)
         if balance is not None:   # (rank, world_size, plan): the slab is cut from this frame's tile counts and reported in `plan`
             rank, world_size, plan = balance
             out = _C._slab.rasterize_balanced(*args, world_size, rank, compact)
@@ -217,23 +219,17 @@ class _ShardedRasterize(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_color, g_radii, g_coord, g_mcoord, g_depth, g_mdepth, g_alpha, g_normal):
-        from diff_gaussian_rasterization import _C, _backward_args, _forward_args
+        from diff_gaussian_rasterization import _C
         s = ctx.s
         colors_precomp, means3D, scales, rotations, cov3Ds_precomp, normal, radii, sh, geom, binning, img, alpha, opacities = ctx.saved_tensors
-        stage1_args = _backward_args(s, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp,
-                                     (g_color, g_coord, g_mcoord, g_depth, g_mdepth, g_alpha, g_normal), normal, sh, geom, ctx.num_rendered,
-                                     binning, img, alpha) + (*ctx.slab, ctx.compact, s.image_height)
-
-        def stage2(acc):
-            # backward-preprocess takes the forward's arguments with the accumulator first, the radii after means3D and the
-            # geometry buffer in place of `prefiltered`
-            f = _forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh)
-            return _C.rasterize_gaussians_backward_preprocess(acc, *f[:2], radii, *f[2:18], geom, *f[19:])
-
+        stage1_args = backward_args(s, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp,
+                                    (g_color, g_coord, g_mcoord, g_depth, g_mdepth, g_alpha, g_normal), normal, sh, geom, ctx.num_rendered,
+                                    binning, img, alpha) + (*ctx.slab, ctx.compact, s.image_height)
         # the device-side exchange (or its dense fallback) owned by the caller, else one all-reduce
         acc = (ctx.exchange.backward_render(_C, *stage1_args) if ctx.exchange is not None
                else allreduce_sum_(_C.rasterize_gaussians_backward_render(*stage1_args), ctx.group))
-        g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot = stage2(acc)
+        g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_sh, g_scales, g_rot = _C.rasterize_gaussians_backward_preprocess(
+            *preprocess_args(s, acc, means3D, radii, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh, geom))
         return g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, None, None, None, None, None, None
 
 

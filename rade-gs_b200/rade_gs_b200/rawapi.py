@@ -4,35 +4,63 @@ Both modules export the reference's `rasterize_gaussians` / `rasterize_gaussians
 (reference: rasterize_points.h:18-76), so the same two functions drive either one -- this is what the parity
 tests and `bench.py` time (SURVEY.md 8d: t_fwd = `_C.rasterize_gaussians`, t_bwd = `_C.rasterize_gaussians_backward`).
 This build's extras -- the tile-row slab forward and the two stages of the multi-GPU backward -- are driven the same way
-(`forward(..., tile_rows=...)`, `backward_render`, `backward_preprocess`).
+(`forward(..., tile_rows=...)`, `backward_render`, `backward_preprocess`).  `forward_args`, `backward_args` and `preprocess_args`
+spell each call's argument order once, for these helpers and the autograd wrappers; this module imports no extension.
 """
 from __future__ import annotations
+
+from types import SimpleNamespace
 
 import torch
 
 FWD_KEYS = ("num_rendered", "color", "coord", "mcoord", "alpha", "normal", "depth", "mdepth", "radii", "geom", "binning", "img")
 BWD_KEYS = ("means2D", "colors", "opacity", "means3D", "cov3D", "sh", "scales", "rotations")
+_CALL_SETTINGS = ("kernel_size", "scale_modifier", "sh_degree", "require_coord", "require_depth", "debug")
 
 
 def _absent():
     return torch.Tensor([])
 
 
+def forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3D_precomp, sh, sh_rest=None) -> tuple:
+    """The forward's arguments in the order of RasterizeGaussiansCUDA (reference: rasterize_points.h:18-41), from raster settings
+    `s` (the fields of `GaussianRasterizationSettings`) and the Gaussians.  The split-SH symbol takes `sh_rest` after `sh`."""
+    return (s.bg, means3D, colors_precomp, opacities, scales, rotations, s.scale_modifier, cov3D_precomp,
+            s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.kernel_size, s.image_height, s.image_width,
+            *((sh,) if sh_rest is None else (sh, sh_rest)), s.sh_degree, s.campos, s.prefiltered, s.require_coord, s.require_depth, s.debug)
+
+
+def backward_args(s, means3D, radii, colors_precomp, scales, rotations, cov3D_precomp, grads, normal, sh, geom, num_rendered, binning, img,
+                  alpha, sh_rest=None) -> tuple:
+    """The backward's arguments in the order of RasterizeGaussiansBackwardCUDA (reference: rasterize_points.h:43-76); `grads` are the
+    gradients of the maps color, coord, mcoord, depth, mdepth, alpha, normal.  The split-SH symbol takes `sh_rest` after `sh`."""
+    return (s.bg, means3D, radii, colors_precomp, scales, rotations, s.scale_modifier, cov3D_precomp,
+            s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.kernel_size, *grads, normal,
+            *((sh,) if sh_rest is None else (sh, sh_rest)), s.sh_degree, s.campos, geom, num_rendered, binning, img, alpha,
+            s.require_coord, s.require_depth, s.debug)
+
+
+def preprocess_args(s, acc, means3D, radii, colors_precomp, opacities, scales, rotations, cov3D_precomp, sh, geom) -> tuple:
+    """The arguments of stage 2 (`rasterize_gaussians_backward_preprocess`) for the summed accumulator rows `acc`."""
+    return (acc, s.bg, means3D, radii, colors_precomp, opacities, scales, rotations, s.scale_modifier, cov3D_precomp,
+            s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, s.kernel_size, s.image_height, s.image_width, sh, s.sh_degree, s.campos,
+            geom, s.require_coord, s.require_depth, s.debug)
+
+
+def _settings(sc, c: dict) -> SimpleNamespace:  # the raster settings of call `c` on scene `sc`
+    return SimpleNamespace(image_height=sc.height, image_width=sc.width, tanfovx=sc.tanfovx, tanfovy=sc.tanfovy, bg=sc.bg, viewmatrix=sc.viewmatrix,
+                           projmatrix=sc.projmatrix, campos=sc.campos, prefiltered=False, **{k: c[k] for k in _CALL_SETTINGS})
+
+
 def _forward_args(sc, c: dict) -> tuple:
-    # order of RasterizeGaussiansCUDA (reference: rasterize_points.h:18-41)
-    return (sc.bg, sc.means3D, c["cols"], sc.opacities, c["scales"], c["rots"], c["scale_modifier"], c["cov"],
-            sc.viewmatrix, sc.projmatrix, sc.tanfovx, sc.tanfovy, c["kernel_size"], sc.height, sc.width,
-            c["shs"], c["sh_degree"], sc.campos, False, c["require_coord"], c["require_depth"], c["debug"])
+    return forward_args(_settings(sc, c), sc.means3D, c["cols"], sc.opacities, c["scales"], c["rots"], c["cov"], c["shs"])
 
 
 def _backward_args(sc, fwd: dict, grads: dict) -> tuple:
-    # order of RasterizeGaussiansBackwardCUDA (reference: rasterize_points.h:43-76)
     c = fwd["_call"]
-    return (sc.bg, sc.means3D, fwd["radii"], c["cols"], c["scales"], c["rots"], c["scale_modifier"], c["cov"],
-            sc.viewmatrix, sc.projmatrix, sc.tanfovx, sc.tanfovy, c["kernel_size"],
-            grads["color"], grads["coord"], grads["mcoord"], grads["depth"], grads["mdepth"], grads["alpha"],
-            grads["normal"], fwd["normal"], c["shs"], c["sh_degree"], sc.campos, fwd["geom"], fwd["num_rendered"],
-            fwd["binning"], fwd["img"], fwd["alpha"], c["require_coord"], c["require_depth"], c["debug"])
+    return backward_args(_settings(sc, c), sc.means3D, fwd["radii"], c["cols"], c["scales"], c["rots"], c["cov"],
+                         [grads[k] for k in ("color", "coord", "mcoord", "depth", "mdepth", "alpha", "normal")], fwd["normal"], c["shs"],
+                         fwd["geom"], fwd["num_rendered"], fwd["binning"], fwd["img"], fwd["alpha"])
 
 
 def forward(C, sc, require_coord: bool, require_depth: bool, kernel_size: float = 0.0, sh_degree: int = 3,
@@ -68,9 +96,9 @@ def backward_render(C, sc, fwd: dict, grads: dict) -> torch.Tensor:
 
 def backward_preprocess(C, sc, fwd: dict, acc: torch.Tensor) -> dict:
     """Stage 2: the (summed) accumulator rows -> the parameter gradients of `backward`."""
-    f = _forward_args(sc, fwd["_call"])
-    # the forward's arguments with the accumulator first, the radii after means3D and the geometry buffer in place of `prefiltered`
-    return dict(zip(BWD_KEYS, C.rasterize_gaussians_backward_preprocess(acc, *f[:2], fwd["radii"], *f[2:18], fwd["geom"], *f[19:])))
+    c = fwd["_call"]
+    args = preprocess_args(_settings(sc, c), acc, sc.means3D, fwd["radii"], c["cols"], sc.opacities, c["scales"], c["rots"], c["cov"], c["shs"], fwd["geom"])
+    return dict(zip(BWD_KEYS, C.rasterize_gaussians_backward_preprocess(*args)))
 
 
 # ---- views into the private buffers (parity tests only) ----------------------------------------------------------
