@@ -84,7 +84,8 @@ struct BinView {
 	uint32_t* point_list;          // [R] sorted Gaussian ids
 	uint64_t* keys_sorted;         // [R]
 	uint32_t* hitmask;             // [(R/32 + tiles + 1) * 8] per 32-instance chunk: one ballot word per 8x4 pixel block of the tile,
-	                               // written by forward-render (which splats can reach alpha >= 1/255 in the block), read by backward
+	                               // written by forward-render (which splats can reach alpha >= 1/255 in the 8x8 block holding it; both
+	                               // halves of a block carry the same word), read by backward
 	uint64_t* keys_unsorted;       // [R] local keys (depth bits << 32 | Gaussian index) of the tile sort
 };
 

@@ -4,9 +4,6 @@
 
 namespace rgs {
 
-constexpr int BATCH = 256;     // splats staged per round (one per thread)
-constexpr int NTHREADS = 256;  // 8 warps, one 8x4 pixel block each
-
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
 	const uint32_t dst = (uint32_t)__cvta_generic_to_shared(smem_dst);
 	asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(dst), "l"(gmem_src));

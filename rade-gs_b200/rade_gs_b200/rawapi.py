@@ -136,8 +136,9 @@ def ours_views(fwd: dict, sc) -> dict:
     b = _Cursor(fwd["binning"])
     point_list = b.take(R, torch.int32, 4)
     keys = b.take(R, torch.int64, 8)
-    # forward-render's ballots: word (chunk_base[tile] + k) * 8 + warp holds, for list positions [32k, 32k + 32) of the tile, the
-    # entries that warp's 8x4 pixel block did not cull (warp w covers tile columns 8 (w & 1) .. +7, rows 4 (w >> 1) .. +3)
+    # forward-render's ballots: word (chunk_base[tile] + k) * 8 + s holds, for list positions [32k, 32k + 32) of the tile, the
+    # entries the box test kept for the 8x8 pixel block holding 8x4 half s (half s covers tile columns 8 (s & 1) .. +7, rows
+    # 4 (s >> 1) .. +3); the two halves of a block, s and s + 2 with s & 2 == 0, hold the same word
     hitmask = b.take((R // 32 + tiles + 1) * 8, torch.int32, 4)
     i = _Cursor(fwd["img"])
     ranges = i.take(tiles * 2, torch.int32, 4).view(tiles, 2)

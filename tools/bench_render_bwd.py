@@ -3,9 +3,11 @@ walks, for the two pixel-block layouts the kernel can give a warp.
 
 A warp of the backward blend walks the tile list from the back and runs its per-hit body for every list entry whose bit is
 set in the hit mask forward-render stored for its pixel block, up to the last contributor of any pixel of the block.  The
-forward stores one ballot word per 32 list entries per 8x4 block.  Counted from the buffers one forward leaves:
-  8x4   one warp per 8x4 block (32 pixels, one per lane): the block's own word, cut at the block's max(n_contrib);
+forward stores one ballot word per 32 list entries per 8x4 half-block: the ballot of the 8x8 block holding it (a build whose
+forward warps own 8x4 blocks stores each half's own ballot).  Counted from the buffers one forward leaves:
+  8x4   one warp per 8x4 block (32 pixels, one per lane): the half's word, cut at the half's max(n_contrib);
   8x8   one warp per 8x8 block (64 pixels, two per lane): the OR of the words of its two 8x4 halves, cut at the 64-pixel max.
+With the 8x8 forward the 8x4 count uses 8x8 ballots, so it is not what an 8x4 backward walked after an 8x4 forward.
 Each counted pair moves its 16-float gradient row through the warp's shared-memory transpose: every lane stores 64 B and the
 flush reads them back, 4 KB per pair in either layout, so per pixel-hit the 8x8 layout moves half the bytes.
 
