@@ -111,6 +111,26 @@ typedef struct rgs_buffers {
 int64_t rgs_forward(const rgs_camera* cam, const rgs_gaussians* g, const rgs_forward_out* out,
                     const rgs_buffers* bufs, void* cuda_stream);
 
+/* ---- rgs_forward without the host read, for CUDA-graph capture (DESIGN.md §9 item 3) ----
+ * The binning buffer and the per-tile sort are sized from the caller's capacities instead of the frame's instance count and
+ * longest tile list, so the call makes no device-to-host copy, no synchronisation and no host allocation (buffers grow only
+ * through the resize callbacks).  Same kernels as rgs_forward; for a frame that fits, the maps, radii, sorted ids and keys are
+ * bit-identical to rgs_forward's.  Returns preset->instances: the num_rendered to give the backward (it fixes the binning
+ * layout).  `status` is DEVICE memory, 4 words, accumulated over calls until the caller clears it:
+ *   [0] overflow bits OR-ed in (1: the frame has more instances than `instances`, 2: a longer tile list than `longest_list`),
+ *   [1] the largest instance count seen, [2] the longest tile list seen, [3] reserved.
+ * A frame that overflows writes nothing outside the carved buffers: its maps are the background and its radii as computed;
+ * the caller discards the result and calls again with larger capacities.  Whole image only: a tile-row slab, compact_slab,
+ * debug (it synchronises) and prefiltered are rejected.  The first call on a device must be made outside stream capture (it
+ * opts the sort kernels in to their shared memory). */
+typedef struct rgs_preset {
+	int64_t instances;      /* the binning buffer is carved for this many instances                          */
+	int32_t longest_list;   /* tile-sort shared memory / long-list passes are sized for this list length     */
+	uint32_t* status;       /* DEVICE, 4 words (above)                                                        */
+} rgs_preset;
+int64_t rgs_forward_preset(const rgs_camera* cam, const rgs_gaussians* g, const rgs_forward_out* out,
+                           const rgs_buffers* bufs, const rgs_preset* preset, void* cuda_stream);
+
 /* ---- balanced row sharding: each frame's slabs cut from that frame's instance counts (DESIGN.md "Multi-GPU") ----
  * Partition rule, integer-only, the same on every rank because preprocess and the tile counts are:
  *   - I_y = instances (splat-tile pairs) in tile row y, over the whole image; grid_x tiles per row;

@@ -34,9 +34,15 @@ static double g_stage_ms[ST_COUNT];
 static int64_t g_stage_n[ST_COUNT];
 static std::atomic<int> g_stage_on{0};
 
+static bool capturing(cudaStream_t s) {
+	cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+	return cudaStreamIsCapturing(s, &st) == cudaSuccess && st != cudaStreamCaptureStatusNone;
+}
+
+// Records nothing while the stream is being captured into a CUDA graph: the events would be graph nodes, read back never.
 struct StageScope {
 	cudaStream_t s; int stage; cudaEvent_t a = nullptr, b = nullptr; bool on;
-	StageScope(int st, cudaStream_t stream) : s(stream), stage(st), on(g_stage_on.load() != 0) {
+	StageScope(int st, cudaStream_t stream) : s(stream), stage(st), on(g_stage_on.load() != 0 && !capturing(stream)) {
 		if (on) { cudaEventCreate(&a); cudaEventCreate(&b); cudaEventRecord(a, s); }
 	}
 	~StageScope() {
@@ -272,9 +278,9 @@ static int preprocess_and_scan(const rgs_camera* cam, const FwdParams& p, int* r
 	return RGS_OK;
 }
 
-// binning buffer for R instances -> scatter and per-tile sort of p's tile rows
+// binning buffer for R instances -> scatter and per-tile sort of p's tile rows (with preset_status: R and max_list are capacities)
 static int64_t bin_tiles(const rgs_camera* cam, const FwdParams& p, int* radii, const rgs_buffers* bufs, cudaStream_t s, GeomView g, BinView& b,
-                         ImgView img, int64_t R, uint32_t max_list) {
+                         ImgView img, int64_t R, uint32_t max_list, uint32_t* preset_status = nullptr) {
 	int rc;
 	const int P = p.P;
 	const int tiles = p.grid_x * p.grid_y;
@@ -293,7 +299,7 @@ static int64_t bin_tiles(const rgs_camera* cam, const FwdParams& p, int* radii, 
 	} else {
 		// lists longer than the shared-memory sort take the multi-CTA path inside launch_tile_binning
 		StageScope sc(ST_BINNING, s);
-		launch_tile_binning(p, g, b, img, radii, R, max_list, s);
+		launch_tile_binning(p, g, b, img, radii, R, max_list, s, preset_status);
 	}
 	if ((rc = debug_sync(cam, s, "binning")) != RGS_OK) return rc;
 	return R;
@@ -333,6 +339,43 @@ int64_t rgs_forward(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_fo
 	BinView b;
 	ImgView img;
 	const int64_t R = forward_to_binning(cam, p, out->radii, bufs, s, g, b, img);
+	if (R < 0) return R;
+	RenderOut ro{out->out_color, out->out_coord, out->out_mcoord, out->out_alpha, out->out_normal, out->out_depth, out->out_mdepth};
+	{ StageScope sc(ST_RENDER_FWD, s); launch_render_forward(p, g, b, img, ro, s); }
+	if ((rc = debug_sync(cam, s, "render")) != RGS_OK) return rc;
+	return R;
+}
+
+// The sort kernels' shared-memory opt-in, once per device: rgs_forward_preset does it outside stream capture and refuses a capture on
+// a device that has not had it.
+static bool g_graph_ready[64];
+
+int64_t rgs_forward_preset(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_forward_out* out, const rgs_buffers* bufs, const rgs_preset* preset,
+                           void* cuda_stream) {
+	FwdParams p;
+	int rc = make_params(cam, gs, p);
+	if (rc != RGS_OK) return rc;
+	if (!out || !bufs || !bufs->geom || !bufs->binning || !bufs->image) return fail(RGS_E_INVALID, "null outputs / buffer callbacks");
+	if (!preset || !preset->status) return fail(RGS_E_INVALID, "rgs_forward_preset: null preset / status");
+	if (preset->instances < 0 || preset->longest_list < 0) return fail(RGS_E_INVALID, "rgs_forward_preset: negative capacity");
+	if (cam->debug) return fail(RGS_E_UNSUPPORTED, "rgs_forward_preset: debug mode synchronizes after every stage; use rgs_forward");
+	if (cam->tile_row_begin != 0 || cam->tile_row_end != -1 || cam->compact_slab)
+		return fail(RGS_E_UNSUPPORTED, "rgs_forward_preset renders the whole image only: no tile-row slab, no compact_slab");
+	cudaStream_t s = (cudaStream_t)cuda_stream;
+	int dev = 0;
+	RGS_CUDA_TRY(cudaGetDevice(&dev));
+	if (!capturing(s)) {
+		prepare_tile_binning();
+		g_graph_ready[dev & 63] = true;
+	} else if (!g_graph_ready[dev & 63]) {
+		return fail(RGS_E_INVALID, "rgs_forward_preset: make one call outside stream capture on this device first (one-time set-up)");
+	}
+	GeomView g;
+	BinView b;
+	ImgView img;
+	if ((rc = carve_img_buffer(p, bufs, img)) != RGS_OK || (rc = carve_geom_buffer(p, bufs, g)) != RGS_OK) return rc;
+	if (p.P > 0 && (rc = preprocess_and_scan(cam, p, out->radii, g, img, s)) != RGS_OK) return rc;
+	const int64_t R = bin_tiles(cam, p, out->radii, bufs, s, g, b, img, preset->instances, (uint32_t)preset->longest_list, p.P > 0 ? preset->status : nullptr);
 	if (R < 0) return R;
 	RenderOut ro{out->out_color, out->out_coord, out->out_mcoord, out->out_alpha, out->out_normal, out->out_depth, out->out_mdepth};
 	{ StageScope sc(ST_RENDER_FWD, s); launch_render_forward(p, g, b, img, ro, s); }
@@ -550,12 +593,14 @@ struct SideStream {
 	cudaStream_t stream = nullptr;
 	cudaEvent_t fork = nullptr, join = nullptr;
 };
-static SideStream* side_stream() {
+// for work ordered after `s`.  Not created while `s` is being captured (none: the caller runs the work on `s`).
+static SideStream* side_stream(cudaStream_t s) {
 	static thread_local SideStream per_dev[64];
 	int dev = 0;
 	if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
 	SideStream& ss = per_dev[dev & 63];
 	if (!ss.stream) {
+		if (capturing(s)) return nullptr;
 		if (cudaStreamCreateWithFlags(&ss.stream, cudaStreamNonBlocking) != cudaSuccess) return nullptr;
 		if (cudaEventCreateWithFlags(&ss.fork, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ss.join, cudaEventDisableTiming) != cudaSuccess)
 			return nullptr;
@@ -577,7 +622,7 @@ int32_t rgs_backward(const rgs_camera* cam, const rgs_gaussians* gs, const rgs_b
 	// The zero-fill of the dense gradient tensors (pure HBM writes, ~280 MB at 1 M Gaussians) runs on a side stream underneath the
 	// issue-bound backward blend; everything queued on `s` before this call is ordered before it (the tensors may be recycled memory).
 	bool prefilled = false;
-	SideStream* ss = !cam->debug ? side_stream() : nullptr;
+	SideStream* ss = !cam->debug ? side_stream(s) : nullptr;
 	if (ss) {
 		FwdParams p;
 		int rc0 = make_params(cam, gs, p);

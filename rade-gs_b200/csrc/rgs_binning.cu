@@ -135,6 +135,27 @@ void launch_tile_scan(const FwdParams& p, ImgView img, cudaStream_t s) {
 	count_launch();
 }
 
+// ---- preset binning (rgs_forward_preset): the buffers and the sort are sized from the caller's capacities, not from the totals
+// the scan just wrote, so that no host read is needed.  Overflow bits of a frame that does not fit: 1 instances, 2 longest list.
+__device__ __forceinline__ uint32_t preset_overflow(const uint32_t* totals, uint32_t cap_instances, uint32_t cap_list) {
+	return (totals[0] > cap_instances ? 1u : 0u) | (totals[1] > cap_list ? 2u : 0u);
+}
+
+// Records the frame's totals in the caller's status words (overflow bits OR-ed, instances and longest list max-ed) and, when the
+// frame does not fit, empties every tile range: the sort and blend kernels then leave the maps at the background, and the
+// scatter returns on the same test, so nothing is written past the carved binning buffer.
+__global__ void __launch_bounds__(256) preset_guard_kernel(int tiles, const uint32_t* __restrict__ totals, uint32_t cap_instances, uint32_t cap_list,
+                                                           uint2* __restrict__ ranges, uint32_t* __restrict__ status) {
+	const uint32_t over = preset_overflow(totals, cap_instances, cap_list);
+	const int t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t == 0) {
+		if (over) atomicOr(status, over);
+		atomicMax(status + 1, totals[0]);
+		atomicMax(status + 2, totals[1]);
+	}
+	if (over && t < tiles) ranges[t] = make_uint2(0u, 0u);
+}
+
 // Scatter: every instance takes a slot inside its tile's segment and stores its 64-bit local key.
 // A warp owns 32 consecutive Gaussians and emits them COOPERATIVELY: the tiles of one splat are spread over the lanes
 // (lane k takes the k-th tile of the rectangle), four splats are in flight per round so that the returning atomics
@@ -143,7 +164,9 @@ void launch_tile_scan(const FwdParams& p, ImgView img, cudaStream_t s) {
 __global__ void __launch_bounds__(256) scatter_kernel(int P, const float* __restrict__ records, int rec_f, const float* __restrict__ depths,
                                                        const uint32_t* __restrict__ tiles_touched, const int* __restrict__ radii, int grid_x, int grid_y,
                                                        int row_begin, int row_end, const uint2* __restrict__ ranges, uint32_t* __restrict__ tile_count,
-                                                       uint64_t* __restrict__ local_keys) {
+                                                       uint64_t* __restrict__ local_keys, const uint32_t* __restrict__ totals, uint32_t cap_instances,
+                                                       uint32_t cap_list) {
+	if (totals && preset_overflow(totals, cap_instances, cap_list)) return;  // preset binning too small: write nothing (preset_guard_kernel)
 	const int lane = threadIdx.x & 31;
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	int cnt = 0, x0 = 0, y0 = 0, w = 1;
@@ -387,25 +410,44 @@ __global__ void __launch_bounds__(LONG_THREADS) long_finalize_kernel(const uint2
 	}
 }
 
-void launch_tile_binning(const FwdParams& p, GeomView g, BinView b, ImgView img, const int* radii, int64_t R, uint32_t max_list, cudaStream_t s) {
-	if (R <= 0 || p.row_end <= p.row_begin) return;
+static size_t g_sort_smem[64] = {}, g_long_smem[64] = {};
+constexpr size_t TILE_SORT_SMEM = (size_t)2 * (TILE_SORT_CAP + (TILE_SORT_CAP >> 4)) * sizeof(uint64_t);
+constexpr size_t LONG_SORT_SMEM = (size_t)2 * (LONG_CHUNK + (LONG_CHUNK >> 4)) * sizeof(uint64_t);
+
+void prepare_tile_binning() {
+	ensure_dynamic_smem(tile_sort_kernel, TILE_SORT_SMEM, g_sort_smem);
+	ensure_dynamic_smem(long_chunk_sort_kernel, LONG_SORT_SMEM, g_long_smem);
+}
+
+void launch_tile_binning(const FwdParams& p, GeomView g, BinView b, ImgView img, const int* radii, int64_t R, uint32_t max_list, cudaStream_t s,
+                         uint32_t* preset_status) {
+	if (p.row_end <= p.row_begin) return;
+	const uint32_t* totals = nullptr;
+	uint32_t cap_instances = 0, cap_list = 0;
+	if (preset_status) {
+		const int tiles = p.grid_x * p.grid_y;
+		totals = img.totals;
+		cap_instances = R > (int64_t)UINT32_MAX ? UINT32_MAX : (uint32_t)R;
+		cap_list = max_list;
+		preset_guard_kernel<<<(tiles + 255) / 256, 256, 0, s>>>(tiles, totals, cap_instances, cap_list, img.ranges, preset_status);
+		count_launch();
+	}
+	if (R <= 0) return;
 	scatter_kernel<<<(p.P + 255) / 256, 256, 0, s>>>(p.P, g.records, rec_floats(p.coord), g.depths, g.tiles_touched, radii, p.grid_x, p.grid_y,
-	                                                  p.row_begin, p.row_end, img.ranges, img.tile_count, b.keys_unsorted);
+	                                                  p.row_begin, p.row_end, img.ranges, img.tile_count, b.keys_unsorted, totals, cap_instances,
+	                                                  cap_list);
 	const int longest_short = (int)min(max_list, (uint32_t)TILE_SORT_CAP);
 	const int cap = (max(longest_short, 256) + 255) & ~255;  // keys per ping-pong buffer
 	const size_t smem = (size_t)2 * (cap + (cap >> 4)) * sizeof(uint64_t);
-	static size_t configured[64] = {};
-	if (smem > 48 * 1024) ensure_dynamic_smem(tile_sort_kernel, (size_t)2 * (TILE_SORT_CAP + (TILE_SORT_CAP >> 4)) * sizeof(uint64_t), configured);
+	if (smem > 48 * 1024) ensure_dynamic_smem(tile_sort_kernel, TILE_SORT_SMEM, g_sort_smem);
 	dim3 grid(p.grid_x, p.row_end - p.row_begin, 1);
 	tile_sort_kernel<<<grid, SORT_THREADS, smem, s>>>(img.ranges, p.grid_x, p.row_begin, b.keys_unsorted, b.point_list, b.keys_sorted, cap);
 	count_launch(2);
 	if (max_list > (uint32_t)TILE_SORT_CAP) {
 		const int chunks = (int)((max_list + LONG_CHUNK - 1) / LONG_CHUNK);
 		dim3 lgrid(p.grid_x, p.row_end - p.row_begin, chunks);
-		const size_t lsmem = (size_t)2 * (LONG_CHUNK + (LONG_CHUNK >> 4)) * sizeof(uint64_t);
-		static size_t lconfigured[64] = {};
-		ensure_dynamic_smem(long_chunk_sort_kernel, lsmem, lconfigured);
-		long_chunk_sort_kernel<<<lgrid, LONG_THREADS, lsmem, s>>>(img.ranges, p.grid_x, p.row_begin, TILE_SORT_CAP, b.keys_unsorted);
+		ensure_dynamic_smem(long_chunk_sort_kernel, LONG_SORT_SMEM, g_long_smem);
+		long_chunk_sort_kernel<<<lgrid, LONG_THREADS, LONG_SORT_SMEM, s>>>(img.ranges, p.grid_x, p.row_begin, TILE_SORT_CAP, b.keys_unsorted);
 		uint64_t* src = b.keys_unsorted;
 		uint64_t* dst = b.keys_sorted;
 		int launches = 2;

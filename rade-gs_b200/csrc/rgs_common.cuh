@@ -262,7 +262,12 @@ void launch_mark_visible(int P, const float* means3D, const float* viewmatrix, u
 // tile-bucket binning: per-tile counts -> ranges/totals -> scatter -> per-tile shared-memory sort
 constexpr int TILE_SORT_CAP = 8192;   // longest tile list the one-CTA shared-memory sort takes (2 x 64 KB ping-pong); longer lists: multi-CTA chunk sort + merge
 void launch_tile_scan(const FwdParams& p, ImgView img, cudaStream_t s);
-void launch_tile_binning(const FwdParams& p, GeomView g, BinView b, ImgView img, const int* radii, int64_t R, uint32_t max_list, cudaStream_t s);
+// With preset_status (rgs_forward_preset), R and max_list are the caller's capacities: a guard kernel records the frame's totals in
+// the four status words and empties the tile ranges of a frame that does not fit, and the scatter then writes nothing.
+void launch_tile_binning(const FwdParams& p, GeomView g, BinView b, ImgView img, const int* radii, int64_t R, uint32_t max_list, cudaStream_t s,
+                         uint32_t* preset_status = nullptr);
+// the sort kernels' dynamic shared memory opted in to its largest size on the current device (once per device; not under capture)
+void prepare_tile_binning();
 
 // balanced row sharding (rgs_balance.cu): per-row instances / longest list / 32-instance chunks of a whole-image scan, then
 // that scan's state (`whole`) restricted to one slab, written into the slab's image buffer (`img`)

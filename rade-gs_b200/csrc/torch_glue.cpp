@@ -223,13 +223,15 @@ using FwdResult = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, t
                              torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
 
 // The forward of tile rows [row_begin, row_end) (the whole image: 0, -1), or with `balance` of the slab the frame's own tile
-// counts give its rank.
+// counts give its rank, or with `preset` of the whole image binned into the preset's capacities (rgs_forward_preset; num_rendered
+// is then preset->instances).
 FwdResult forward_impl(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
                        const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
                        const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
                        const float kernel_size, const int image_height, const int image_width, const torch::Tensor& sh, const int degree,
                        const torch::Tensor& campos, const bool prefiltered, const bool require_coord, const bool require_depth, const bool debug,
-                       int row_begin, int row_end, const torch::Tensor& sh_rest = torch::Tensor(), bool compact = false, Balance* balance = nullptr) {
+                       int row_begin, int row_end, const torch::Tensor& sh_rest = torch::Tensor(), bool compact = false, Balance* balance = nullptr,
+                       const rgs_preset* preset = nullptr) {
 	const Frame f(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
 	              kernel_size, image_height, image_width, sh, degree, campos, prefiltered, require_coord, require_depth, debug, row_begin, row_end, compact,
 	              sh_rest);
@@ -245,7 +247,9 @@ FwdResult forward_impl(const torch::Tensor& background, const torch::Tensor& mea
 	int64_t rc = 0;
 	if (!balance) {
 		m.point(fo);
-		if (P != 0) check(rc = rgs_forward(&f.cam, &f.g, &fo, &bufs, stream));
+		if (preset) rc = P != 0 ? rgs_forward_preset(&f.cam, &f.g, &fo, &bufs, preset, stream) : preset->instances;
+		else if (P != 0) rc = rgs_forward(&f.cam, &f.g, &fo, &bufs, stream);
+		check(rc);
 	} else {
 		const int grid_x = (W + 15) / 16, grid_y = (H + 15) / 16;
 		TORCH_CHECK(balance->world_size > 0 && balance->rank >= 0 && balance->rank < balance->world_size, "rank ", balance->rank, " is not a rank of ",
@@ -297,6 +301,24 @@ std::vector<int32_t> BalancePartition(const std::vector<int64_t>& row_instances,
 	std::vector<int32_t> cuts(std::max(world_size, 0) + 1);
 	check(rgs_balance_partition((int32_t)rows.size(), grid_x, world_size, rows.data(), cuts.data()));
 	return cuts;
+}
+
+// `_graph.rasterize_gaussians`: rasterize_gaussians (split SH when sh_rest is not empty) binned into the capacities `instances` and
+// `longest_list`, with no host read, so that it can be captured in a CUDA graph.  `status` int32 [4] on the device of means3D is
+// accumulated in place (rgs_preset in include/rgs_b200.h).
+FwdResult RasterizePreset(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
+                          const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
+                          const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                          const float kernel_size, const int image_height, const int image_width, const torch::Tensor& sh, const int degree,
+                          const torch::Tensor& campos, const bool prefiltered, const bool require_coord, const bool require_depth, const bool debug,
+                          const torch::Tensor& sh_rest, const int64_t instances, const int64_t longest_list, const torch::Tensor& status) {
+	TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor: no CPU path");
+	const torch::Tensor st = arg(status, "status", torch::kInt32, {4}, "[4]", &means3D, REJECT);
+	TORCH_CHECK(instances >= 0 && longest_list >= 0 && longest_list <= INT32_MAX, "instances and longest_list must be non-negative (longest_list < 2^31)");
+	const rgs_preset preset{instances, (int32_t)longest_list, reinterpret_cast<uint32_t*>(st.data_ptr<int32_t>())};
+	return forward_impl(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	                    kernel_size, image_height, image_width, sh, degree, campos, prefiltered, require_coord, require_depth, debug, 0, -1, sh_rest, false,
+	                    nullptr, &preset);
 }
 
 // ---- the reference's four symbols ------------------------------------------------------------------------------
@@ -1921,6 +1943,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 	       py::arg("row_hi"), py::arg("up4"), py::arg("w2"), py::arg("b2"), py::arg("w3"), py::arg("b3"));
 	sl.def("appearance_l1_backward_rows", &AppearanceL1BackwardRows, py::arg("image"), py::arg("gt"), py::arg("image_lo"), py::arg("H0"), py::arg("row_lo"),
 	       py::arg("row_hi"), py::arg("up4"), py::arg("act"), py::arg("w2"), py::arg("b2"), py::arg("w3"), py::arg("b3"), py::arg("upstream"));
+	// the forward without a host read, for CUDA-graph capture: a private submodule behind diff_gaussian_rasterization's reserve path
+	py::module_ gr = m.def_submodule("_graph", "rasterizer forward binned into preset capacities behind rade_gs_b200.graphs");
+	gr.def("rasterize_gaussians", &RasterizePreset, py::arg("background"), py::arg("means3D"), py::arg("colors"), py::arg("opacity"), py::arg("scales"),
+	       py::arg("rotations"), py::arg("scale_modifier"), py::arg("cov3D_precomp"), py::arg("viewmatrix"), py::arg("projmatrix"), py::arg("tan_fovx"),
+	       py::arg("tan_fovy"), py::arg("kernel_size"), py::arg("image_height"), py::arg("image_width"), py::arg("sh"), py::arg("degree"), py::arg("campos"),
+	       py::arg("prefiltered"), py::arg("require_coord"), py::arg("require_depth"), py::arg("debug"), py::arg("sh_rest"), py::arg("instances"),
+	       py::arg("longest_list"), py::arg("status"));
 	// the decoupled-appearance network's head: a private submodule behind rade_gs_b200.appearance and multigpu
 	py::module_ ah = m.def_submodule("_appearance_head", "conv1 and up1..up4 of the appearance network behind rade_gs_b200.appearance");
 	ah.def("forward", &AppearanceHeadForward, py::arg("down"), py::arg("emb"), py::arg("params"));

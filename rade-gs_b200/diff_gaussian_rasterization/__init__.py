@@ -80,13 +80,18 @@ class _RasterizeGaussians(torch.autograd.Function):
     ``shs=(features_dc, features_rest)`` to ``GaussianRasterizer.forward``."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, sh_rest):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, sh_rest,
+                reserve=None):
         s = raster_settings
         rest = sh_rest if sh_rest.numel() else None
-        args = forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh, rest)
-        fn = _C.rasterize_gaussians if rest is None else _C.rasterize_gaussians_split_sh
-        (num_rendered, color, coord, mcoord, alpha, normal, depth, mdepth, radii,
-         geom_buf, binning_buf, img_buf) = _call_with_dump(fn, args, s.debug, "snapshot_fw.dump", "forward")
+        if reserve is None:
+            args = forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh, rest)
+            fn = _C.rasterize_gaussians if rest is None else _C.rasterize_gaussians_split_sh
+            out = _call_with_dump(fn, args, s.debug, "snapshot_fw.dump", "forward")
+        else:
+            out = _forward_into_reserve(forward_args(s, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh) + (sh_rest,),
+                                        reserve)
+        (num_rendered, color, coord, mcoord, alpha, normal, depth, mdepth, radii, geom_buf, binning_buf, img_buf) = out
         ctx.raster_settings = s
         ctx.num_rendered = num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, normal, radii, sh,
@@ -106,7 +111,25 @@ class _RasterizeGaussians(torch.autograd.Function):
         # the split-SH symbol returns the gradient of sh_rest after that of sh
         (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, *g_sh_rest, g_scales, g_rotations) = _call_with_dump(
             fn, args, s.debug, "snapshot_bw.dump", "backward")
-        return g_means3D, g_means2D, g_sh, g_colors, g_opacities, g_scales, g_rotations, g_cov3D, None, (g_sh_rest[0] if g_sh_rest else None)
+        return (g_means3D, g_means2D, g_sh, g_colors, g_opacities, g_scales, g_rotations, g_cov3D, None, (g_sh_rest[0] if g_sh_rest else None),
+                None)
+
+
+def _forward_into_reserve(args, reserve):
+    """The forward binned into `reserve`'s capacities (`_C._graph`, no host read).  Under stream capture: the call only; the caller
+    reads the reserve's status after the step.  Eagerly: the status is read at once, and a frame that did not fit grows the
+    reserve and runs again."""
+    def call():
+        return _C._graph.rasterize_gaussians(*args, reserve.instances, reserve.longest_list, reserve.status)
+
+    if torch.cuda.is_current_stream_capturing():
+        return call()
+    reserve.clear()
+    out = call()
+    if reserve.overflowed():
+        reserve.clear()
+        out = call()
+    return out
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
@@ -131,9 +154,14 @@ def _inputs(shs, colors_precomp, scales, rotations, cov3D_precomp):
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings: GaussianRasterizationSettings):
+    """``reserve`` (extension, a ``rade_gs_b200.graphs.BinningReserve``): bin every forward into the reserve's capacities without
+    reading the frame's instance count on the host, so that the call can be captured in a CUDA graph (``rade_gs_b200.graphs``).
+    Whole image only; not with ``debug``."""
+
+    def __init__(self, raster_settings: GaussianRasterizationSettings, reserve=None):
         super().__init__()
         self.raster_settings = raster_settings
+        self.reserve = reserve
 
     def markVisible(self, positions):
         """Boolean mask of the points in front of the near plane (reference :193-202)."""
@@ -149,7 +177,7 @@ class GaussianRasterizer(nn.Module):
                 raise ValueError("split SH layout: shs must be the pair (features_dc, features_rest)")
             shs, sh_rest = shs  # a degree-0 model's empty features_rest takes the reference path
         return _RasterizeGaussians.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, self.raster_settings,
-                                         sh_rest)
+                                         sh_rest, self.reserve)
 
     def integrate(self, points3D, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                   cov3D_precomp=None, view2gaussian_precomp=None):
